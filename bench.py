@@ -1,12 +1,16 @@
-"""bench.py — samples/sec of the DLRM-Criteo train step (BASELINE.json metric) on N B200s of one node.
+"""bench.py — samples/sec of the DLRM-Criteo train step (BASELINE.json metric) on N H100s of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path over one synthetic Criteo batch: KJT scan -> (bucketize + all-to-all at
 N>1) -> pooled gather -> DLRM dot interaction + dense towers -> BCE loss -> backward with the fused sparse
 Adagrad update -> dense Adam step.  fp32 everywhere (TF32 off, as the reference's default train.proto:14).
 Workload at N=1: BASELINE.json configs[1] (examples/dlrm_criteo.config, full hash sizes, row-wise, B=65536
-per rank) — it fits one GPU (12.2 GiB tables + 12.2 GiB Adagrad state).
+per rank) — it fits one 80 GB GPU (12.2 GiB tables + 12.2 GiB Adagrad state).
+
+--dump-outputs DIR: after the timed steps, what the last one computed (loss, dense parameters, a fixed seeded sample of
+embedding rows and their optimizer state) as DIR/<name>.npy; the inputs depend only on the arguments, so two builds
+can be compared output for output.
 
 N>1 (torchrun): tables sharded --sharding {row_wise,table_wise,mixed}, exchange over peer memory (default) or NCCL;
 the line then carries `verify` (the sharded step against its unsharded twin, run inside this process) and an NVLink
@@ -41,26 +45,9 @@ METRIC = "samples/sec (DLRM-Criteo synth, train step fwd+bwd+optimizer)"
 UNIT = "samples/s"
 # DLRM-Criteo (F=26, L=1, D=16) per-sample algorithmic bytes, SURVEY.md §8d — computed from the layout at run time:
 #   gather 1664 rows + 1664 pooled write + 208 ids + 104 lengths = 3640 B; backward 1664 grad + 26*4*64 RMW + 208 = 8528 B
-NVLINK_GBS = 900.0     # NVLink 5, per direction per GPU (nominal; B200_PROFILING.md) — the N>1 roofline's denominator
-
-
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the fused backward's / the gather's kernels, as
-    written by scripts/ncu_traffic.py from an `ncu --set full` capture of THIS build (the file carries a hash of the
-    kernel sources it was taken on; a stale file is ignored)."""
-    import hashlib
-
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if not os.path.exists(path):
-        return None
-    try:
-        d = json.load(open(path))
-        h = hashlib.sha256()
-        for fn in ("tzk_bwd.cu", "tzk_gather.cu", "tzk_common.cuh"):
-            h.update(open(os.path.join(ROOT, "torcheasyrec_b200", "csrc", fn), "rb").read())
-        return d if d.get("source_sha16") == h.hexdigest()[:16] else None
-    except Exception:
-        return None
+NVLINK_GBS = 450.0     # NVLink 4 of the H100 SXM, per direction per GPU (data sheet) — the N>1 roofline's denominator
+HBM_GBS = 3350.0       # HBM3 of the H100 SXM (data sheet) — the N=1 roofline's denominator
+DUMP_BUDGET = 64 << 20  # --dump-outputs writes at most this many bytes
 
 
 def parse_args():
@@ -95,11 +82,13 @@ def parse_args():
                     help="N>1: skip the in-process parity check of the sharded step against its unsharded twin")
     ap.add_argument("--force-sharded", action="store_true",
                     help="N=1 only: still go through bucketize / all-to-all / owner gather (1-rank process group)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps: what the last one computed, as DIR/<name>.npy (float32, <= 64 MB)")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -136,10 +125,7 @@ class ClockSampler:
 
 
 def measured_peak_gbs():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return HBM_GBS, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
 def dist_env():
@@ -157,8 +143,7 @@ def cpu_step_rate(model: str, batch: int, steps: int, warmup: int, max_rows: int
     from torcheasyrec_b200 import functional as Fn
     from torcheasyrec_b200.engine import Pipeline
 
-    # thread scan on a 128-core host (scripts/cpu_threads.py, profiles/README.md): 8 -> 237k, 16 -> 307k,
-    # 32 -> 313k, 64 -> 271k, 128 -> 31k samples/s; beyond 32 the two OpenMP pools fight each other
+    # beyond 32 threads the two OpenMP pools (torch, oracle) fight each other (scripts/cpu_threads.py scans it)
     cores = min(os.cpu_count() or 1, 32)
     torch.set_num_threads(cores)
     os.environ["OMP_NUM_THREADS"] = str(cores)
@@ -179,7 +164,7 @@ def run_reference(args):
     """The reference's CPU path of the same step (`kind: "port"`: tzrec's own path needs the torchrec / fbgemm wheels,
     which cannot be installed offline — DESIGN.md §7): this repo's Pipeline / model shells stepped with the oracle
     (oracle/tzk_oracle.c, OpenMP) as the sparse backend and torch-CPU dense towers, on all the host threads that help
-    (capped at 32: measured scan in profiles/README.md).  Honours --steps / --warmup; every step is a bounded sample of
+    (capped at 32, see cpu_step_rate).  Honours --steps / --warmup; every step is a bounded sample of
     --cpu-batch samples of the workload (a 65536-sample step takes ~0.25 s on 32 threads)."""
     rank, _, world = dist_env()
     if rank != 0:
@@ -371,12 +356,15 @@ def run_ours(args):
     clocks = ClockSampler(local_rank).start() if rank == 0 else None
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    loss = None
     for i in range(K):
         step.load(ring[i % len(ring)])
-        step.replay()
+        loss = step.replay()
     e1.record()
     barrier()
     ms_total = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pipe, loss, sharded)
     # ---- e2e: pinned host batch -> H2D -> step -> loss back on the host, every step --------------------------
     # The H2D of batch i+1 runs on the copy stream while step i computes (graphed steps); the loss of EVERY step
     # reaches the host inside the timed region through a pinned D2H copy + event, read one step later so that the
@@ -518,13 +506,6 @@ def run_ours(args):
     dominant = ("tzk_fused_bwd (id half: linearize + radix sort + run lists; gradient half: fused_apply_kernel over the short-run list + long-run chunks)" if bwd_ms > fwd_ms
                 else "pooled_gather_fwd_kernel")
     ach = bwd_gbs if bwd_ms > fwd_ms else fwd_gbs
-    # dram__bytes_read.sum + dram__bytes_write.sum per launch, all kernels of the dominant op, from the ncu --set full
-    # capture scripts/ncu_traffic.py took on this build (profiles/ncu_traffic.json; null when absent or stale)
-    std = (args.model == "dlrm_criteo" and B == 65536 and not args.max_rows and args.id_dist == "uniform")
-    nt = ncu_traffic() if std else None
-    traffic = None
-    if nt:
-        traffic = nt.get("fused_bwd_bytes") if bwd_ms > fwd_ms else nt.get("pooled_gather_fwd_bytes")
     kernels = {
         "pooled_gather_fwd": {"ms": fwd_ms, "algorithmic_GBps": fwd_gbs, "frac": fwd_gbs / peak,
                               "row_read_GBps": row_b * B / (fwd_ms * 1e-3) / 1e9, "bytes_per_sample": gather_b},
@@ -555,11 +536,8 @@ def run_ours(args):
                                        "frac": ib_b * B / (ib_ms * 1e-3) / 1e9 / peak, "bytes_per_sample": ib_b}
     roofline = {
         "bound": "hbm", "kernel": dominant, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-        "traffic": traffic,
-        "traffic_note": (f"dram read+write bytes per launch summed over the kernels of the dominant op "
-                         f"({', '.join(nt.get('kernels', []))}), ncu --set full via scripts/ncu_traffic.py "
-                         f"({nt.get('when', '?')})" if traffic else
-                         "null: no profiles/ncu_traffic.json taken on this build (scripts/ncu_traffic.py writes it)"),
+        "traffic": None,
+        "traffic_note": "not measured: achieved is algorithmic bytes over CUDA-event kernel time",
         "peak_source": peak_src,
         "kernels": kernels,
         "share_of_step": {k: v["ms"] / (ms_total / K) for k, v in kernels.items()},
@@ -583,6 +561,37 @@ def run_ours(args):
             extras["e2e_blocking"] = {"failed": repr(e)[:200]}
         args._extras = extras
     _emit(args, world, B, K, W, ms_total, ms_e2e, host, last, launches_per_step, clk, roofline, cpu, len(ring))
+
+
+def dump_outputs(out_dir, pipe, loss, sharded):
+    """What the last timed step computed, as <out_dir>/<name>.npy (float32): the loss, every dense parameter and — for
+    unsharded tables — the same seeded sample of rows of every table with their optimizer state."""
+    import numpy as np
+
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().reshape(1)}
+    dense = {id(p) for p in pipe.model.dense_parameters()}
+    arrays.update({"dense." + n: p.detach() for n, p in pipe.model.named_parameters() if id(p) in dense})
+    if not sharded:
+        for c, coll in enumerate(pipe.model.sparse_collections()):
+            for t in range(len(coll._configs)):
+                if t not in coll._table_off:
+                    continue
+                w = coll.table_weight(t)
+                g = torch.Generator().manual_seed(1000 * c + t)
+                rows = torch.randint(0, w.shape[0], (min(4096, w.shape[0]),), generator=g).to(w.device)
+                arrays[f"emb{c}.table{t}.rows"] = w[rows]
+                st = coll.table_state(t)
+                if st is not None:
+                    arrays[f"emb{c}.table{t}.state"] = st[rows]
+    total = 0
+    for name, a in arrays.items():
+        a = a.float().cpu().numpy()
+        total += a.nbytes
+        if total > DUMP_BUDGET:
+            raise RuntimeError(f"--dump-outputs: more than {DUMP_BUDGET >> 20} MB at {name}")
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def _peer_roofline(pipe, kern, ring, B, world, iters, step_ms):
@@ -609,7 +618,7 @@ def _peer_roofline(pipe, kern, ring, B, world, iters, step_ms):
     ach = nvl / (ms * 1e-3) / 1e9
     return {"bound": "nvlink", "kernel": "peer_pooled_gather_fwd_kernel (requester-side gather over peer memory)",
             "achieved": ach, "peak": NVLINK_GBS, "unit": "GB/s", "frac": ach / NVLINK_GBS, "traffic": None,
-            "peak_source": "nominal NVLink 5 per direction per GPU (B200_PROFILING.md)",
+            "peak_source": "data sheet NVLink 4 per direction per GPU (H100 SXM)",
             "ms": ms, "nvlink_bytes_per_launch": nvl, "row_bytes_per_launch": row_bytes,
             "share_of_step": ms / step_ms,
             "note": "algorithmic inbound NVLink bytes = embedding-row bytes x (W-1)/W (uniform ids; 64-B reads); "
@@ -666,7 +675,7 @@ def _emit(args, world, B, K, W, ms_total, ms_e2e, host, last, launches_per_step,
                    "global_batch": global_batch,
                    "parallelism": (f"{ {'row_wise': 'rw', 'table_wise': 'tw', 'mixed': 'tw+rw'}[args.sharding] }{world}+dp{world}"
                                    if sharded else "1 gpu"),
-                   "l2": f"inputs rotate over {ring_len} distinct batches; tables + optimizer state >> 126 MB L2",
+                   "l2": f"inputs rotate over {ring_len} distinct batches; tables + optimizer state >> 50 MB L2",
                    "cuda_graph": bool(mode == "graph"),
                    "exchange": exch},
         "e2e": {"value": global_batch * K / (ms_e2e * 1e-3), "unit": UNIT, "h2d_bytes_per_step": h2d,

@@ -1,10 +1,10 @@
 /*
- * tzk.h — C-ABI of the B200-native sparse-embedding + feature-interaction engine.
+ * tzk.h — C-ABI of the H100-native sparse-embedding + feature-interaction engine.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Every entry point replaces one operator that the
  * reference reaches through third-party wheels (torchrec 1.7.0 / fbgemm-gpu 1.7.0, pinned in
- * /root/reference/requirements/runtime.txt:5,25) or plain ATen; the call site inside the reference is
- * cited on each declaration (paths relative to /root/reference).
+ * requirements/runtime.txt:5,25 of the reference) or plain ATen; the call site inside the reference is
+ * cited on each declaration (paths relative to the reference checkout (alibaba/TorchEasyRec @ 54cac316)).
  *
  * Conventions
  *  - extern "C", plain pointers and sizes, no torch types.  All pointers are DEVICE pointers unless the

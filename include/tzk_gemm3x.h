@@ -1,23 +1,19 @@
 /* tzk_gemm3x.h — C-ABI of libtzk_gemm3x.so (torcheasyrec_b200/csrc/tzk_gemm3x.cu): the one wide tower layer of the
  * rank models (tzrec/modules/mlp.py:20-84 Perceptron; DLRM's final MLP input, tzrec/models/dlrm.py:113-131, 783 wide,
- * travelling as [B, 784]) on hand-written sm_100a tensor-core kernels: tcgen05.mma kind::tf32 with the 3xTF32 split
- * (fp32-level accuracy), TMA-fed, accumulators in TMEM.  Replaces the three library GEMMs of that layer
- * (forward, input gradient, weight gradient).  Plain pointers and sizes; caller-owned memory and stream; returns 0 or
- * 1 bad argument / 2 tensor-map encoding failed / 3 launch failure.  Rows must be 16-B aligned (ld % 4 == 0).
+ * travelling as [B, 784]) on hand-written sm_90a tensor-core kernels: mma.sync m16n8k8 TF32 with the 3xTF32 split
+ * (fp32-level accuracy), TMA-fed through mbarrier-guarded shared-memory stages.  Replaces the three library GEMMs of
+ * that layer (forward, input gradient, weight gradient).  Plain pointers and sizes; caller-owned memory and stream;
+ * returns 0 or 1 bad argument / 2 tensor-map encoding failed / 3 launch failure.  Rows must be 16-B aligned
+ * (ld % 4 == 0).
  *
  *   tzk_gemm3x   y[M,N] = act(x[M,K] @ w[N,K]^T + bias)   N = 64 (forward, K = 784; bias / relu optional) or a
  *                multiple of 112 (input gradient: x = dZ [M,64], w = W^T [784,64]).  K columns beyond the tensor read
  *                as zeros up to the next multiple of 32.  w_hi / w_lo: [N, ld_w] scratch (the TF32 split of w).
- *                TZK_GEMM3X_STACK=1 selects the two-MMA-per-k-step variant, TZK_GEMM3X_TW=8 eight transform /
- *                epilogue warps instead of four, TZK_GEMM3X_RAW=1 the raw fp32 tensors as hi operands,
- *                TZK_GEMM3X_SPLIT=1 four dedicated epilogue warps, TZK_GEMM3X_PREFETCH=1 (with STACK) L2 prefetch of
- *                the x boxes 12 chunks ahead of the loads, TZK_GEMM3X_RING=1 the ring kernel (x in a ring of its own,
- *                used in place as the hi operand; implies RAW / STACK / dedicated epilogue warps).
  *   tzk_wgrad3x  dw[64,K] = dz[M,64]^T @ x[M,K], reduction over the batch split into `slabs` row slabs whose partial
  *                results (scratch `partial`, tzk_wgrad3x_partial_floats(K, slabs) floats) are added in a fixed order:
  *                bit-repeatable.
- * Accuracy note: the tensor core rounds its fp32 accumulator toward zero; the kernels spread a tile's K range over
- * several TMEM accumulators and add them in round-to-nearest (see the comment at Cfg in the source). */
+ * Accuracy note: the tensor core's fp32 accumulation is not round-to-nearest; the kernels accumulate every k-step
+ * (8 columns of K) in fresh registers and add them in round-to-nearest (see the comment at the top of the source). */
 #ifndef TZK_GEMM3X_H_
 #define TZK_GEMM3X_H_
 #include <stddef.h>

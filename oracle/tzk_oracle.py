@@ -5,8 +5,8 @@ __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs use 
 checker or as the timed CPU baseline — never as the product.
 
 It is a numpy restatement of the algorithm the reference runs for this path.  The arithmetic lives in
-third-party wheels that are NOT vendored in /root/reference (torchrec==1.7.0, fbgemm-gpu==1.7.0;
-/root/reference/requirements/runtime.txt:25,5), so each function restates the published semantics of the
+third-party wheels that are NOT vendored in the reference (torchrec==1.7.0, fbgemm-gpu==1.7.0;
+requirements/runtime.txt:25,5), so each function restates the published semantics of the
 upstream operator it names ([EXT], SURVEY.md Appendix A) and cites the reference call site that reaches it.
 
 PINNING STATUS (see DESIGN.md §5):

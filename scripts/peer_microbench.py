@@ -55,24 +55,24 @@ def main():
         n2 = 2 * n                              # a whole N = 2 gather: half of the rows local, half on the peer
         idx2 = torch.randint(0, rows, (n2,), device=dev, dtype=torch.int32)
         loc2 = torch.empty(n2 * 16, device=dev)
-        for grid in (148 * 4, 148 * 8):
+        for grid in (132 * 4, 132 * 8):
             ms = timed(lambda: L.bench_rand_read64_mixed(mine, peer, idx2.data_ptr(), n2, loc2.data_ptr(), grid, st))
             print(f"rand_read64  MIXED local/peer in every warp, {n2} rows grid={grid:<5} {ms * 1e3:8.1f} us  "
                   f"(peer half: {gb / ms * 1e3:7.1f} GB/s)", flush=True)
         for U in (1, 8):
-            for grid in (148, 148 * 8):
+            for grid in (132, 132 * 8):
                 ms = timed(lambda: L.bench_rand_read64(peer, idx.data_ptr(), n, loc.data_ptr(), U, grid, st))
                 print(f"rand_read64  peer  U={U:<2} grid={grid:<5} {ms * 1e3:8.1f} us  {gb / ms * 1e3:7.1f} GB/s", flush=True)
-        ms = timed(lambda: L.bench_rand_read64(mine, idx.data_ptr(), n, loc.data_ptr(), 8, 148 * 8, st))
+        ms = timed(lambda: L.bench_rand_read64(mine, idx.data_ptr(), n, loc.data_ptr(), 8, 132 * 8, st))
         print(f"rand_read64  LOCAL U=8  grid=1184  {ms * 1e3:8.1f} us  {gb / ms * 1e3:7.1f} GB/s", flush=True)
-        for grid in (148, 148 * 4, 148 * 8, 148 * 16):
+        for grid in (132, 132 * 4, 132 * 8, 132 * 16):
             ms = timed(lambda: L.bench_rand_write64(loc.data_ptr(), idx.data_ptr(), n, peer, grid, st))
             print(f"rand_write64 peer       grid={grid:<5} {ms * 1e3:8.1f} us  {gb / ms * 1e3:7.1f} GB/s", flush=True)
-        ms = timed(lambda: L.bench_rand_write64(loc.data_ptr(), idx.data_ptr(), n, mine, 148 * 8, st))
+        ms = timed(lambda: L.bench_rand_write64(loc.data_ptr(), idx.data_ptr(), n, mine, 132 * 8, st))
         print(f"rand_write64 LOCAL      grid=1184  {ms * 1e3:8.1f} us  {gb / ms * 1e3:7.1f} GB/s", flush=True)
         nf = 64 * 1024 * 1024                   # 256 MB contiguous
         big = torch.empty(nf, device=dev)
-        for grid in (148 * 4, 148 * 16):
+        for grid in (132 * 4, 132 * 16):
             ms = timed(lambda: L.bench_seq_copy(peer, nf, big.data_ptr(), grid, st))
             print(f"seq read  peer->local   grid={grid:<5} {ms * 1e3:8.1f} us  {nf * 4 / 1e9 / ms * 1e3:7.1f} GB/s", flush=True)
             ms = timed(lambda: L.bench_seq_copy(big.data_ptr(), nf, peer, grid, st))

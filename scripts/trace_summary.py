@@ -1,6 +1,6 @@
 """Kernel timeline of the LAST step in a chrome trace written by `bench.py --trace` (torch.profiler): per kernel
 start offset, duration, stream — to see what overlaps what inside the captured step.
-    python scripts/trace_summary.py gpurun_out/trace_n2.json"""
+    python scripts/trace_summary.py trace_n2.json"""
 import json
 import sys
 

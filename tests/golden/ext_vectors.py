@@ -1,6 +1,6 @@
 """[EXT] known-answer vectors for the third-party half of the path, restated from the upstream projects' own unit tests
 and docstrings (torchrec 1.x / fbgemm_gpu 1.x — the wheels the reference pins in requirements/runtime.txt:5,25; their
-sources are not under /root/reference and cannot be installed offline, so these are written down from the published
+sources are not part of the reference and cannot be installed offline, so these are written down from the published
 material, each with the upstream symbol it comes from).  Every vector was re-derived by hand from the documented
 semantics when it was added (the derivation is in the comment) — a vector that only restated this repo's own reading
 would prove nothing.

@@ -3,9 +3,9 @@
 The reference package cannot be imported as a whole (torchrec / fbgemm_gpu / pyfg are absent), but
 tzrec/modules/fm.py, interaction.py, mlp.py, mmoe.py, task_tower.py and sequence.py are plain PyTorch: they are loaded file by file
 through stub parent packages, executed on seeded inputs, and their outputs (and autograd gradients) are
-stored as small .npz fixtures.  /root/reference does not travel to the GPU box; the fixtures do.
+stored as small .npz fixtures; the tests read only the fixtures.
 
-    python tests/golden/make_golden_from_reference.py [dense|blocks]
+    TZREC_REFERENCE=<checkout of alibaba/TorchEasyRec @ 54cac316> python tests/golden/make_golden_from_reference.py [dense|blocks]
 """
 import os
 import sys
@@ -14,7 +14,7 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("TZREC_REFERENCE", "")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

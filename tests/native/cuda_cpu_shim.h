@@ -38,7 +38,7 @@ constexpr int cudaSuccess = 0;
 constexpr int cudaDevAttrMultiProcessorCount = 16;
 inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
-inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 148; return cudaSuccess; }
+inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 132; return cudaSuccess; }
 
 namespace tzk_shim {
 inline thread_local dim3 t_thread, t_block, t_bdim, t_gdim;

@@ -80,7 +80,7 @@ def test_package_import_graph_never_reaches_the_oracle():
 
 
 def test_gemm3x_library_exports_its_header():
-    """include/tzk_gemm3x.h <-> libtzk_gemm3x.so (the tcgen05 GEMMs of the wide tower layer)."""
+    """include/tzk_gemm3x.h <-> libtzk_gemm3x.so (the 3xTF32 GEMMs of the wide tower layer)."""
     src = open(os.path.join(ROOT, "include", "tzk_gemm3x.h")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
     declared = set(re.findall(r"\b(tzk_[a-z0-9_]+)\s*\(", src))

@@ -1,4 +1,4 @@
-"""N>1 on real GPUs (needs >= 2 devices: `gpurun --gpus 2 -- python -m pytest tests/test_distributed_gpu.py`):
+"""N>1 on real GPUs (needs >= 2 devices: `python -m pytest tests/test_distributed_gpu.py` on a multi-GPU node):
 the same sharded-vs-unsharded comparison as tests/test_distributed_cpu.py, but with the CUDA kernels as compute and
 NCCL all-to-alls.  Skipped on single-GPU boxes."""
 import pytest

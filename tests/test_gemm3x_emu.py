@@ -1,13 +1,12 @@
-"""The tcgen05 3xTF32 GEMM (torcheasyrec_b200/csrc/tzk_gemm3x.cu) executed on the CPU from its actual source.
+"""The 3xTF32 GEMMs of the wide tower layer (torcheasyrec_b200/csrc/tzk_gemm3x.cu) executed on the CPU from their actual
+source.
 
-`cuda_cpu_shim.h` runs the kernels with one std::thread per CUDA thread (192 per CTA: TMA producer, MMA issuer, four
-transform / epilogue warps) and `tcgen05_cpu_emu.h` stands in for the hardware: mbarriers with transaction counts,
-TMA box loads with SWIZZLE_128B and out-of-bounds zero fill, tcgen05.mma decoded from the instruction and
-shared-memory descriptors (K-major and MN-major canonical layouts, TF32 operand truncation), TMEM with the
-per-warp lane-ownership rule, tcgen05.ld.  What this proves: control flow, barrier protocol, descriptor arithmetic
-(k-step advance inside the swizzle atom, LBO / SBO), tile -> (row, column) mapping, K-tail and M-tail handling and the
-epilogues are consistent with those semantics and produce fp32-accurate results.  What it cannot prove: that the
-hardware agrees with the emulation (the descriptor FIELDS are checked against CuTe in test_umma_desc.py)."""
+`cuda_cpu_shim.h` runs the kernels with one std::thread per CUDA thread (256 per CTA) and `sm90_cpu_emu.h` stands in
+for the hardware: mbarriers with transaction counts, TMA box loads with SWIZZLE_128B and out-of-bounds zero fill, and
+mma.sync m16n8k8 TF32 with the fragment layouts of the PTX ISA and TF32 operand truncation.  What this proves: control
+flow, barrier protocol, swizzled shared-memory addressing, fragment -> (row, column) mapping, K-tail and M-tail handling
+and the epilogues are consistent with those semantics and produce fp32-accurate results.  What it cannot prove: that
+the hardware agrees with the emulation (tests/test_kernels_gpu.py checks that on the GPU)."""
 import ctypes
 import os
 import subprocess
@@ -45,7 +44,7 @@ def lib(tmp_path_factory):
 
 def _delegate(request, lib) -> bool:
     """Every case runs in a child pytest process: the emulation aborts the process on a protocol violation or a
-    deadlock (192-320 real threads per emulated CTA), and that must fail ONE test, not take the whole suite down.
+    deadlock (256 real threads per emulated CTA), and that must fail ONE test, not take the whole suite down.
     An abnormal exit is retried once (thread-scheduling artefacts of the emulation have been seen once in thousands of
     CTAs); an ordinary assertion failure is not."""
     if CHILD:
@@ -67,16 +66,15 @@ def _p(a):
     return None if a is None else a.ctypes.data
 
 
-# error budget: the emulated tensor core adds ~2400 fp32 products one after another (a plain running sum), which costs
-# more than the split itself; numpy's blocked fp32 matmul sits at ~2e-6 on the same data
+# error budget: the emulated tensor core adds the products of a 32-column chunk one after another (a plain running sum),
+# which costs more than the split itself; numpy's blocked fp32 matmul sits at ~2e-6 on the same data
 TOL = 2e-5
 
 
 @pytest.fixture
 def stack():
-    """One configuration is built since round 2 (stacked W_hi / W_lo as one N = 2*BN MMA + lo(x) * W_hi, four transform
-    warps + four dedicated epilogue warps); the other variants were timed on hardware and deleted
-    (profiles/r2_gemm3x_variants.txt)."""
+    """One configuration is built: W arrives split into W_hi / W_lo (the scratch the forward writes), X is split in
+    registers."""
     return ("1", "4", "0", "1", "0", "0")
 
 
@@ -97,7 +95,7 @@ def test_forward_784_to_64(request, lib, stack, M, relu, bias):
     ref = np.maximum(ref, 0) if relu else ref
     np.testing.assert_allclose(y[:M], ref, rtol=0, atol=TOL)
     assert np.isnan(y[M]).all()
-    if stack[2] == "0":     # the split really is hi + lo with hi on the TF32 grid (raw mode writes lo only)
+    if stack[2] == "0":     # the split really is hi + lo with hi on the TF32 grid
         assert (wh.view(np.uint32) & 0x1FFF == 0).all() and (wl.view(np.uint32) & 0x1FFF == 0).all()
         np.testing.assert_allclose(wh.astype(np.float64) + wl, w, rtol=2 ** -21)
     # plain TF32 (hi x hi only) would be ~1000x worse: the lo terms are doing their job
@@ -108,7 +106,7 @@ def test_forward_784_to_64(request, lib, stack, M, relu, bias):
 
 
 def test_dgrad_64_to_784(request, lib, stack):
-    """The input-gradient pass: BN = 112, seven column tiles per row tile, two k-chunks, three stages."""
+    """The input-gradient pass: BN = 56, fourteen column tiles per row tile, two k-chunks, three stages."""
     if _delegate(request, lib):
         return
     rng = np.random.default_rng(1)

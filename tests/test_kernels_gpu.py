@@ -575,9 +575,9 @@ def test_gradient_clipping_on_classic_optimizers(kernels, bwd_path):
 
 @pytest.mark.parametrize("M", [300, 65536 + 5])
 def test_gemm3x_kernels_match_fp64(monkeypatch, M):
-    """csrc/tzk_gemm3x.cu (libtzk_gemm3x.so), the three passes of the 783 -> 64 tower layer on hand-written tcgen05
-    kind::tf32 kernels with the 3xTF32 split: forward (bias + ReLU epilogue), dgrad (W^T), wgrad (MN-major operands,
-    bit-repeatable slab reduction).  fp32-level error against float64 — the same bound torch's fp32 SIMT GEMM meets."""
+    """csrc/tzk_gemm3x.cu (libtzk_gemm3x.so), the three passes of the 783 -> 64 tower layer on hand-written TMA-fed
+    mma.sync TF32 kernels with the 3xTF32 split: forward (bias + ReLU epilogue), dgrad (W^T), wgrad (dZ^T X straight
+    from the row-major tensors, bit-repeatable slab reduction).  fp32-level error against float64 — the same bound torch's fp32 SIMT GEMM meets."""
     from torcheasyrec_b200 import dense_gemm as G
 
     lib = G._gemm3x_lib()
@@ -606,7 +606,8 @@ def test_gemm3x_kernels_match_fp64(monkeypatch, M):
 @pytest.mark.parametrize("M", [300, 65536 + 5])
 def test_wide_layer_on_tcgen05_matches_fp64(monkeypatch, M):
     """TZK_GEMM3X=1: the 783 -> 64 tower layer (input travelling as [B, 784] with a zero column) through
-    dense_gemm.linear — forward with fused bias + ReLU, dgrad, wgrad — against float64 autograd."""
+    dense_gemm.linear — forward with fused bias + ReLU, dgrad, wgrad — against float64 autograd.  (The name is that of
+    the layer's first, Blackwell implementation; the test is the same for the Hopper kernels.)"""
     from torcheasyrec_b200 import dense_gemm as G
 
     if G._gemm3x_lib() is None:
@@ -738,10 +739,10 @@ def test_fp16_sequence_collection_rows(kernels):
     assert torch.equal(rows, ec.table_weight(0)[cu(ids)].float())
 
 
-# Paths that have not been through a GPU validation pass yet run only when asked for (scripts/gpu_call_n1.sh sets
-# TZK_EXPERIMENTAL=1); a validated path loses the mark and gets its default flipped in the library.
+# Paths that have not been through a GPU validation pass yet run only when asked for (TZK_EXPERIMENTAL=1); a
+# validated path loses the mark and gets its default flipped in the library.
 unvalidated = pytest.mark.skipif(os.environ.get("TZK_EXPERIMENTAL") != "1",
-                                 reason="unvalidated path: set TZK_EXPERIMENTAL=1 (scripts/gpu_call_n1.sh)")
+                                 reason="unvalidated path: set TZK_EXPERIMENTAL=1")
 
 
 # ---- interleaved [weight row | Adagrad accumulator row] arenas (tzk_opt_args.interleaved) -----------------------------------

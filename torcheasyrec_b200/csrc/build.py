@@ -1,4 +1,4 @@
-"""Builds libtzk.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libtzk.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 No torch dependency: plain `nvcc -shared`.  Objects are rebuilt only when a source is newer.
 """
@@ -13,7 +13,7 @@ HEADERS = ["tzk_common.cuh", "tzk_tower_bwd2.cuh", "tzk_interact_tc.cuh", "tzk_t
 LIB = os.path.join(HERE, "libtzk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -50,7 +50,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if failed:
         raise RuntimeError("libtzk build failed")
     if force or procs or _mtime(LIB) < max(_mtime(o) for o in objs):
-        # link next to the target and rename: a reader (a gpurun snapshot, another process) never sees a torn library
+        # link next to the target and rename: a reader (another process) never sees a torn library
         cmd = [NVCC, "-shared", "-Wno-deprecated-gpu-targets", "-o", LIB + ".tmp", *objs]
         subprocess.run(cmd, check=True)
         os.replace(LIB + ".tmp", LIB)
@@ -60,10 +60,10 @@ def build(verbose: bool = False, force: bool = False) -> str:
 
 
 def build_gemm3x(force: bool = False) -> str:
-    """libtzk_gemm3x.so: hand-written tcgen05 3xTF32 GEMMs of the wide tower layer (forward, dgrad, wgrad)."""
+    """libtzk_gemm3x.so: hand-written TMA + mma.sync 3xTF32 GEMMs of the wide tower layer (forward, dgrad, wgrad)."""
     src = os.path.join(HERE, "tzk_gemm3x.cu")
     lib = os.path.join(HERE, "libtzk_gemm3x.so")
-    deps = [src] + [os.path.join(HERE, h) for h in ("tzk_umma_desc.h", "tzk_tcgen05_ptx.h")]
+    deps = [src] + [os.path.join(HERE, h) for h in ("tzk_sm90_ptx.h",)]
     if force or _mtime(lib) < max(_mtime(d) for d in deps):
         subprocess.run([NVCC, *FLAGS, "-shared", src, "-o", lib + ".tmp"], check=True)
         os.replace(lib + ".tmp", lib)

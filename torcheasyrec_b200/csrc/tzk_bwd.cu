@@ -1,4 +1,4 @@
-// tzk_bwd.cu — K5 fused segmented backward + sparse optimizer (sm_100a).
+// tzk_bwd.cu — K5 fused segmented backward + sparse optimizer (sm_90a).
 //
 // Pipeline (all on the caller's stream, no host sync):
 //   1. linearize : key[l] = feat_key_base[f] + id[l], val[l] = bag (pooled) or l (sequence)
@@ -680,8 +680,8 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
     }
     return;
   }
-  // One sorted position per lane group and iteration (2 and 4 positions with a batched single-run path were measured
-  // slower in round 1: 349 / 375 / 461 us for 1 / 2 / 4 on DLRM-Criteo).  The keys / value of the NEXT position are
+  // One sorted position per lane group and iteration (2 and 4 positions with a batched single-run path were slower on
+  // DLRM-Criteo).  The keys / value of the NEXT position are
   // requested before the current one is worked on.
   int64_t p0 = (int64_t)cta * NG + threadIdx.x / G;
   KeyT kl = 0, kc = 0, kr = 0;     // left neighbour, this position, right neighbour
@@ -1224,7 +1224,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   wl.counters = reinterpret_cast<int32_t*>(ws + L.counters);
   wl.partials = reinterpret_cast<float*>(ws + L.partials);
   // short-run head list in the sort's dead INPUT buffers (n int32 positions in vals_in, n int32 lengths in keys_in).
-  // Default on (validated on B200: gradient half 176 -> 130 us on DLRM-Criteo); TZK_BWD_HEADS=0: walk every position.
+  // Default on; TZK_BWD_HEADS=0: walk every position.
   // Both halves of a step read the switch, so it must not change between a sort and its apply.
   wl.head_pos = nullptr;
   wl.head_len = nullptr;
@@ -1240,7 +1240,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   if ((phases & 1) && pw) {
     size_t cub_bytes = L.cub_bytes;
     cudaError_t ce;
-    const int grid_p = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountB200 * 8);
+    const int grid_p = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountH100 * 8);
     if (k64) {
       peer_pull_linearize_kernel<uint64_t><<<grid_p, kThreads, 0, st>>>(*pw, (uint64_t)sentinel, (uint64_t*)keys_in,
                                                                          vals_in, overflow);
@@ -1257,11 +1257,11 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
     TZK_REQUIRE(ce == cudaSuccess, "fused_bwd: radix sort failed: %s", cudaGetErrorString(ce));
   } else if (phases & 1) {
   const int64_t n_bags = (int64_t)F * B;
-  int grid_lin = (int)std::min<int64_t>(ceil_div64(n_bags, kThreads), kSmCountB200 * 16);
+  int grid_lin = (int)std::min<int64_t>(ceil_div64(n_bags, kThreads), kSmCountH100 * 16);
   size_t cub_bytes = L.cub_bytes;
   cudaError_t ce;
   const size_t smem_lin = (size_t)(3 * F + 1) * sizeof(int64_t);
-  const int grid_seq = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountB200 * 16);
+  const int grid_seq = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountH100 * 16);
   if (k64) {
     if (pooled)
       linearize_kernel<uint64_t><<<grid_lin, kThreads, 0, st>>>(ids, offsets, feat_rows, feat_key_base, F, B,
@@ -1287,7 +1287,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   }
   if (phases & 1) {   // work list of the long runs (tiny tables, hot ids) for the gradient half's chunk CTAs
     zero_counters<<<1, 1, 0, st>>>(wl.counters);
-    const int grid_f = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountB200 * 8);
+    const int grid_f = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountH100 * 8);
     if (k64) find_long_runs_kernel<uint64_t><<<grid_f, kThreads, 0, st>>>((const uint64_t*)keys_out, nnz, (uint64_t)sentinel, wl);
     else find_long_runs_kernel<uint32_t><<<grid_f, kThreads, 0, st>>>((const uint32_t*)keys_out, nnz, (uint32_t)sentinel, wl);
     TZK_CHECK_LAUNCH("find_long_runs_kernel");
@@ -1330,11 +1330,10 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   TZK_REQUIRE(ch <= 8, "fused_bwd: max_dim=%d needs %d chunks per lane (> 8); unaligned wide rows are not supported",
               max_dim, ch);
   const int NG = kThreads / G;
-  int grid_s = (int)std::min<int64_t>(ceil_div64(nnz, NG), kSmCountB200 * 16);
-  // TZK_BWD_TILE=1 selects the tile path.  Measured on DLRM-Criteo (B200, 1.7 M ids): both paths spend ~200 us in
-  // the gradient half — the random 64-B weight/state/gradient accesses top out near 2-2.3 TB/s of DRAM traffic either
-  // way — and the general kernels execute fewer instructions (74 M vs 87 M warp-instructions) without the three
-  // barriers per tile, so they stay the default.
+  int grid_s = (int)std::min<int64_t>(ceil_div64(nnz, NG), kSmCountH100 * 16);
+  // TZK_BWD_TILE=1 selects the tile path.  Both paths are bound by the random 64-B weight/state/gradient accesses of
+  // the gradient half, and the general kernels execute fewer instructions without the three barriers per tile, so
+  // they stay the default.
   const char* tile_env = getenv("TZK_BWD_TILE");
   const bool tile_path = tile_env && tile_env[0] == '1' && !a.w_f16 && !a.interleaved && optimizer != TZK_OPT_ACCUM_OUT;   // (fp32 tables, real updates)
   if (vec == 4 && ch == 1 && tile_path) {
@@ -1350,7 +1349,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
     if (smem_t > 48 * 1024)                                                                                     \
       cudaFuncSetAttribute(tile_update_kernel<KeyT, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
                            (int)smem_t);                                                                        \
-    const int grid_t = (int)std::min<int64_t>(n_tiles, kSmCountB200 * 8);                                       \
+    const int grid_t = (int)std::min<int64_t>(n_tiles, kSmCountH100 * 8);                                       \
     tile_update_kernel<KeyT, G_><<<grid_t, kThreads, smem_t, st>>>(                                             \
         a, feat_w_off, feat_rows, feat_key_base, feat_dim, feat_col, feat_pool, (const KeyT*)keys_out, vals_out, \
         carry_first, carry_last, gp);                                                                           \
@@ -1360,7 +1359,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
       if (smem_c > 48 * 1024)                                                                                   \
         cudaFuncSetAttribute(carry_combine_kernel<KeyT, G_>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
                              (int)smem_c);                                                                      \
-      const int grid_c = (int)std::min<int64_t>(ceil_div64(n_tiles - 1, C::NG), kSmCountB200 * 8);              \
+      const int grid_c = (int)std::min<int64_t>(ceil_div64(n_tiles - 1, C::NG), kSmCountH100 * 8);              \
       carry_combine_kernel<KeyT, G_><<<grid_c, kThreads, smem_c, st>>>(                                         \
           a, feat_w_off, feat_rows, feat_key_base, feat_dim, feat_col, feat_pool, (const KeyT*)keys_out,        \
           vals_out, carry_first, carry_last);                                                                   \
@@ -1383,7 +1382,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   }
 
   // general path: one launch — short runs by sorted position + the long-run list's chunk CTAs (CH compiled for 1, 2, 8)
-  const int n_long = kSmCountB200 * 2;
+  const int n_long = kSmCountH100 * 2;
   if (k64) {
     if (vec == 4) { if (ch == 1) { TZK_BWD_DISPATCH_G(uint64_t, 4, 1) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint64_t, 32, 4, 2); } else { TZK_BWD_LAUNCH(uint64_t, 32, 4, 8); } }
     else { if (ch == 1) { TZK_BWD_DISPATCH_G(uint64_t, 1, 1) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint64_t, 32, 1, 2); } else { TZK_BWD_LAUNCH(uint64_t, 32, 1, 8); } }
@@ -1557,7 +1556,7 @@ extern "C" int tzk_peer_small_update(const tzk_opt_args* opt, const uint64_t* ps
   int G = 1;
   while (G * 4 < max_dim) G <<= 1;
   const int NG = kThreads / G;
-  const int grid = (int)std::min<int64_t>(ceil_div64(total_rows, NG), kSmCountB200 * 8);
+  const int grid = (int)std::min<int64_t>(ceil_div64(total_rows, NG), kSmCountH100 * 8);
   const size_t smem = (size_t)n_tabs * sizeof(SmallTab);
   cudaStream_t st = as_stream(stream);
   const SmallTab* tp = static_cast<const SmallTab*>(tabs);
@@ -1634,7 +1633,7 @@ extern "C" int tzk_bag_grad_expand(const float* grad_out, int64_t ld_grad, const
   cudaStream_t st = as_stream(stream);
   const bool vec = (D % 4 == 0) && ((uintptr_t)grad_out % 16 == 0) && ((uintptr_t)g_rows % 16 == 0) && (ld_grad % 4 == 0);
   const int64_t items = (int64_t)F * B * (vec ? D / 4 : D);
-  const int grid = (int)std::min<int64_t>(ceil_div64(items, kThreads), kSmCountB200 * 16);
+  const int grid = (int)std::min<int64_t>(ceil_div64(items, kThreads), kSmCountH100 * 16);
   if (vec)
     bag_grad_expand_kernel<<<grid, kThreads, 0, st>>>(grad_out, ld_grad, feat_col, feat_pool, offsets, slot, F, B, D,
                                                        g_rows);

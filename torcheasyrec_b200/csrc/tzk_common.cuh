@@ -1,4 +1,4 @@
-// Shared helpers for the tzk kernels (sm_100a only).
+// Shared helpers for the tzk kernels (sm_90a only).
 #pragma once
 #include <stdlib.h>
 #include <cuda_fp16.h>
@@ -31,10 +31,10 @@ inline cudaStream_t as_stream(tzk_stream_t s) { return reinterpret_cast<cudaStre
     }                                 \
   } while (0)
 
-constexpr int kSmCountB200 = 148;
+constexpr int kSmCountH100 = 132;   // H100 SXM
 
 // Switches of code paths that have not been through a GPU validation pass yet: `name`=0/1 decides; unset,
-// TZK_EXPERIMENTAL=1 turns them all on (scripts/gpu_call_n1.sh); otherwise they stay off.
+// TZK_EXPERIMENTAL=1 turns them all on; otherwise they stay off.
 inline bool unvalidated_switch(const char* name) {
   const char* e = getenv(name);
   if (e && (e[0] == '0' || e[0] == '1')) return e[0] == '1';
@@ -64,8 +64,6 @@ __device__ __forceinline__ float4 ld_coh_f4(const float* p) {
   return r;
 }
 // rows that the same kernel writes back (weights / optimizer state): coherent load
-// (measured, round 1: neither cudaLimitMaxL2FetchGranularity 32/64/128 nor the .L2::64B load hint changes the gather
-//  or fused-backward time on B200 — the default fetch granularity is already 64 B)
 __device__ __forceinline__ float4 ld_rw_f4(const float* p) {
   float4 r;
   asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"

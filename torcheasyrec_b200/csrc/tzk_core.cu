@@ -172,7 +172,7 @@ extern "C" int tzk_lengths_to_offsets(const int32_t* lengths, int64_t n, int64_t
   TZK_CHECK_LAUNCH("scan_tile_sums");
   scan_tile_offsets<<<1, kScanThreads, 0, st>>>(tile_sum, tiles);
   TZK_CHECK_LAUNCH("scan_tile_offsets");
-  const char* staged_env = getenv("TZK_SCAN_STAGED");      // default on (validated: 18.5 -> 9.8 us at n = 1.7 M); 0: direct stores
+  const char* staged_env = getenv("TZK_SCAN_STAGED");      // default on; 0: direct stores
   if (!(staged_env && staged_env[0] == '0')) scan_tiles<true><<<(unsigned)tiles, kScanThreads, 0, st>>>(lengths, n, tile_sum, offsets);
   else scan_tiles<false><<<(unsigned)tiles, kScanThreads, 0, st>>>(lengths, n, tile_sum, offsets);
   TZK_CHECK_LAUNCH("scan_tiles");

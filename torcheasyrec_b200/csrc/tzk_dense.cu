@@ -191,7 +191,7 @@ __device__ __forceinline__ void stage_x(float* X, const float* dense, int64_t ld
 
 // DT = compile-time embedding dim (0 = take the runtime value): with DT known every /D, %D and swizzle offset
 // folds into shifts and the k loop unrolls — the kernel is issue-bound, not bandwidth-bound, otherwise.
-// 4 CTAs/SM (64 registers, a few spilled words) measured 105 us against 127 us at 3 CTAs/SM (80 registers).
+// 4 CTAs/SM (64 registers, a few spilled words) rather than 3 CTAs/SM (80 registers): the occupancy hides the latency.
 template <int DT, bool ONE, int NT>
 __global__ void __launch_bounds__(kIWarps * 32, 4)
 dot_interact_fwd_kernel(const float* __restrict__ dense, int64_t ld_dense, const float* __restrict__ sparse,
@@ -509,7 +509,7 @@ dot_interact_bwd_kernel(const float* __restrict__ dense, int64_t ld_dense, const
 }
 
 // The DLRM-Criteo shape (27 x 16, aligned output row) on the tensor cores (tzk_interact_tc.cuh); read per call (tests flip
-// it).  Forward: default on (validated on B200: 82.7 -> 58.7 us at B = 65536), TZK_INTERACT_TC=0 / TZK_INTERACT_TC_FWD=0
+// it).  Forward: default on, TZK_INTERACT_TC=0 / TZK_INTERACT_TC_FWD=0
 // selects the FFMA kernel.  Backward: default on since its pass-through loads are requested up front (step 1.031 -> 1.010 ms);
 // TZK_INTERACT_TC_BWD=0 selects the FFMA kernel.
 inline bool env_is(const char* name, char v) {
@@ -539,7 +539,7 @@ extern "C" int tzk_col_gather_sum(const float* const* srcs_host, const int64_t* 
     srcs.p[i] = i < n_src ? srcs_host[i] : nullptr;
     srcs.ld[i] = i < n_src ? src_ld_host[i] : 0;
   }
-  col_gather_sum_kernel<<<grid_for(rows * C, kThreads, kSmCountB200 * 16), kThreads, 0, as_stream(stream)>>>(
+  col_gather_sum_kernel<<<grid_for(rows * C, kThreads, kSmCountH100 * 16), kThreads, 0, as_stream(stream)>>>(
       srcs, col_start, col_src, col_srccol, C, rows, out, ld_out);
   TZK_CHECK_LAUNCH("col_gather_sum_kernel");
   return 0;
@@ -550,7 +550,7 @@ extern "C" int tzk_jagged_to_padded(const float* values, const int64_t* offsets,
   TZK_REQUIRE(B >= 0 && T >= 0 && D >= 1, "jagged_to_padded: bad sizes");
   if (B == 0 || T == 0) return 0;
   TZK_REQUIRE(offsets && out, "jagged_to_padded: NULL argument");
-  jagged_to_padded_kernel<<<grid_for((int64_t)B * T * D, kThreads, kSmCountB200 * 16), kThreads, 0,
+  jagged_to_padded_kernel<<<grid_for((int64_t)B * T * D, kThreads, kSmCountH100 * 16), kThreads, 0,
                             as_stream(stream)>>>(values, offsets, B, T, D, out);
   TZK_CHECK_LAUNCH("jagged_to_padded_kernel");
   return 0;
@@ -561,7 +561,7 @@ extern "C" int tzk_padded_to_jagged(const float* grad_out, const int64_t* offset
   TZK_REQUIRE(B >= 0 && T >= 0 && D >= 1 && nnz >= 0, "padded_to_jagged: bad sizes");
   if (nnz == 0) return 0;
   TZK_REQUIRE(B > 0 && offsets && grad_values && (T == 0 || grad_out), "padded_to_jagged: NULL argument");
-  padded_to_jagged_kernel<<<grid_for(nnz * D, kThreads, kSmCountB200 * 16), kThreads, 0, as_stream(stream)>>>(
+  padded_to_jagged_kernel<<<grid_for(nnz * D, kThreads, kSmCountH100 * 16), kThreads, 0, as_stream(stream)>>>(
       grad_out, offsets, B, T, D, nnz, grad_values);
   TZK_CHECK_LAUNCH("padded_to_jagged_kernel");
   return 0;
@@ -572,7 +572,7 @@ extern "C" int tzk_fm_fwd(const float* x, int64_t ld_x, int64_t B, int32_t N, in
   TZK_REQUIRE(B >= 0 && N >= 0 && D >= 1, "fm_fwd: bad sizes");
   if (B == 0) return 0;
   TZK_REQUIRE(x && y, "fm_fwd: NULL argument");
-  fm_fwd_kernel<<<grid_for(B * D, kThreads, kSmCountB200 * 16), kThreads, 0, as_stream(stream)>>>(
+  fm_fwd_kernel<<<grid_for(B * D, kThreads, kSmCountH100 * 16), kThreads, 0, as_stream(stream)>>>(
       x, ld_x, B, N, D, y, ld_y);
   TZK_CHECK_LAUNCH("fm_fwd_kernel");
   return 0;
@@ -583,7 +583,7 @@ extern "C" int tzk_fm_bwd(const float* x, int64_t ld_x, const float* dy, int64_t
   TZK_REQUIRE(B >= 0 && N >= 0 && D >= 1, "fm_bwd: bad sizes");
   if (B == 0) return 0;
   TZK_REQUIRE(x && dy && dx, "fm_bwd: NULL argument");
-  fm_bwd_kernel<<<grid_for(B * D, kThreads, kSmCountB200 * 16), kThreads, 0, as_stream(stream)>>>(
+  fm_bwd_kernel<<<grid_for(B * D, kThreads, kSmCountH100 * 16), kThreads, 0, as_stream(stream)>>>(
       x, ld_x, dy, ld_dy, B, N, D, dx, ld_dx);
   TZK_CHECK_LAUNCH("fm_bwd_kernel");
   return 0;
@@ -614,7 +614,7 @@ extern "C" int tzk_dot_interact_fwd(const float* dense, int64_t ld_dense, const 
   const int P = N * (N - 1) / 2;
   TZK_REQUIRE(p_pad >= 0 && p_pad < 4, "dot_interact_fwd: p_pad must be in [0,3]");
   if (use_interact_tc_fwd() && tzk_itc::covers(dense, ld_dense, ld_sparse, Ns, D, copy_dense, copy_sparse, p_pad, out, ld_out)) {
-    tzk_itc::dot_interact27_fwd_tc_kernel<<<tzk_itc::grid_for(B, kSmCountB200 * 8), tzk_itc::kWarps * 32,
+    tzk_itc::dot_interact27_fwd_tc_kernel<<<tzk_itc::grid_for(B, kSmCountH100 * 8), tzk_itc::kWarps * 32,
                                             tzk_itc::fwd_smem(), as_stream(stream)>>>(dense, ld_dense, sparse, ld_sparse,
                                                                                       B, out, ld_out);
     TZK_CHECK_LAUNCH("dot_interact27_fwd_tc_kernel");
@@ -628,7 +628,7 @@ extern "C" int tzk_dot_interact_fwd(const float* dense, int64_t ld_dense, const 
     if (smem > 48 * 1024)                                                                                    \
       cudaFuncSetAttribute(dot_interact_fwd_kernel<DT_, ONE_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                            (int)smem);                                                                       \
-    dot_interact_fwd_kernel<DT_, ONE_, NT_><<<grid_for(B, kIWarps, kSmCountB200 * 8), kIWarps * 32, smem,     \
+    dot_interact_fwd_kernel<DT_, ONE_, NT_><<<grid_for(B, kIWarps, kSmCountH100 * 8), kIWarps * 32, smem,     \
                                               as_stream(stream)>>>(                                          \
         dense, ld_dense, sparse, ld_sparse, B, Ns, D, copy_dense, copy_sparse, p_pad, aligned, out, ld_out); \
   } while (0)
@@ -673,7 +673,7 @@ extern "C" int tzk_dot_interact_bwd(const float* dense, int64_t ld_dense, const 
   const int P = N * (N - 1) / 2;
   TZK_REQUIRE(p_pad >= 0 && p_pad < 4, "dot_interact_bwd: p_pad must be in [0,3]");
   if (use_interact_tc_bwd() && tzk_itc::covers(dense, ld_dense, ld_sparse, Ns, D, copy_dense, copy_sparse, p_pad, d_out, ld_dout)) {
-    tzk_itc::dot_interact27_bwd_tc_kernel<<<tzk_itc::grid_for(B, kSmCountB200 * 8), tzk_itc::kWarps * 32,
+    tzk_itc::dot_interact27_bwd_tc_kernel<<<tzk_itc::grid_for(B, kSmCountH100 * 8), tzk_itc::kWarps * 32,
                                             tzk_itc::bwd_smem(), as_stream(stream)>>>(
         dense, ld_dense, sparse, ld_sparse, d_out, ld_dout, B, d_dense, ld_ddense, d_sparse, ld_dsparse);
     TZK_CHECK_LAUNCH("dot_interact27_bwd_tc_kernel");
@@ -686,7 +686,7 @@ extern "C" int tzk_dot_interact_bwd(const float* dense, int64_t ld_dense, const 
     if (smem > 48 * 1024)                                                                                    \
       cudaFuncSetAttribute(dot_interact_bwd_kernel<DT_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
                            (int)smem);                                                                       \
-    dot_interact_bwd_kernel<DT_, NT_><<<grid_for(B, kIWarps, kSmCountB200 * 8), kIWarps * 32, smem,           \
+    dot_interact_bwd_kernel<DT_, NT_><<<grid_for(B, kIWarps, kSmCountH100 * 8), kIWarps * 32, smem,           \
                                         as_stream(stream)>>>(                                                \
         dense, ld_dense, sparse, ld_sparse, d_out, ld_dout, B, Ns, D, copy_dense, copy_sparse, p_pad, aligned, \
         d_dense, ld_ddense, d_sparse, ld_dsparse);                                                           \
@@ -809,10 +809,10 @@ extern "C" int tzk_bias_act(float* y, int64_t ld_y, const float* bias, int64_t M
   const bool vec = (N % 4 == 0) && (ld_y % 4 == 0) && ((uintptr_t)y % 16 == 0) &&
                    (!bias || (uintptr_t)bias % 16 == 0) && (M * N / 4 < ((int64_t)1 << 31));
   if (vec)
-    bias_act_vec_kernel<<<grid_for(M * N / 4, kThreads, kSmCountB200 * 16), kThreads, 0, as_stream(stream)>>>(
+    bias_act_vec_kernel<<<grid_for(M * N / 4, kThreads, kSmCountH100 * 16), kThreads, 0, as_stream(stream)>>>(
         y, ld_y, bias, (int)(M * N / 4), N / 4, relu);
   else
-    bias_act_kernel<<<grid_for(M * N, kThreads, kSmCountB200 * 16), kThreads, 0, as_stream(stream)>>>(y, ld_y, bias,
+    bias_act_kernel<<<grid_for(M * N, kThreads, kSmCountH100 * 16), kThreads, 0, as_stream(stream)>>>(y, ld_y, bias,
                                                                                                     M, N, relu);
   TZK_CHECK_LAUNCH("bias_act_kernel");
   return 0;

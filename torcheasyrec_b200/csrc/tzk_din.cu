@@ -127,7 +127,7 @@ jagged_softmax_wsum_bwd_kernel(const float* __restrict__ d_out, const float* __r
 
 inline int grid_for(int B) {
   const int64_t ctas = ceil_div64(B, kWarps);
-  return (int)(ctas < kSmCountB200 * 8 ? (ctas > 0 ? ctas : 1) : kSmCountB200 * 8);
+  return (int)(ctas < kSmCountH100 * 8 ? (ctas > 0 ? ctas : 1) : kSmCountH100 * 8);
 }
 }  // namespace
 

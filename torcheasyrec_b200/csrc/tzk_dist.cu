@@ -137,8 +137,8 @@ extern "C" int tzk_bucketize_rw(const int64_t* ids, const int64_t* offsets, int3
   if (n_bags == 0) return tzk_lengths_to_offsets(nullptr, 0, out_offsets, workspace, workspace_bytes, stream);
   TZK_REQUIRE(offsets && feat_block && out_lengths && (nnz == 0 || (ids && out_ids)),
               "bucketize_rw: NULL argument");
-  int grid = (int)(ceil_div64(n_bags, kThreads) < kSmCountB200 * 16 ? ceil_div64(n_bags, kThreads)
-                                                                   : kSmCountB200 * 16);
+  int grid = (int)(ceil_div64(n_bags, kThreads) < kSmCountH100 * 16 ? ceil_div64(n_bags, kThreads)
+                                                                   : kSmCountH100 * 16);
   bucketize_count_kernel<<<grid, kThreads, 0, st>>>(ids, offsets, feat_block, feat_owner, F, B, W, out_lengths);
   TZK_CHECK_LAUNCH("bucketize_count_kernel");
   int rc = tzk_lengths_to_offsets(out_lengths, n_bags * W, out_offsets, workspace, workspace_bytes, stream);
@@ -157,7 +157,7 @@ extern "C" int tzk_permute_lengths(const int32_t* lengths, const int32_t* perm, 
   const int64_t n = (int64_t)S_out * B;
   if (n == 0) return 0;
   TZK_REQUIRE(lengths && perm && out_lengths, "permute_lengths: NULL argument");
-  int grid = (int)(ceil_div64(n, kThreads) < kSmCountB200 * 16 ? ceil_div64(n, kThreads) : kSmCountB200 * 16);
+  int grid = (int)(ceil_div64(n, kThreads) < kSmCountH100 * 16 ? ceil_div64(n, kThreads) : kSmCountH100 * 16);
   permute_lengths_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(lengths, perm, S_out, B, out_lengths);
   TZK_CHECK_LAUNCH("permute_lengths_kernel");
   return 0;

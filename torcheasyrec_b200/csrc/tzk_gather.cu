@@ -1,4 +1,4 @@
-// tzk_gather.cu — K4 pooled gather forward and K4-nobag sequence gather (sm_100a).
+// tzk_gather.cu — K4 pooled gather forward and K4-nobag sequence gather (sm_90a).
 //
 // HBM-bound byte mover.  Layout decisions (DESIGN.md §3):
 //  * a CTA owns a tile of TB consecutive samples x all F features, so its output region
@@ -256,7 +256,7 @@ static int pooled_gather_fwd_impl(const WT* weights, const int64_t* feat_w_off, 
   cudaStream_t st = as_stream(stream);
   const int n_tiles = (B + kTB - 1) / kTB;
   const int n_work = n_tiles * ((F + kItemsPerCta / kTB - 1) / (kItemsPerCta / kTB));
-  int grid = n_work < kSmCountB200 * 8 ? n_work : kSmCountB200 * 8;
+  int grid = n_work < kSmCountH100 * 8 ? n_work : kSmCountH100 * 8;
   size_t smem = align16((size_t)F * sizeof(FeatDesc)) + (size_t)kItemsPerCta * (sizeof(BagStage) + sizeof(int32_t));
   TZK_REQUIRE(smem <= 48 * 1024, "pooled_gather_fwd: F=%d keys need %zu B of shared memory (> 48 KB)", F, smem);
   if (vec == 4) {
@@ -304,7 +304,7 @@ static int seq_gather_fwd_impl(const WT* weights, const int64_t* feat_w_off, con
   cudaStream_t st = as_stream(stream);
   const int NG = kThreads / G;
   int64_t blocks = ceil_div64(nnz, NG);
-  int grid = blocks < kSmCountB200 * 16 ? (int)blocks : kSmCountB200 * 16;
+  int grid = blocks < kSmCountH100 * 16 ? (int)blocks : kSmCountH100 * 16;
   size_t smem = (size_t)(3 * F + 1) * sizeof(int64_t);
   if (vec == 4) {
     TZK_DISPATCH_G(G, 4, WT, seq_gather_fwd_kernel, weights, feat_w_off, feat_rows, ids, offsets, F, B, D, nnz, out, row_stride)

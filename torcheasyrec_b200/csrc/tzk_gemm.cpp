@@ -1,9 +1,9 @@
 // tzk_gemm.cpp — fp32-accurate tensor-core GEMMs for the dense towers (library GEMM, not a hot-path row).
 //
 // The reference runs its MLP towers as plain fp32 cuBLAS GEMMs with TF32 off (train.proto field 14), i.e. on the
-// CUDA cores.  cuBLASLt 12.9 can run the same fp32 GEMM on Blackwell's tensor cores with the BF16x9 split
+// CUDA cores.  cuBLASLt 12.9 can run the same fp32 GEMM on the tensor cores of GPUs that support the BF16x9 split
 // (CUBLAS_COMPUTE_32F_EMULATED_16BFX9: every fp32 operand is split into three bf16 values, nine products,
-// fp32-equivalent accuracy).  PyTorch 2.11+cu128 bundles cuBLAS 12.8, which lacks it, so this file loads the
+// fp32-equivalent accuracy); where it offers no algorithm for that compute type the plain fp32 GEMM runs.  PyTorch 2.11+cu128 bundles cuBLAS 12.8, which lacks it, so this file loads the
 // toolkit's own libcublasLt.so.12.9 by absolute path (dlopen, RTLD_LOCAL — it coexists with torch's copy) and
 // exposes one row-major GEMM entry point.  If the library or the emulated algorithm is unavailable the caller
 // keeps using torch's GEMM; nothing here is required for correctness.

@@ -1,30 +1,28 @@
-// tzk_gemm3x.cu — libtzk_gemm3x.so: the wide tower layer on the 5th-gen tensor cores (TZK_GEMM3X=1 in dense_gemm.py).
+// tzk_gemm3x.cu — libtzk_gemm3x.so: the wide tower layer on the tensor cores (TZK_GEMM3X=1 in dense_gemm.py).
 //
-// Round-2 groundwork (DESIGN.md §9.1): the one wide tower layer of DLRM's final MLP,
+// The one wide tower layer of DLRM's final MLP,
 //     Y[M,64] = act(X[M,K] @ W[64,K]^T + bias)            (tzrec/modules/mlp.py:20-84, K = 784)
-// as a hand-written sm_100a kernel with fp32-equivalent accuracy on the 5th-gen tensor cores: tcgen05.mma kind::tf32
-// with the 3xTF32 split  x*w ~= hi(x)*hi(w) + lo(x)*hi(w) + hi(x)*lo(w),  hi = cvt.rna.tf32(v), lo = cvt.rna.tf32(v - hi).
-// It replaces cuBLASLt's BF16x9 path (100 us GEMM + 97 us inf/nan scan + 6.5 us bias/ReLU at B = 65536).
+// as hand-written sm_90a kernels with fp32-equivalent accuracy: mma.sync m16n8k8 TF32 with the 3xTF32 split
+//     x*w ~= hi(x)*hi(w) + lo(x)*hi(w) + hi(x)*lo(w),  hi = cvt.rna.tf32(v), lo = cvt.rna.tf32(v - hi),
+// fed by TMA (SWIZZLE_128B boxes) through a ring of shared-memory stages guarded by mbarriers.
 //
-// Structure (one CTA per SM, persistent over 128-row tiles, 192 threads):
-//   warp 0      TMA producer: per K-chunk of 32 columns, X[128x32] -> smem (SWIZZLE_128B), W_hi / W_lo[64x32] -> smem
-//   warp 1      MMA issuer (one elected lane) + TMEM allocation: per chunk 4 k-steps x 3 products into a
-//               128 x 64 fp32 accumulator in TMEM; two accumulators so the epilogue overlaps the next tile
-//   warps 2..5  transform: rewrite the landed X chunk in place as hi and write lo to a second buffer (same swizzled
-//               addresses -> no layout knowledge needed), fence.proxy.async, signal the MMA warp;
-//               epilogue: tcgen05.ld (warp w owns TMEM lanes 32*(w%4)..), + bias, ReLU, coalesced-enough row stores
-// Barriers per stage: full (TMA -> transform), ready (transform -> MMA), empty (MMA commit -> TMA);
-// per accumulator: acc_full (MMA commit -> epilogue), acc_empty (epilogue -> MMA).
+// Forward / input gradient (gemm3x_kernel, 256 threads, one 128 x BN output tile per CTA):
+//   thread 0    issues the TMA loads of a K-chunk (X[128x32], W_hi / W_lo[BNx32]) STAGES chunks ahead
+//   warp w      rows 16w .. 16w+15 of the tile, all BN columns: splits its X fragments into hi / lo in registers
+//               (W arrives split: split_w_kernel), three MMAs per k-step, then bias, ReLU and the stores
+// The tensor core's fp32 accumulation is not round-to-nearest, and the error grows with the number of accumulations
+// into one register: the three products of every k-step are accumulated into fresh registers and added to the running
+// sum in fp32 round-to-nearest.
 //
-// GPU tests: tests/test_kernels_gpu.py (test_gemm3x_kernels_match_fp64, test_wide_layer_on_tcgen05_matches_fp64)
+// GPU tests: tests/test_kernels_gpu.py (test_gemm3x_kernels_match_fp64, test_wide_layer_on_tcgen05_matches_fp64);
+// the same source runs on the CPU under tests/native/sm90_cpu_emu.h (tests/test_gemm3x_emu.py).
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 
-#include "tzk_umma_desc.h"
 #ifdef TZK_CPU_SHIM
 #include "cuda_cpu_shim.h"      // (tests/native, -I) host execution for tests/test_gemm3x_emu.py:
-#include "tcgen05_cpu_emu.h"    // TMA / tcgen05 / mbarrier / TMEM emulated from their documented semantics
+#include "sm90_cpu_emu.h"       // TMA / mbarrier / mma.sync emulated from their documented semantics
 #else
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -35,296 +33,144 @@
 
 namespace {
 #ifndef TZK_CPU_SHIM
-#include "tzk_tcgen05_ptx.h"
+#include "tzk_sm90_ptx.h"
 #endif
 
+constexpr int BM = 128;          // rows per output tile
 constexpr int BK = 32;           // K-chunk: 32 floats = one 128-B swizzled row
-constexpr int UK = 8;            // UMMA K for tf32 (32 bytes)
 constexpr int X_BYTES = BM * BK * 4;       // 16 KB
-constexpr int NUM_THREADS = 192;
-// BN = output columns per tile (UMMA N, multiple of 16, <= 128): 64 for the forward pass (N = 64), 112 for the
-// input-gradient pass (N = 784 = 7 x 112).  Per stage: X(hi) | X lo | W hi | W lo, each buffer 1024-B aligned.
+constexpr int NUM_THREADS = 256;
+// BN = output columns per tile: 64 for the forward pass (N = 64), 56 for the input-gradient pass (N = 784 = 14 x 56).
+// Per stage: X | W hi | W lo, each buffer 1024-B aligned (BN x 128 B is a multiple of 1 KB for both).  Three stages
+// (96 / 90 KB) leave room for two CTAs per SM.
 template <int BN>
 struct Cfg {
   static constexpr int W_BYTES = BN * BK * 4;
-  static constexpr int W_PAD = (W_BYTES + 1023) / 1024 * 1024;
-  static constexpr int STAGE_BYTES = 2 * X_BYTES + 2 * W_PAD;
-  // The tensor core rounds its fp32 accumulator TOWARD ZERO on every MMA (measured: 2.2e-5 max error over K = 784 with
-  // one accumulator, against 2.6e-6 for round-to-nearest).  The bias grows with the number of accumulations into one
-  // large accumulator, so (i) the small products (lo*hi, hi*lo) get an accumulator of their own — their truncation is
-  // relative to their own tiny magnitude — and (ii) the hi*hi products of a tile are spread over P partial
-  // accumulators, each covering 1/P of K, which the epilogue adds in fp32 round-to-nearest.  All of TMEM is used:
-  // 2 tiles in flight x (P + 1) x BN columns  (stacked: 2 x P x 2 BN, partial p = [hi*hi | small terms]).
-  static constexpr int P = BN <= 64 ? 3 : 1;
-  static constexpr int P_STACKED = BN <= 64 ? 2 : 1;
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int STAGES = BN <= 64 ? 4 : 3;          // 4 x 48 KB / 3 x 60 KB of shared memory
+  static constexpr int STAGE_BYTES = X_BYTES + 2 * W_BYTES;
+  static constexpr int STAGES = 3;
+  static_assert(W_BYTES % 1024 == 0, "SWIZZLE_128B boxes need 1 KB alignment");
 };
 
-__device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
-
 struct Params {
-  const float* bias;   // [64] or NULL
+  const float* bias;   // [N] or NULL
   float* y;            // [M, ld_y]
   int64_t ld_y;
   int64_t M;
-  int K;               // multiple of 32 after padding (the caller's X / W carry zero columns up to it)
+  int K;               // multiple of 32 after padding (TMA reads the columns past the tensor as zeros)
   int N;               // output columns (multiple of BN)
   int relu;
 };
 
-// STACK: W_hi and W_lo lie back to back in shared memory (whole 8-row groups), so hi(x) * [W_hi ; W_lo] is ONE MMA with
-// N = 2 * BN (columns [0, BN) collect hi*hi, columns [BN, 2 BN) hi*lo) and lo(x) * W_hi a second one with N = BN into
-// the first half; the epilogue adds the halves.  Two MMAs and 14 KB of operand reads per k-step instead of three and
-// 18 KB — at N = 64 the MMA is bound by operand reads, not flops.
-// TW = transform / epilogue warps (4 or 8; TZK_GEMM3X_TW): two warps share a TMEM lane quarter when TW = 8 and split the
-// tile's column groups between them.
-// RAW (TZK_GEMM3X_RAW=1): the hi operands are the raw fp32 tensors themselves — kind::tf32 ignores the low 13 mantissa
-// bits, so the hardware multiplies trunc(x) — and only lo = rna(x - trunc(x)) is computed and stored (one shared-memory
-// write stream and one conversion per element less).  If the hardware rounded instead of truncating, the error would
-// jump to ~1e-3: the accuracy tests decide.
-// SPLIT (TZK_GEMM3X_SPLIT=1): four dedicated epilogue warps after the TW transform warps, so that draining tile i (TMEM ->
-// registers -> global, the dominant cost of the input-gradient pass) overlaps the transform + MMA work of tile i+1 —
-// which is what the two accumulator sets are for; without it the same warps do both, one after the other.
-// PF (TZK_GEMM3X_PREFETCH=1): the producer asks L2 for the X boxes PF_DIST chunks ahead (cp.async.bulk.prefetch.tensor).
-// The first hardware numbers (same ~0.9 us per 16-KB chunk in the forward and the weight-gradient pass, 2.6 TB/s) are
-// what four 16-KB stages in flight per SM give at an HBM -> shared-memory latency of ~3.7 us (Little's law); shared
-// memory for deeper stages is gone, the 126 MB L2 is not.
-constexpr int PF_DIST = 12;
-template <int BN, bool STACK, int TW, bool RAW, bool SPLIT, bool PF>
-__global__ void __launch_bounds__(64 + 32 * TW + (SPLIT ? 128 : 0), 1)
+// element (row, col) of a [rows x 32 floats] SWIZZLE_128B box: the 16-B chunk index is XOR-ed with row % 8
+__device__ __forceinline__ int swz(int row, int col) { return row * 32 + ((((col >> 2) ^ row) & 7) << 2) + (col & 3); }
+
+template <int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 2)
 gemm3x_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
               const __grid_constant__ CUtensorMap map_wlo, Params p) {
-  constexpr int W_BYTES = Cfg<BN>::W_BYTES, W_PAD = Cfg<BN>::W_PAD, STAGE_BYTES = Cfg<BN>::STAGE_BYTES;
-  constexpr int TMEM_COLS = Cfg<BN>::TMEM_COLS, STAGES = Cfg<BN>::STAGES;
-  constexpr int P = STACK ? Cfg<BN>::P_STACKED : Cfg<BN>::P;          // partial accumulators of the hi*hi products
-  constexpr int ACC_COLS = STACK ? P * 2 * BN : (P + 1) * BN;         // TMEM columns per tile in flight
-  static_assert(2 * ACC_COLS <= TMEM_COLS, "two tiles in flight must fit TMEM");
-  static_assert(!STACK || W_PAD == W_BYTES, "stacked B needs W_hi and W_lo contiguous");
+  constexpr int W_BYTES = Cfg<BN>::W_BYTES, STAGE_BYTES = Cfg<BN>::STAGE_BYTES, STAGES = Cfg<BN>::STAGES;
+  constexpr int NT = BN / 8;                       // n8 tiles per warp
   TZK_DYN_SMEM(uint8_t, smem);
-  uint8_t* stage_base = smem;                                        // STAGES x 48 KB, each buffer 1024-B aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full = bars;                 // [STAGES] TMA -> transform   (1 arrival + tx bytes)
-  uint64_t* ready = bars + STAGES;       // [STAGES] transform -> MMA   (4 arrivals: one per transform warp)
-  uint64_t* empty = bars + 2 * STAGES;   // [STAGES] MMA -> TMA         (1 arrival via tcgen05.commit)
-  uint64_t* acc_full = bars + 3 * STAGES;        // [2] MMA -> epilogue
-  uint64_t* acc_empty = bars + 3 * STAGES + 2;   // [2] epilogue -> MMA (4 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * STAGES + 4);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES] TMA -> all warps
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int n_tiles = p.N / BN;                    // n fastest: the X rows of a row tile are re-read from L2
+  const int64_t m0 = (int64_t)(blockIdx.x / n_tiles) * BM;
+  const int col0 = (int)(blockIdx.x % n_tiles) * BN;
   const int num_k = p.K / BK;
-  const int n_used = num_k < P ? num_k : P;                // partials that receive at least one chunk
-  const int n_tiles = p.N / BN;                            // a tile = (128 rows) x (BN columns); n fastest so that the
-  const int64_t num_tiles = (p.M + BM - 1) / BM * n_tiles; // X rows of an m-tile are re-read from L2, not from HBM
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full + s, 1);
-      mbar_init(ready + s, TW);
-      mbar_init(empty + s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(acc_full + a, 1);
-      mbar_init(acc_empty + a, SPLIT ? 4 : TW);
-    }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) mbar_init(full + s, 1);
     fence_mbarrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  auto load = [&](int kb) {                        // thread 0 only
+    uint8_t* sb = smem + (kb % STAGES) * STAGE_BYTES;
+    uint64_t* bar = full + kb % STAGES;
+    mbar_expect_tx(bar, X_BYTES + 2 * W_BYTES);
+    tma_load_2d(sb, &map_x, bar, kb * BK, (int)m0);
+    tma_load_2d(sb + X_BYTES, &map_whi, bar, kb * BK, col0);
+    tma_load_2d(sb + X_BYTES + W_BYTES, &map_wlo, bar, kb * BK, col0);
+  };
+  if (threadIdx.x == 0)
+    for (int kb = 0; kb < STAGES && kb < num_k; ++kb) load(kb);
 
-  if (warp == 0) {
-    // ===== TMA producer ======================================================================================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      auto load_chunk = [&](int64_t t, int kb) {
-        mbar_wait(empty + stage, phase ^ 1);
-        uint8_t* sb = stage_base + stage * STAGE_BYTES;
-        mbar_expect_tx(full + stage, X_BYTES + 2 * W_BYTES);   // W_BYTES, not W_PAD: the box is BN rows
-        tma_load_2d(sb, &map_x, full + stage, kb * BK, (int)(t / n_tiles * BM));
-        tma_load_2d(sb + 2 * X_BYTES, &map_whi, full + stage, kb * BK, (int)(t % n_tiles) * BN);
-        tma_load_2d(sb + 2 * X_BYTES + W_PAD, &map_wlo, full + stage, kb * BK, (int)(t % n_tiles) * BN);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      };
-      if constexpr (PF) {
-        int64_t pt = blockIdx.x;                // prefetch cursor: (tile, k-block) PF_DIST chunks ahead of the loads
-        int pkb = 0;
-        auto prefetch_next = [&] {
-          if (pt < num_tiles) {
-            tma_prefetch_2d(&map_x, pkb * BK, (int)(pt / n_tiles * BM));
-            if (++pkb == num_k) { pkb = 0; pt += gridDim.x; }
-          }
-        };
-        for (int i = 0; i < PF_DIST; ++i) prefetch_next();
-        for (int64_t t = blockIdx.x; t < num_tiles; t += gridDim.x)
-          for (int kb = 0; kb < num_k; ++kb) {
-            prefetch_next();
-            load_chunk(t, kb);
-          }
-      } else {
-        for (int64_t t = blockIdx.x; t < num_tiles; t += gridDim.x)
-          for (int kb = 0; kb < num_k; ++kb) load_chunk(t, kb);
+  const int r = warp * 16 + g;                     // this lane's rows r and r + 8 (both have row % 8 == g)
+  float acc[NT][4], part[NT][4];
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[nt][q] = 0.f;
+  for (int kb = 0; kb < num_k; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(full + s, (uint32_t)(kb / STAGES) & 1u);
+    const float* xs = reinterpret_cast<const float*>(smem + s * STAGE_BYTES);
+    const uint32_t* whi = reinterpret_cast<const uint32_t*>(smem + s * STAGE_BYTES + X_BYTES);
+    const uint32_t* wlo = whi + W_BYTES / 4;
+#pragma unroll
+    for (int ks = 0; ks < BK / 8; ++ks) {
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) part[nt][q] = 0.f;
+      const int k0 = ks * 8 + t, k1 = k0 + 4;
+      const float a[4] = {xs[swz(r, k0)], xs[swz(r + 8, k0)], xs[swz(r, k1)], xs[swz(r + 8, k1)]};
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        ah[i] = tf32_bits(a[i]);
+        al[i] = tf32_bits(a[i] - __uint_as_float(ah[i]));
       }
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt) {
+        const int n = nt * 8 + g;
+        const uint32_t bh[2] = {whi[swz(n, k0)], whi[swz(n, k1)]};
+        const uint32_t bl[2] = {wlo[swz(n, k0)], wlo[swz(n, k1)]};
+        mma_tf32(part[nt], al, bh);                // small terms first
+        mma_tf32(part[nt], ah, bl);
+        mma_tf32(part[nt], ah, bh);
+      }
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[nt][q] += part[nt][q];
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer ==========================================================================================
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    constexpr uint32_t idesc = make_idesc<BN>();
-    constexpr uint32_t idesc2 = make_idesc<2 * BN>();    // STACK only
-    for (int64_t t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait_all(acc_empty + acc, acc_phase ^ 1);      // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-      uint32_t started = 0;                           // bit p: partial p holds data of this tile (bit P: the small terms)
-      for (int kb = 0; kb < num_k; ++kb) {
-        mbar_wait_all(ready + stage, phase);              // hi / lo of this chunk are in shared memory
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sb = smem_u32(stage_base + stage * STAGE_BYTES);
-          const uint32_t a_hi = sb, a_lo = sb + X_BYTES, b_hi = sb + 2 * X_BYTES, b_lo = b_hi + W_PAD;
-          const int part = kb * n_used / num_k;       // this chunk's partial accumulator
+    __syncthreads();                               // every warp is done with stage s: refill it
+    if (threadIdx.x == 0 && kb + STAGES < num_k) load(kb + STAGES);
+  }
+
+  // ---- epilogue: c0/c1 row r, columns 2t, 2t+1 of the n8 tile; c2/c3 row r + 8 --------------------------------------
 #pragma unroll
-          for (int k = 0; k < BK / UK; ++k) {
-            const uint32_t ko = k * UK * 4;           // 32 B per k-step inside the 128-B swizzled row
-            const uint32_t more = (started >> part) & 1u;
-            if (STACK) {
-              const uint32_t region = d_tmem + part * 2 * BN;     // [hi*hi | hi*lo + lo*hi]
-              mma_tf32(region, make_desc(a_hi + ko), make_desc(b_hi + ko), idesc2, more);   // B = [W_hi ; W_lo]
-              mma_tf32(region + BN, make_desc(a_lo + ko), make_desc(b_hi + ko), idesc, 1u);
-            } else {
-              const uint32_t small = d_tmem + P * BN;
-              mma_tf32(d_tmem + part * BN, make_desc(a_hi + ko), make_desc(b_hi + ko), idesc, more);
-              mma_tf32(small, make_desc(a_lo + ko), make_desc(b_hi + ko), idesc, (started >> P) & 1u);
-              mma_tf32(small, make_desc(a_hi + ko), make_desc(b_lo + ko), idesc, 1u);
-            }
-            started |= (1u << part) | (1u << P);
-          }
-          tc_commit(empty + stage);                    // shared-memory slot is free once these MMAs retire
-          if (kb == num_k - 1) tc_commit(acc_full + acc);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  for (int nt = 0; nt < NT; ++nt) {
+    const int col = col0 + nt * 8 + 2 * t;
+    const float b0 = p.bias ? __ldg(p.bias + col) : 0.f, b1 = p.bias ? __ldg(p.bias + col + 1) : 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = m0 + r + 8 * h;
+      if (row >= p.M) continue;
+      float2 o = make_float2(acc[nt][2 * h] + b0, acc[nt][2 * h + 1] + b1);
+      if (p.relu) {
+        o.x = fmaxf(o.x, 0.f);
+        o.y = fmaxf(o.y, 0.f);
       }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else {
-    // ===== transform warps (2 .. 2+TW-1) and epilogue warps (the same ones, or with SPLIT the four after them) ==========
-    const int tw = warp - 2;                 // 0..TW-1 transform; TW..TW+3 epilogue-only (SPLIT)
-    const int quarter = warp & 3;            // TMEM lane quarter this warp may read
-    const bool do_transform = !SPLIT || tw < TW;
-    const bool do_epilogue = !SPLIT || tw >= TW;
-    const int part0 = SPLIT ? 0 : tw / 4, part_step = SPLIT ? 1 : TW / 4;
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int64_t t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      for (int kb = 0; do_transform && kb < num_k; ++kb) {
-        mbar_wait_all(full + stage, phase);
-        float4* hi = reinterpret_cast<float4*>(stage_base + stage * STAGE_BYTES);
-        float4* lo = reinterpret_cast<float4*>(stage_base + stage * STAGE_BYTES + X_BYTES);
-        // 1024 float4 per X chunk over the TW * 32 transform threads; element-wise, so the swizzle is irrelevant
-#pragma unroll
-        for (int q = 0; q < X_BYTES / 16 / (TW * 32); ++q) {
-          const int i = q * (TW * 32) + tw * 32 + lane;
-          const float4 x = hi[i];
-          float4 h, l;
-          if (RAW) {
-            h.x = tf32_trunc(x.x); h.y = tf32_trunc(x.y); h.z = tf32_trunc(x.z); h.w = tf32_trunc(x.w);
-          } else {
-            h.x = tf32_rna(x.x); h.y = tf32_rna(x.y); h.z = tf32_rna(x.z); h.w = tf32_rna(x.w);
-          }
-          l.x = tf32_rna(x.x - h.x); l.y = tf32_rna(x.y - h.y); l.z = tf32_rna(x.z - h.z); l.w = tf32_rna(x.w - h.w);
-          if (!RAW) hi[i] = h;
-          lo[i] = l;
-        }
-        fence_proxy_async();   // generic-proxy writes -> visible to the MMA
-        __syncwarp();
-        if (lane == 0) mbar_arrive(ready + stage);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      // ---- epilogue of this tile ---------------------------------------------------------------------------
-      if (!do_epilogue) continue;
-      mbar_wait_all(acc_full + acc, acc_phase);
-      tc_fence_after();
-      const int64_t row = t / n_tiles * BM + quarter * 32 + lane;
-      const int col0 = (int)(t % n_tiles) * BN;
-      const uint32_t taddr = tmem_base + acc * ACC_COLS + ((uint32_t)(quarter * 32) << 16);
-      float v[16];
-#pragma unroll
-      for (int part = part0; part < BN / 16; part += part_step) {   // TW = 8 without SPLIT: the two warps of a lane quarter alternate
-        // small terms first, then the partials (fp32 round-to-nearest adds)
-        float v2[16];
-        if (STACK) {
-          tmem_ld16(taddr + BN + part * 16, v);
-          for (int q = 1; q < n_used; ++q) {
-            tmem_ld16(taddr + q * 2 * BN + BN + part * 16, v2);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) v[c] += v2[c];
-          }
-          for (int q = 0; q < n_used; ++q) {
-            tmem_ld16(taddr + q * 2 * BN + part * 16, v2);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) v[c] += v2[c];
-          }
-        } else {
-          tmem_ld16(taddr + P * BN + part * 16, v);
-          for (int q = 0; q < n_used; ++q) {
-            tmem_ld16(taddr + q * BN + part * 16, v2);
-#pragma unroll
-            for (int c = 0; c < 16; ++c) v[c] += v2[c];
-          }
-        }
-        if (row < p.M) {
-          float* yr = p.y + row * p.ld_y + col0 + part * 16;
-#pragma unroll
-          for (int c = 0; c < 16; c += 4) {
-            float4 o;
-            o.x = v[c] + (p.bias ? __ldg(p.bias + col0 + part * 16 + c) : 0.f);
-            o.y = v[c + 1] + (p.bias ? __ldg(p.bias + col0 + part * 16 + c + 1) : 0.f);
-            o.z = v[c + 2] + (p.bias ? __ldg(p.bias + col0 + part * 16 + c + 2) : 0.f);
-            o.w = v[c + 3] + (p.bias ? __ldg(p.bias + col0 + part * 16 + c + 3) : 0.f);
-            if (p.relu) {
-              o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-            }
-            *reinterpret_cast<float4*>(yr + c) = o;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty + acc);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
+      *reinterpret_cast<float2*>(p.y + row * p.ld_y + col) = o;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_free(tmem_base, TMEM_COLS);
 }
 
 // ======================================================================================================================
 // Weight gradient of the same layer:  dW[n, k] = sum_m dZ[m, n] * X[m, k]   (n < 64, k < K = 784, m < M = batch).
-// The reduction runs over the batch, so both operands are MN-major as they lie in memory: A = X^T (UMMA M = 128 of
-// X's columns), B = dZ^T (UMMA N = 64) — for 32-bit elements that means the SWIZZLE_128B_BASE32B shared-memory layout
-// (TMA: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B; see tzk_umma_desc.h), 4-row k groups 512 B apart.  Work item = (column tile j of 128, row slab s); each CTA owns one item, streams
-// its slab in chunks of 32 rows (4 k-steps of 8), and writes a partial [128 x 64] block; wgrad_reduce_kernel adds the
-// slabs in a fixed order and transposes into dW[64, K].  X is read exactly once over all items (tiles read disjoint
-// columns); dZ is re-read by the 7 column tiles from L2.
-// Per stage: A hi (4 boxes of 32 rows x 128 B = 16 KB) | A lo | B hi (2 boxes = 8 KB) | B lo.
+// Work item = (column tile j of 128 X columns, row slab s); each CTA owns one item and computes the [64 x 128] block
+// dZ[slab]^T X[slab, tile] with A = dZ^T and B = X straight from the row-major boxes, streaming the slab in chunks of
+// 32 rows (4 k-steps of 8).  Warp w: n rows 16 (w % 4) .. +16, X columns 64 (w / 4) .. +64.  The partial block goes to
+// `partial`; wgrad_reduce_kernel adds the slabs in a fixed order and transposes into dW[64, K].  X is read exactly once
+// over all items (tiles read disjoint columns); dZ is re-read by the 7 column tiles from L2.
+// Per stage: X (4 boxes of 32 rows x 128 B = 16 KB) | dZ (2 boxes = 8 KB).
 constexpr int WG_ROWS = 32;                         // batch rows per chunk = 4 k-steps
 constexpr int WG_BOX = WG_ROWS * 128;               // one TMA box: 32 rows x 32 floats = 4 KB
 constexpr int WG_A = 4 * WG_BOX, WG_B = 2 * WG_BOX; // 16 KB, 8 KB
-constexpr int WG_STAGE = 2 * WG_A + 2 * WG_B;       // 48 KB
-constexpr int WG_STAGES = 4;
-constexpr int WG_P = 7;                             // partial accumulators (see Cfg): 7 x 64 + 64 small-term columns = all of TMEM
+constexpr int WG_STAGE = WG_A + WG_B;               // 24 KB
+constexpr int WG_STAGES = 4;                        // 96 KB: two CTAs per SM
 
 struct WgParams {
   float* partial;      // [slabs, k_tiles * 128, 64]
@@ -333,147 +179,93 @@ struct WgParams {
   int k_tiles;         // ceil(K / 128)
 };
 
-template <bool PF>      // PF: L2 prefetch of the X / dZ boxes PF_DIST chunks ahead (TZK_GEMM3X_PREFETCH=1), see gemm3x_kernel
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(NUM_THREADS, 2)
 wgrad3x_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_dz, WgParams p) {
   TZK_DYN_SMEM(uint8_t, smem);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE);
-  uint64_t* full = bars;                    // TMA -> transform
-  uint64_t* ready = bars + WG_STAGES;       // transform -> MMA (4 arrivals)
-  uint64_t* empty = bars + 2 * WG_STAGES;   // MMA -> TMA
-  uint64_t* acc_full = bars + 3 * WG_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * WG_STAGES + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int jt = blockIdx.x % p.k_tiles;                  // column tile of X
   const int64_t slab = blockIdx.x / p.k_tiles;
   const int64_t row0 = slab * p.slab_rows;
   const int64_t rows = (p.M - row0 < p.slab_rows) ? p.M - row0 : p.slab_rows;
   const int num_c = (int)((rows + WG_ROWS - 1) / WG_ROWS);  // rows past M are zero-filled by the TMA
-  const int n_used = num_c < WG_P ? num_c : WG_P;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) {
-      mbar_init(full + s, 1);
-      mbar_init(ready + s, 4);
-      mbar_init(empty + s, 1);
-    }
-    mbar_init(acc_full, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < WG_STAGES; ++s) mbar_init(full + s, 1);
     fence_mbarrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  auto load = [&](int c) {                                // thread 0 only
+    uint8_t* sb = smem + (c % WG_STAGES) * WG_STAGE;
+    uint64_t* bar = full + c % WG_STAGES;
+    const int r = (int)(row0 + (int64_t)c * WG_ROWS);
+    mbar_expect_tx(bar, WG_A + WG_B);
+#pragma unroll
+    for (int b = 0; b < 4; ++b) tma_load_2d(sb + b * WG_BOX, &map_x, bar, jt * 128 + b * 32, r);
+#pragma unroll
+    for (int b = 0; b < 2; ++b) tma_load_2d(sb + WG_A + b * WG_BOX, &map_dz, bar, b * 32, r);
+  };
+  if (threadIdx.x == 0)
+    for (int c = 0; c < WG_STAGES && c < num_c; ++c) load(c);
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      if constexpr (PF) {
-        for (int c = 0; c < PF_DIST && c < num_c; ++c) {
-          const int r = (int)(row0 + (int64_t)c * WG_ROWS);
-          for (int b = 0; b < 4; ++b) tma_prefetch_2d(&map_x, jt * 128 + b * 32, r);
-          for (int b = 0; b < 2; ++b) tma_prefetch_2d(&map_dz, b * 32, r);
+  const int n0 = (warp & 3) * 16 + g;                     // this lane's n rows n0 and n0 + 8
+  const int kc0 = (warp >> 2) * 64 + g;                   // this lane's X column in n8 tile nt: kc0 + 8 nt
+  float acc[8][4], part[8][4];
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[nt][q] = 0.f;
+  for (int c = 0; c < num_c; ++c) {
+    const int s = c % WG_STAGES;
+    mbar_wait(full + s, (uint32_t)(c / WG_STAGES) & 1u);
+    const float* xs = reinterpret_cast<const float*>(smem + s * WG_STAGE);
+    const float* zs = reinterpret_cast<const float*>(smem + s * WG_STAGE + WG_A);
+    // element (m, col) of a [32 rows x 128 floats] operand held as 32-column boxes
+    auto at = [](const float* base, int m, int col) { return base[(col >> 5) * (WG_BOX / 4) + swz(m, col & 31)]; };
+#pragma unroll
+    for (int ks = 0; ks < WG_ROWS / 8; ++ks) {
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) part[nt][q] = 0.f;
+      const int m = ks * 8 + t;                           // batch rows m (a0, a1, b0) and m + 4 (a2, a3, b1)
+      const float a[4] = {at(zs, m, n0), at(zs, m, n0 + 8), at(zs, m + 4, n0), at(zs, m + 4, n0 + 8)};
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        ah[i] = tf32_bits(a[i]);
+        al[i] = tf32_bits(a[i] - __uint_as_float(ah[i]));
+      }
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const float b[2] = {at(xs, m, kc0 + 8 * nt), at(xs, m + 4, kc0 + 8 * nt)};
+        uint32_t bh[2], bl[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          bh[i] = tf32_bits(b[i]);
+          bl[i] = tf32_bits(b[i] - __uint_as_float(bh[i]));
         }
+        mma_tf32(part[nt], al, bh);
+        mma_tf32(part[nt], ah, bl);
+        mma_tf32(part[nt], ah, bh);
       }
-      for (int c = 0; c < num_c; ++c) {
-        if constexpr (PF) {
-          if (c + PF_DIST < num_c) {
-            const int r = (int)(row0 + (int64_t)(c + PF_DIST) * WG_ROWS);
-            for (int b = 0; b < 4; ++b) tma_prefetch_2d(&map_x, jt * 128 + b * 32, r);
-            for (int b = 0; b < 2; ++b) tma_prefetch_2d(&map_dz, b * 32, r);
-          }
-        }
-        mbar_wait(empty + stage, phase ^ 1);
-        uint8_t* sb = smem + stage * WG_STAGE;
-        mbar_expect_tx(full + stage, WG_A + WG_B);
-        const int r = (int)(row0 + (int64_t)c * WG_ROWS);
 #pragma unroll
-        for (int b = 0; b < 4; ++b) tma_load_2d(sb + b * WG_BOX, &map_x, full + stage, jt * 128 + b * 32, r);
+      for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
-        for (int b = 0; b < 2; ++b) tma_load_2d(sb + 2 * WG_A + b * WG_BOX, &map_dz, full + stage, b * 32, r);
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
+        for (int q = 0; q < 4; ++q) acc[nt][q] += part[nt][q];
     }
-  } else if (warp == 1) {
-    int stage = 0;
-    uint32_t phase = 0;
-    constexpr uint32_t idesc = make_idesc<64, true>();
-    uint32_t started = 0;
-    for (int c = 0; c < num_c; ++c) {
-      mbar_wait_all(ready + stage, phase);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t sb = smem_u32(smem + stage * WG_STAGE);
-        const uint32_t a_hi = sb, a_lo = sb + WG_A, b_hi = sb + 2 * WG_A, b_lo = b_hi + WG_B;
-        const int part = c * n_used / num_c;
-        const uint32_t d_main = tmem_base + part * 64, d_small = tmem_base + WG_P * 64;
-#pragma unroll
-        for (int k = 0; k < WG_ROWS / UK; ++k) {
-          const uint32_t ko = k * 1024;             // next group of 8 batch rows inside every box
-          mma_tf32(d_main, make_desc_mn(a_hi + ko, WG_BOX, 512), make_desc_mn(b_hi + ko, WG_BOX, 512), idesc,
-                   (started >> part) & 1u);
-          mma_tf32(d_small, make_desc_mn(a_lo + ko, WG_BOX, 512), make_desc_mn(b_hi + ko, WG_BOX, 512), idesc,
-                   (started >> WG_P) & 1u);
-          mma_tf32(d_small, make_desc_mn(a_hi + ko, WG_BOX, 512), make_desc_mn(b_lo + ko, WG_BOX, 512), idesc, 1u);
-          started |= (1u << part) | (1u << WG_P);
-        }
-        tc_commit(empty + stage);
-        if (c == num_c - 1) tc_commit(acc_full);
-      }
-      __syncwarp();
-      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-    }
-  } else {
-    const int tw = warp - 2, quarter = warp & 3;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int c = 0; c < num_c; ++c) {
-      mbar_wait_all(full + stage, phase);
-      uint8_t* sb = smem + stage * WG_STAGE;
-      // A: 1024 float4 (hi at +0, lo at +WG_A); B: 512 float4 (hi at +2*WG_A, lo at +2*WG_A+WG_B); element-wise.
-#pragma unroll
-      for (int q = 0; q < (WG_A + WG_B) / 16 / 128; ++q) {
-        const int i = q * 128 + tw * 32 + lane;                       // 0..1535
-        float4* hi = reinterpret_cast<float4*>(i < WG_A / 16 ? sb : sb + 2 * WG_A) + (i < WG_A / 16 ? i : i - WG_A / 16);
-        float4* lo = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(hi) + (i < WG_A / 16 ? WG_A : WG_B));
-        const float4 x = *hi;
-        float4 h, l;
-        h.x = tf32_rna(x.x); h.y = tf32_rna(x.y); h.z = tf32_rna(x.z); h.w = tf32_rna(x.w);
-        l.x = tf32_rna(x.x - h.x); l.y = tf32_rna(x.y - h.y); l.z = tf32_rna(x.z - h.z); l.w = tf32_rna(x.w - h.w);
-        *hi = h;
-        *lo = l;
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(ready + stage);
-      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-    }
-    // epilogue: TMEM lane = X column inside the tile, TMEM column = n
-    mbar_wait_all(acc_full, 0);
-    tc_fence_after();
-    const int krow = jt * 128 + quarter * 32 + lane;
-    float* out = p.partial + ((int64_t)slab * p.k_tiles * 128 + krow) * 64;
-    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    float v[16], v2[16];
-#pragma unroll
-    for (int part = 0; part < 4; ++part) {
-      tmem_ld16(taddr + WG_P * 64 + part * 16, v);          // small terms first, then the partials
-      for (int q = 0; q < n_used; ++q) {
-        tmem_ld16(taddr + q * 64 + part * 16, v2);
-#pragma unroll
-        for (int c = 0; c < 16; ++c) v[c] += v2[c];
-      }
-#pragma unroll
-      for (int c = 0; c < 16; c += 4)
-        *reinterpret_cast<float4*>(out + part * 16 + c) = make_float4(v[c], v[c + 1], v[c + 2], v[c + 3]);
-    }
+    __syncthreads();
+    if (threadIdx.x == 0 && c + WG_STAGES < num_c) load(c + WG_STAGES);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_free(tmem_base, 512);
+  // c0/c1: n row n0, X columns 2t, 2t+1 of the n8 tile; c2/c3: n row n0 + 8
+  float* out = p.partial + ((int64_t)slab * p.k_tiles + jt) * 128 * 64;
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    const int kcol = (warp >> 2) * 64 + nt * 8 + 2 * t;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) out[(int64_t)(kcol + (q & 1)) * 64 + n0 + 8 * (q >> 1)] = acc[nt][q];
+  }
 }
 
 // dW[n, k] = sum over slabs (fixed order) of partial[s, k, n]; one thread per (k, n), n fastest for the reads
@@ -489,10 +281,8 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int slabs
 
 // ---- host: tensor maps -------------------------------------------------------------------------------------
 #ifdef TZK_CPU_SHIM
-int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
-             bool atom32 = false) {
+int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
   map->base = base; map->rows = rows; map->cols = cols; map->ld = ld; map->box_rows = box_rows;
-  map->atom32 = atom32;
   return 0;
 }
 #else
@@ -500,9 +290,8 @@ typedef CUresult (*EncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, v
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// atom32: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B (32-B chunks swizzled) for MN-major 32-bit operands, else SWIZZLE_128B
-int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
-             bool atom32 = false) {
+// box [32 floats x box_rows], SWIZZLE_128B
+int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
   static EncodeTiled encode = nullptr;
   if (!encode) {
     cudaDriverEntryPointQueryResult q;
@@ -515,8 +304,7 @@ int make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, in
   cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS ? 0 : 2;
 }
 #endif
@@ -531,22 +319,18 @@ __global__ void split_w_kernel(const float* __restrict__ w, int64_t n, float* __
 }
 }  // namespace
 
-template <int BN, bool STACK, int TW, bool RAW, bool SPLIT, bool PF>
+template <int BN>
 static int launch(const CUtensorMap& mx, const CUtensorMap& mh, const CUtensorMap& ml, const Params& p, cudaStream_t st) {
-  const size_t smem = (size_t)Cfg<BN>::STAGES * Cfg<BN>::STAGE_BYTES + 256;
-  static int sms = 0;                 // once per instantiation: nothing but the launch happens inside a stream capture
-  if (sms == 0) {
+  const size_t smem = (size_t)Cfg<BN>::STAGES * Cfg<BN>::STAGE_BYTES + 64;
 #ifndef TZK_CPU_SHIM
-    cudaFuncSetAttribute(gemm3x_kernel<BN, STACK, TW, RAW, SPLIT, PF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-#endif
-    int dev = 0, n = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    sms = n > 0 ? n : 148;
+  static bool configured = false;     // once per instantiation: nothing but the launch happens inside a stream capture
+  if (!configured) {
+    cudaFuncSetAttribute(gemm3x_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    configured = true;
   }
+#endif
   const int64_t tiles = (p.M + BM - 1) / BM * (p.N / BN);
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  TZK_LAUNCH((gemm3x_kernel<BN, STACK, TW, RAW, SPLIT, PF>), grid, 64 + 32 * TW + (SPLIT ? 128 : 0), smem, st, mx, mh, ml, p);
+  TZK_LAUNCH((gemm3x_kernel<BN>), (unsigned)tiles, NUM_THREADS, smem, st, mx, mh, ml, p);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
 
@@ -560,23 +344,19 @@ extern "C" int tzk_gemm3x(const float* x, int64_t ld_x, const float* w, int64_t 
   if (M <= 0 || K <= 0 || (ld_x % 4) || (ld_w % 4) || (ld_y % 4)) return 1;
   if (N != 64 && N % 112 != 0) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int BN = N == 64 ? 64 : 112;
+  const int BN = N == 64 ? 64 : 56;
   const int64_t nw = (int64_t)N * ld_w;
-  // One configuration is built (measured r2, B = 65536: 3-MMA 93 / 125 us, stacked 80 / 121, stacked + dedicated
-  // epilogue warps 76 / 99 us forward / input gradient; raw-hi, eight transform warps, L2 prefetch and the ring variant
-  // were equal or slower — profiles/r2_gemm3x_variants.txt): stacked W_hi / W_lo, four transform + four epilogue warps.
   TZK_LAUNCH((split_w_kernel), (unsigned)((nw + 255) / 256), 256, 0, st, w, nw, w_hi, w_lo);
   CUtensorMap mx, mh, ml;
   if (make_map(&mx, x, M, K, ld_x, BM) || make_map(&mh, w_hi, N, K, ld_w, BN) || make_map(&ml, w_lo, N, K, ld_w, BN))
     return 2;
   Params p;
   p.bias = bias; p.y = y; p.ld_y = ld_y; p.M = M; p.K = (K + BK - 1) / BK * BK; p.N = N; p.relu = relu;
-  return BN == 64 ? launch<64, true, 4, false, true, false>(mx, mh, ml, p, st)
-                  : launch<112, true, 4, false, true, false>(mx, mh, ml, p, st);
+  return BN == 64 ? launch<64>(mx, mh, ml, p, st) : launch<56>(mx, mh, ml, p, st);
 }
 
 // dw[64, K] = dz[M, 64]^T @ x[M, K]  (3xTF32; fixed-order reduction over `slabs` row slabs -> run-to-run deterministic).
-// partial: scratch of slabs * ceil(K/128)*128 * 64 floats.  slabs <= 0 picks one work item per SM.
+// partial: scratch of slabs * ceil(K/128)*128 * 64 floats.
 extern "C" int64_t tzk_wgrad3x_partial_floats(int32_t K, int32_t slabs) {
   return (int64_t)slabs * ((K + 127) / 128 * 128) * 64;
 }
@@ -585,22 +365,22 @@ extern "C" int tzk_wgrad3x(const float* x, int64_t ld_x, const float* dz, int64_
   if (M <= 0 || K <= 0 || slabs <= 0 || (ld_x % 4) || (ld_dz % 4)) return 1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CUtensorMap mx, mz;
-  if (make_map(&mx, x, M, K, ld_x, WG_ROWS, true) || make_map(&mz, dz, M, 64, ld_dz, WG_ROWS, true)) return 2;
+  if (make_map(&mx, x, M, K, ld_x, WG_ROWS) || make_map(&mz, dz, M, 64, ld_dz, WG_ROWS)) return 2;
   WgParams p;
   p.partial = partial;
   p.M = M;
   p.k_tiles = (K + 127) / 128;
   p.slab_rows = ((M + slabs - 1) / slabs + WG_ROWS - 1) / WG_ROWS * WG_ROWS;
   const int used = (int)((M + p.slab_rows - 1) / p.slab_rows);           // slabs that hold rows (<= slabs)
-  const size_t smem = (size_t)WG_STAGES * WG_STAGE + 256;
+  const size_t smem = (size_t)WG_STAGES * WG_STAGE + 64;
 #ifndef TZK_CPU_SHIM
   static bool configured = false;     // once: nothing but the launches happens inside a stream capture
   if (!configured) {
-    cudaFuncSetAttribute(wgrad3x_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(wgrad3x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     configured = true;
   }
 #endif
-  TZK_LAUNCH((wgrad3x_kernel<false>), used * p.k_tiles, NUM_THREADS, smem, st, mx, mz, p);
+  TZK_LAUNCH((wgrad3x_kernel), used * p.k_tiles, NUM_THREADS, smem, st, mx, mz, p);
   TZK_LAUNCH((wgrad_reduce_kernel), (K * 64 + 255) / 256, 256, 0, st, partial, used, p.k_tiles * 128, K, dw, ld_dw);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }

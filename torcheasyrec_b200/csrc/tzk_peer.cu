@@ -248,8 +248,8 @@ peer_seq_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* 
 // ---- per-step local copy of the small tables ------------------------------------------------------------------------------
 // Most lookups of a Criteo-like workload hit tables of a few thousand rows (18 of 26 features, 69 % of the ids): their
 // shards are a few MB in total, so every rank copies them from the owners once per step — long sequential NVLink reads
-// at ~750 GB/s — and its gather reads those features from local memory; only the big tables' rows cross NVLink as
-// random 64-B reads (~430 GB/s, measured).  Segment s: n[s] floats from rank r[s]'s arena at src[s] to mirror + dst[s].
+// — and its gather reads those features from local memory; only the big tables' rows cross NVLink as
+// random 64-B reads.  Segment s: n[s] floats from rank r[s]'s arena at src[s] to mirror + dst[s].
 __global__ void __launch_bounds__(kThreads)
 peer_mirror_refresh_simple_kernel(const __grid_constant__ Peers tables, const int32_t* __restrict__ seg_rank,
                                   const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
@@ -265,7 +265,7 @@ peer_mirror_refresh_simple_kernel(const __grid_constant__ Peers tables, const in
 
 // The segments cut into chunks of kMirrorChunk floats, chunks dealt round-robin to the CTAs: every thread has
 // kMirrorChunk / (4 * kThreads) independent 16-B NVLink reads in flight (one load in flight per thread — the simple kernel —
-// pays the NVLink round trip once per 16 B and thread: ~100 us for Criteo's 7.7 MB at W = 2).  n_seg <= kMirrorMaxSeg.
+// pays the NVLink round trip once per 16 B and thread).  n_seg <= kMirrorMaxSeg.
 constexpr int kMirrorChunk = 4096;
 constexpr int kMirrorMaxSeg = 4 * kThreads;
 __global__ void __launch_bounds__(kThreads)
@@ -598,7 +598,7 @@ int fill(Peers* dst, const uint64_t* host_ptrs, int W) {
   return 0;
 }
 int grid_for(int64_t work_ctas) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t cap = (int64_t)sms * 8;
@@ -692,7 +692,7 @@ extern "C" int tzk_peer_mirror_refresh(const uint64_t* table_ptrs, int32_t W, co
   if (fill(&t, table_ptrs, W) || n_seg < 0) return 1;
   if (n_seg == 0) return 0;
   if (!seg_rank || !seg_src || !seg_dst || !seg_n || !mirror) return 1;
-  // the chunked kernel is the default (validated on B200: 10.5 us for Criteo's 7.7 MB at W = 2); TZK_PEER_MIRROR_CHUNKED=0:
+  // the chunked kernel is the default; TZK_PEER_MIRROR_CHUNKED=0:
   // one load in flight per thread
   const char* mc = getenv("TZK_PEER_MIRROR_CHUNKED");
   const char* xp = "1";
@@ -715,7 +715,7 @@ extern "C" int tzk_peer_mirror_refresh(const uint64_t* table_ptrs, int32_t W, co
 #ifdef TZK_CPU_SHIM
   const int grid = 3;             // (host emulation: one std::thread per CUDA thread — keep the launch small)
 #else
-  const int grid = 148 * 4;
+  const int grid = 132 * 4;
 #endif
   TZK_LAUNCH((peer_mirror_refresh_kernel), grid, kThreads, (kMirrorMaxSeg + 1 + kThreads) * sizeof(int32_t),
              reinterpret_cast<cudaStream_t>(stream), t, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);

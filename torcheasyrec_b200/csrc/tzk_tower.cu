@@ -68,7 +68,7 @@ __device__ __forceinline__ void store_tile(float* __restrict__ dst, int64_t ld, 
 // ---------------------------------------------------------------------------------------------------
 // forward: y = act(x @ W^T + b)   x [M,K]  W [N,K]  y [M,N]   K, N <= 64
 // One thread per row, no tile staging and no barrier after the weight matrix is in shared memory (a staged-tile
-// variant with three barriers per 128 rows was measured 1.6x slower: 99 vs 61 us over the four DLRM layers).  A thread reads its own row straight from global memory (the 32 rows of a warp are one
+// variant with three barriers per 128 rows was slower over the four DLRM layers).  A thread reads its own row straight from global memory (the 32 rows of a warp are one
 // contiguous 32*K*4-byte span, so every sector that is fetched is fully consumed through L1 over the k loop) and
 // writes its own output row with 16-B stores.  Many independent warps per SM hide the load latency.
 // ---------------------------------------------------------------------------------------------------
@@ -293,7 +293,7 @@ inline int pad_pow(int v, int lo) {  // smallest of {lo, 16, 32, 64} >= v
 }
 inline int bwd_grid(int64_t M) {   // = number of weight-gradient partials; 4 CTAs (16 warps) per SM hide the tile loads
   const int64_t t = ceil_div64(M < 1 ? 1 : M, kTM);
-  return (int)(t < kSmCountB200 * 4 ? t : kSmCountB200 * 4);
+  return (int)(t < kSmCountH100 * 4 ? t : kSmCountH100 * 4);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -363,7 +363,7 @@ extern "C" int tzk_small_linear_fwd(const float* x, int64_t ld_x, const float* w
     const size_t smem_r = ((size_t)K * NP + NP) * sizeof(float);
     const bool vec = (K % 4 == 0) && (ld_x % 4 == 0) && ((uintptr_t)x % 16 == 0);
     const int64_t blocks = ceil_div64(M, kRowThreads);
-    const int grid_r = (int)(blocks < kSmCountB200 * 16 ? blocks : kSmCountB200 * 16);
+    const int grid_r = (int)(blocks < kSmCountH100 * 16 ? blocks : kSmCountH100 * 16);
 #define TZK_SLR(NP_)                                                                                                \
   do {                                                                                                              \
     if (vec)                                                                                                        \

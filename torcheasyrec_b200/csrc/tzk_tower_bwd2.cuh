@@ -22,7 +22,7 @@
 
 namespace tzk_bwd2 {
 constexpr int kThreads = 128;
-constexpr int kSms = 148;
+constexpr int kSms = 132;   // H100 SXM
 
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
@@ -409,7 +409,7 @@ inline bool unvalidated_switch(const char* name) {
   return x && x[0] == '1';
 }
 
-// The dW tile kernel (default; validated on B200: 64->32 at B = 65536 17.5 us against 87 us); TZK_SMALL_LINEAR_DW=0: the
+// The dW tile kernel (default); TZK_SMALL_LINEAR_DW=0: the
 // row-group dW kernel (straight from global memory, U rows in flight per thread).  Read per call.
 inline bool use_dw_tiles() {
   const char* e = getenv("TZK_SMALL_LINEAR_DW");

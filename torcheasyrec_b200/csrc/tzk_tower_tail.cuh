@@ -5,7 +5,7 @@
 //     loss = mean BCE-with-logits(z, label)                                (tzrec/models/rank_model.py:181-262)
 //
 // and, in the same kernel, d loss / d {y1, W1, b1, w2, b2}.  On DLRM-Criteo (64 -> 32 -> 1, B = 65536) the unfused
-// chain is 18 launches and ~140 us of latency-bound kernels around 24 MB of data; here every row is read once.
+// chain is 18 launches of latency-bound kernels around 24 MB of data; here every row is read once.
 //
 // A CTA walks tiles of 128 rows, thread r <-> row r of the tile:
 //   phase 1 (a row per thread, W1 broadcast from shared memory): h, z, the row's loss term, dz = (sigmoid(z) - y) / M,
@@ -23,7 +23,7 @@
 
 namespace tzk_tail {
 constexpr int kRows = 128;       // rows per tile = threads per CTA
-constexpr int kMaxCtas = 148 * 4;
+constexpr int kMaxCtas = 132 * 4;   // 4 CTAs per H100 SM
 
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

@@ -1,9 +1,11 @@
-"""fp32-accurate tensor-core Linear for the dense towers (cuBLASLt 12.9 BF16x9 emulation, csrc/tzk_gemm.cpp).
+"""fp32 Linear for the dense towers: hand-written kernels for the small layers (csrc/tzk_tower.cu) and the wide
+783 -> 64 layer (csrc/tzk_gemm3x.cu), cuBLASLt (csrc/tzk_gemm.cpp) for the rest.
 
 The towers are caller code (plain PyTorch in the reference, tzrec/modules/mlp.py); this only swaps the GEMM
-algorithm: same fp32 inputs/outputs, fp32-equivalent accuracy, tensor cores instead of CUDA cores.  Falls back to
-torch.nn.functional.linear whenever the library, the device or the algorithm is unavailable (set
-TZK_DENSE_GEMM=torch to force the fallback).
+algorithm: same fp32 inputs/outputs, fp32-equivalent accuracy.  cuBLASLt (>= 12.9) is asked for the BF16x9-emulated
+fp32 compute type and for plain fp32 when it offers no algorithm for that; which kernels it runs is its choice per GPU.
+Falls back to torch.nn.functional.linear whenever the library or the device is unavailable (set TZK_DENSE_GEMM=torch to force
+the fallback).
 """
 
 import ctypes
@@ -159,7 +161,7 @@ class _SmallLinearFn(torch.autograd.Function):
 
 # --------------------------------------------------------------------------------------------------------------------
 # The one wide layer (N = 64 outputs, input width a multiple of 112: DLRM's 783-wide final-MLP input travels as
-# [B, 784]) on hand-written tcgen05 3xTF32 kernels (csrc/tzk_gemm3x.cu -> libtzk_gemm3x.so): forward with bias + ReLU
+# [B, 784]) on hand-written TMA + mma.sync 3xTF32 kernels (csrc/tzk_gemm3x.cu -> libtzk_gemm3x.so): forward with bias + ReLU
 # in the epilogue, dgrad on W^T, wgrad with a fixed-order slab reduction.  TZK_GEMM3X=1 selects it.
 # --------------------------------------------------------------------------------------------------------------------
 _G3 = {"lib": None, "tried": False}
@@ -174,7 +176,7 @@ def _gemm3x_lib():
     return _G3["lib"]
 
 
-SLABS = 21          # 7 column tiles x 21 row slabs = 147 CTAs
+SLABS = 37          # 7 column tiles x 37 row slabs = 259 CTAs: two per SM of an H100 (132 SMs)
 
 
 def _declare_gemm3x(L):
@@ -374,7 +376,7 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], 
 
 
 class Linear(nn.Linear):
-    """nn.Linear whose 2-D fp32 CUDA GEMMs run as BF16x9-emulated fp32 on the tensor cores."""
+    """nn.Linear whose 2-D fp32 CUDA GEMMs go through `linear`."""
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return linear(x, self.weight, self.bias)

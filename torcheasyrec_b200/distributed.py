@@ -4,7 +4,7 @@ Replaces what the reference obtains from torchrec's DistributedModelParallel (tz
 tzrec/utils/dist_util.py:164-195): ShardedEmbeddingBagCollection / ShardedEmbeddingCollection with their
 input-dist (KJT bucketize + all-to-all, App. A.5/A.7), lookup, output-dist (A.6/A.8) and fused backward.
 
-B200-first design (DESIGN.md §6) — ONE exchange pattern for every sharding type:
+H100-first design (DESIGN.md §6) — ONE exchange pattern for every sharding type:
   forward   1. K1 bucketize: every id -> (owner rank, local row); table-wise = "block >= rows, owner = rank of
                the table", row-wise = "block = ceil(rows/W), owner 0" (tzk_bucketize_rw)
             2. all-to-all of the per-(dest, feature) id COUNTS [W,F] (a few hundred bytes, instead of torchrec's

@@ -318,7 +318,7 @@ class _ArenaCollection(nn.Module):
         dev = self.weights.device
         if self.layout.interleaved:        # a second set_optimizer: back to dense rows first (the old state is dropped)
             self._relayout(False, 0.0)
-        # TZK_INTERLEAVE: "0": dense rows; "force": also off CUDA (host-logic tests); default on (validated on B200)
+        # TZK_INTERLEAVE: "0": dense rows; "force": also off CUDA (host-logic tests); default on
         env = os.environ.get("TZK_INTERLEAVE", "1")
         if (spec.kind == OPT_ADAGRAD and self.allow_interleave and self.table_dtype == torch.float32
                 and ((dev.type == "cuda" and env != "0") or env == "force")):

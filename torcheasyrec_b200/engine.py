@@ -1,8 +1,8 @@
-"""Step driver: builds a model from a tzrec pipeline config and runs train steps on one B200.
+"""Step driver: builds a model from a tzrec pipeline config and runs train steps on one H100.
 
 Replaces the part of tzrec/main.py that surrounds the hot path (model construction :763-781, optimizers
 :814-876, the step loop :519-547) and torchrec's TrainPipelineSparseDist (tzrec/utils/dist_util.py:221-303)
-with a B200-first design: the whole step (KJT scan, gather, interaction, dense towers, loss, backward incl.
+with an H100-first design: the whole step (KJT scan, gather, interaction, dense towers, loss, backward incl.
 the fused sparse update, dense optimizer) is captured ONCE in a CUDA graph over static device buffers and
 replayed; a side stream stages the next host batch (pinned H2D) while the current graph runs.
 Variable-shape workloads (sequence features) run the same code eagerly.

@@ -1,10 +1,10 @@
 """Generators for the pipeline configs BASELINE.json names (text format, same message tree as the reference's
 examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao}.config).
 
-/root/reference does not exist on the GPU box and its files are not copied into this repo, so the configs are
-re-derived here from their defining facts (SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table
-list and price boundaries, and the model blocks.  tests/test_config.py checks (when the reference is present)
-that each generated config parses to the same tree as the reference's example file — i.e. the reference's own
+The package does not depend on the reference's files, so the configs are re-derived here from their defining facts
+(SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table list and price boundaries, and the model
+blocks.  tests/test_config.py checks, against copies stored under tests/golden/ref_examples/, that each generated
+config parses to the same tree as the reference's example file — i.e. the reference's own
 examples/*.config load unchanged through `config.load_pipeline_config` and mean the same thing.
 """
 

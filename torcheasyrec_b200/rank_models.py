@@ -354,8 +354,7 @@ class DLRM(RankModel):
     def _fused_tail(self, batch: Batch, all_feat: torch.Tensor, in_map):
         """Training steps on CUDA: the last Perceptron of the final MLP, the output layer and the BCE loss as ONE kernel
         that also produces their gradients (csrc/tzk_tower_tail.cuh; 18 launches of latency-bound work on DLRM-Criteo).
-        The loss is handed to `loss()` through `_tail_loss`.  Default on (validated on B200: 313 + 13 GPU tests, step
-        0.951 -> 0.935 ms); TZK_FUSED_TAIL=0 keeps the layer-by-layer chain."""
+        The loss is handed to `loss()` through `_tail_loss`.  Default on; TZK_FUSED_TAIL=0 keeps the layer-by-layer chain."""
         from .dense_gemm import tower_tail_bce, tower_tail_usable
 
         self._tail_loss = None

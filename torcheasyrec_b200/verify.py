@@ -83,7 +83,7 @@ def verify_sharded(name: str, device, sharding: str, rw_min_rows: int = 0, stati
             got = v.cpu().numpy()
             if bit_exact_logits:
                 np.testing.assert_array_equal(got, want)
-            else:   # cuBLAS / tcgen05 tiles differ between batch B and W*B: not bit-stable across shapes
+            else:   # cuBLAS / gemm3x tiles differ between batch B and W*B: not bit-stable across shapes
                 np.testing.assert_allclose(got, want, rtol=1e-6, atol=1e-6)
             worst["logits"] = max(worst["logits"], float(np.abs(got - want).max()))
     for _ in range(steps):
