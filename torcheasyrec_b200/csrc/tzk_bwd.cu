@@ -1260,8 +1260,12 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   int grid_lin = (int)std::min<int64_t>(ceil_div64(n_bags, kThreads), kSmCountH100 * 16);
   size_t cub_bytes = L.cub_bytes;
   cudaError_t ce;
-  const size_t smem_lin = (size_t)(3 * F + 1) * sizeof(int64_t);
+  const size_t smem_lin = (size_t)(3 * F + 1) * sizeof(int64_t);   // 49 160 B at F = 2048: opt-in above 48 KB
   const int grid_seq = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountH100 * 16);
+  if (!pooled && smem_lin > 48 * 1024) {
+    if (k64) cudaFuncSetAttribute(linearize_seq_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_lin);
+    else cudaFuncSetAttribute(linearize_seq_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_lin);
+  }
   if (k64) {
     if (pooled)
       linearize_kernel<uint64_t><<<grid_lin, kThreads, 0, st>>>(ids, offsets, feat_rows, feat_key_base, F, B,

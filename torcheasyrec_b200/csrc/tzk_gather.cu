@@ -289,6 +289,16 @@ extern "C" int tzk_pooled_gather_fwd_f16(const void* weights, const int64_t* fea
                                         feat_pool, ids, offsets, F, B, max_dim, vec_ok, out, ld_out, stream);
 }
 
+// the kernel stages 3 F + 1 int64 in shared memory: 49 160 B at F = 2048, above the 48 KB a launch gets by default
+template <int VEC, typename WT>
+static void seq_gather_allow_smem(int G, size_t smem) {
+  if (smem <= 48 * 1024) return;
+  auto k = G == 1 ? seq_gather_fwd_kernel<1, VEC, WT> : G == 2 ? seq_gather_fwd_kernel<2, VEC, WT>
+         : G == 4 ? seq_gather_fwd_kernel<4, VEC, WT> : G == 8 ? seq_gather_fwd_kernel<8, VEC, WT>
+         : G == 16 ? seq_gather_fwd_kernel<16, VEC, WT> : seq_gather_fwd_kernel<32, VEC, WT>;
+  cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
 template <typename WT>
 static int seq_gather_fwd_impl(const WT* weights, const int64_t* feat_w_off, const int64_t* feat_rows,
                                const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t D, int64_t nnz,
@@ -306,6 +316,7 @@ static int seq_gather_fwd_impl(const WT* weights, const int64_t* feat_w_off, con
   int64_t blocks = ceil_div64(nnz, NG);
   int grid = blocks < kSmCountH100 * 16 ? (int)blocks : kSmCountH100 * 16;
   size_t smem = (size_t)(3 * F + 1) * sizeof(int64_t);
+  if (vec == 4) seq_gather_allow_smem<4, WT>(G, smem); else seq_gather_allow_smem<1, WT>(G, smem);
   if (vec == 4) {
     TZK_DISPATCH_G(G, 4, WT, seq_gather_fwd_kernel, weights, feat_w_off, feat_rows, ids, offsets, F, B, D, nnz, out, row_stride)
   } else {
