@@ -270,6 +270,17 @@ int tzk_dot_interact_bwd(const float* dense, int64_t ld_dense, const float* spar
                          const float* d_out, int64_t ld_dout, int64_t B, int32_t Ns, int32_t D,
                          int32_t copy_dense, int32_t copy_sparse, int32_t p_pad, float* d_dense,
                          int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, tzk_stream_t stream);
+/* DLRM-Criteo (26 sparse features of D = 16 plus the bottom-MLP output, interaction output laid out
+ * [351 pairs | 0 | dense 16 | sparse 416], 784 wide) followed by a 784 -> 64 layer: the backward of both at once.
+ * d_dense [M,16] and d_sparse [M,416] from dz [M,64] (gradient of the layer's pre-activation) and its weight w [64, ld_w]
+ * (columns 0..783 in the interaction's layout, ld_w >= 784); the layer's input gradient [M,784] is never written.
+ * 3xTF32 like libtzk_gemm3x.so: the same bits as its input-gradient pass followed by tzk_dot_interact_bwd.  Row strides
+ * multiples of 4 floats, every pointer 16-B aligned; wt_hi / wt_lo: [784, 64] scratch (the TF32 split of w^T).
+ * (tzrec/models/dlrm.py:113-131 + tzrec/modules/mlp.py:20-84, backward) */
+int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_t ld_w, const float* dense,
+                          int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
+                          int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
+                          tzk_stream_t stream);
 
 /* ---- dense-tower helpers (callers of the path: tzrec/modules/mlp.py:20-84, Perceptron = Linear -> ReLU) ----
  * The tower GEMMs stay library calls; these fuse the element-wise passes around them.

@@ -23,9 +23,9 @@
 // Accuracy: x = hi + lo with hi = tf32(x), lo = tf32(x - hi); the dropped lo*lo term is 2^-22 relative — the same class as
 // the fp32 FFMA kernels (tests hold both to 1e-5).  Summation order differs from a sequential dot product.
 //
-// The includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_dense.cu; g++ + tests/native/cuda_cpu_shim.h:
-// tests/test_interact_tc_cpu.py runs this source on the host with an emulated mma), tzk_itc::mma_tf32 and
-// tzk_itc::cvt_tf32.
+// The includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_dense.cu, and tzk_interact_wide.cu for bwd_sample; g++ +
+// tests/native/cuda_cpu_shim.h: tests/test_interact_tc_cpu.py runs this source on the host with an emulated mma),
+// tzk_itc::mma_tf32 and tzk_itc::cvt_tf32.
 #pragma once
 #include <stdint.h>
 
@@ -135,6 +135,106 @@ dot_interact27_fwd_tc_kernel(const float* __restrict__ dense, int64_t ld_dense, 
 }
 
 // ---- backward -------------------------------------------------------------------------------------------------------
+// pair index -> (i << 8) | j, for the kP pairs; written by the whole CTA (the caller synchronises)
+__device__ __forceinline__ void init_pair_ij(unsigned short* pair_ij) {
+  for (int idx = threadIdx.x; idx < kP; idx += blockDim.x) {
+    int i = 0, rs = 0;
+    while (idx >= rs + (kN - 1 - i)) { rs += kN - 1 - i; ++i; }
+    pair_ij[idx] = (unsigned short)((i << 8) | (i + 1 + (idx - rs)));
+  }
+}
+
+// One sample, one warp: dE[i][.] = sum_j S[i][j] E[j][.] + pass, S = G + G^T from the kP pair gradients gp[] (global or
+// shared memory), E = rows dr (dense) and sr (sparse).  pass[q] = pass-through gradient dE[g + 8 q][4 t .. 4 t + 3] (zero
+// beyond row 26), loaded by the caller so that its latency overlaps other work.  S: this warp's [32 x kSS] scratch, zero
+// outside the pair entries; dd / ds: the sample's d_dense / d_sparse rows.
+__device__ __forceinline__ void bwd_sample(const float* gp, const float* dr, const float* sr, const float4 (&pass)[4],
+                                           const unsigned short* pair_ij, float* S, float* dd, float* ds, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  // B fragments: X[j = t + 4 h + 8 ks][2 g, 2 g + 1]  (8-B loads; 4 rows x 64 B per instruction)
+  float2 xv[4][2];
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int j = t + 4 * h + 8 * ks;
+      float2 v = make_float2(0.f, 0.f);
+      if (j == 0) v = *reinterpret_cast<const float2*>(dr + 2 * g);
+      else if (j < kN) v = *reinterpret_cast<const float2*>(sr + (j - 1) * kD + 2 * g);
+      xv[ks][h] = v;
+    }
+  // pair gradients -> symmetric S (coalesced reads, 11 per lane)
+  {
+    float gv[11];
+#pragma unroll
+    for (int q = 0; q < 11; ++q) {
+      const int idx = lane + 32 * q;
+      gv[q] = idx < kP ? gp[idx] : 0.f;
+    }
+#pragma unroll
+    for (int q = 0; q < 11; ++q) {
+      const int idx = lane + 32 * q;
+      if (idx < kP) {
+        const int i = pair_ij[idx] >> 8, j = pair_ij[idx] & 0xff;
+        S[i * kSS + j] = gv[q];
+        S[j * kSS + i] = gv[q];
+      }
+    }
+  }
+  __syncwarp();
+  uint32_t xh[4][2][2], xl[4][2][2];      // [ks][h][nt]
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      split_tf32(xv[ks][h].x, xh[ks][h][0], xl[ks][h][0]);
+      split_tf32(xv[ks][h].y, xh[ks][h][1], xl[ks][h][1]);
+    }
+  float acc[2][2][4];
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[mt][nt][q] = 0.f;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      // A fragment: S[g + 16 mt (+8)][t + 8 ks (+4)]
+      const float* sp = S + (g + 16 * mt) * kSS + t + 8 * ks;
+      uint32_t ah[4], al[4];
+      split_tf32(sp[0], ah[0], al[0]);
+      split_tf32(sp[8 * kSS], ah[1], al[1]);
+      split_tf32(sp[4], ah[2], al[2]);
+      split_tf32(sp[8 * kSS + 4], ah[3], al[3]);
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt) {
+        const uint32_t bh[2] = {xh[ks][0][nt], xh[ks][1][nt]};
+        const uint32_t bl[2] = {xl[ks][0][nt], xl[ks][1][nt]};
+        mma_tf32(acc[mt][nt], al, bh);
+        mma_tf32(acc[mt][nt], ah, bl);
+        mma_tf32(acc[mt][nt], ah, bh);
+      }
+    }
+  }
+  __syncwarp();        // every lane is done reading S before the next sample's scatter
+  // accumulators -> dX[i][4 t .. 4 t + 3]: tile nt holds d = 4 t + nt (q even) and 4 t + 2 + nt (q odd)
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int hrow = 0; hrow < 2; ++hrow) {
+      const int i = g + 16 * mt + 8 * hrow;
+      if (i >= kN) continue;
+      float4 v = make_float4(acc[mt][0][2 * hrow], acc[mt][1][2 * hrow], acc[mt][0][2 * hrow + 1],
+                             acc[mt][1][2 * hrow + 1]);
+      const float4 p = pass[2 * mt + hrow];
+      v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w;
+      if (i == 0) *reinterpret_cast<float4*>(dd + 4 * t) = v;
+      else *reinterpret_cast<float4*>(ds + (i - 1) * kD + 4 * t) = v;
+    }
+}
+
 __global__ void __launch_bounds__(kWarps * 32)
 dot_interact27_bwd_tc_kernel(const float* __restrict__ dense, int64_t ld_dense, const float* __restrict__ sparse,
                              int64_t ld_sparse, const float* __restrict__ d_out, int64_t ld_dout, int64_t B,
@@ -146,107 +246,20 @@ dot_interact27_bwd_tc_kernel(const float* __restrict__ dense, int64_t ld_dense, 
   // CTA-wide table: pair index -> (i, j); then one S matrix per warp
   unsigned short* pair_ij = reinterpret_cast<unsigned short*>(smem);
   float* S = smem + kInter / 2 + warp * (32 * kSS);       // (352 u16 = 176 floats)
-  for (int idx = threadIdx.x; idx < kP; idx += blockDim.x) {
-    int i = 0, rs = 0;
-    while (idx >= rs + (kN - 1 - i)) { rs += kN - 1 - i; ++i; }
-    pair_ij[idx] = (unsigned short)((i << 8) | (i + 1 + (idx - rs)));
-  }
+  init_pair_ij(pair_ij);
   for (int i = lane; i < 32 * kSS; i += 32) S[i] = 0.f;   // diagonal and padding stay zero for the whole kernel
   __syncthreads();
   const int64_t stride = (int64_t)gridDim.x * kWarps;
   for (int64_t b = (int64_t)blockIdx.x * kWarps + warp; b < B; b += stride) {
     const float* go = d_out + b * ld_dout;
-    const float* dr = dense + b * ld_dense;
-    const float* sr = sparse + b * ld_sparse;
-    // B fragments: X[j = t + 4 h + 8 ks][2 g, 2 g + 1]  (8-B loads; 4 rows x 64 B per instruction)
-    float2 xv[4][2];
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int j = t + 4 * h + 8 * ks;
-        float2 v = make_float2(0.f, 0.f);
-        if (j == 0) v = *reinterpret_cast<const float2*>(dr + 2 * g);
-        else if (j < kN) v = *reinterpret_cast<const float2*>(sr + (j - 1) * kD + 2 * g);
-        xv[ks][h] = v;
-      }
-    // pass-through gradient of the four rows this lane finishes: requested now, consumed after the MMAs
     float4 pass[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int i = g + 8 * q;
       pass[q] = i < kN ? *reinterpret_cast<const float4*>(go + kInter + i * kD + 4 * t) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    // pair gradients -> symmetric S (coalesced reads, 11 per lane)
-    {
-      float gv[11];
-#pragma unroll
-      for (int q = 0; q < 11; ++q) {
-        const int idx = lane + 32 * q;
-        gv[q] = idx < kP ? __ldg(go + idx) : 0.f;
-      }
-#pragma unroll
-      for (int q = 0; q < 11; ++q) {
-        const int idx = lane + 32 * q;
-        if (idx < kP) {
-          const int i = pair_ij[idx] >> 8, j = pair_ij[idx] & 0xff;
-          S[i * kSS + j] = gv[q];
-          S[j * kSS + i] = gv[q];
-        }
-      }
-    }
-    __syncwarp();
-    uint32_t xh[4][2][2], xl[4][2][2];      // [ks][h][nt]
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        split_tf32(xv[ks][h].x, xh[ks][h][0], xl[ks][h][0]);
-        split_tf32(xv[ks][h].y, xh[ks][h][1], xl[ks][h][1]);
-      }
-    float acc[2][2][4];
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[mt][nt][q] = 0.f;
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        // A fragment: S[g + 16 mt (+8)][t + 8 ks (+4)]
-        const float* sp = S + (g + 16 * mt) * kSS + t + 8 * ks;
-        uint32_t ah[4], al[4];
-        split_tf32(sp[0], ah[0], al[0]);
-        split_tf32(sp[8 * kSS], ah[1], al[1]);
-        split_tf32(sp[4], ah[2], al[2]);
-        split_tf32(sp[8 * kSS + 4], ah[3], al[3]);
-#pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
-          const uint32_t bh[2] = {xh[ks][0][nt], xh[ks][1][nt]};
-          const uint32_t bl[2] = {xl[ks][0][nt], xl[ks][1][nt]};
-          mma_tf32(acc[mt][nt], al, bh);
-          mma_tf32(acc[mt][nt], ah, bl);
-          mma_tf32(acc[mt][nt], ah, bh);
-        }
-      }
-    }
-    __syncwarp();        // every lane is done reading S before the next sample's scatter
-    // accumulators -> dX[i][4 t .. 4 t + 3]: tile nt holds d = 4 t + nt (q even) and 4 t + 2 + nt (q odd)
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-      for (int hrow = 0; hrow < 2; ++hrow) {
-        const int i = g + 16 * mt + 8 * hrow;
-        if (i >= kN) continue;
-        float4 v = make_float4(acc[mt][0][2 * hrow], acc[mt][1][2 * hrow], acc[mt][0][2 * hrow + 1],
-                               acc[mt][1][2 * hrow + 1]);
-        const float4 p = pass[2 * mt + hrow];
-        v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w;
-        if (i == 0) *reinterpret_cast<float4*>(d_dense + b * ld_ddense + 4 * t) = v;
-        else *reinterpret_cast<float4*>(d_sparse + b * ld_dsparse + (i - 1) * kD + 4 * t) = v;
-      }
+    bwd_sample(go, dense + b * ld_dense, sparse + b * ld_sparse, pass, pair_ij, S, d_dense + b * ld_ddense,
+               d_sparse + b * ld_dsparse, lane);
   }
 }
 

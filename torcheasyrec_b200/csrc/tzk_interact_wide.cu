@@ -1,0 +1,234 @@
+// tzk_interact_wide.cu — DLRM-Criteo's dot interaction and the first layer of its final MLP (783 -> 64) share one
+// backward kernel: the layer's input gradient dX [B, 784] is turned into the interaction's input gradients inside the
+// CTA that computes it and never reaches global memory (tzk_interact_wide_bwd, include/tzk.h).
+//
+// The GEMM part is written like tzk_gemm3x.cu (TMA SWIZZLE_128B boxes through mbarrier-guarded stages, mma.sync m16n8k8
+// TF32 with the 3xTF32 split, every k-step accumulated in fresh registers and added in round-to-nearest); the per-sample
+// interaction backward is tzk_interact_tc.cuh's.  The same source runs on the CPU under tests/native/cuda_cpu_shim.h and
+// sm90_cpu_emu.h (tests/test_interact_wide_fused.py).
+#include <stdint.h>
+#include <stdio.h>
+#include <stdlib.h>
+
+#ifdef TZK_CPU_SHIM
+#include "cuda_cpu_shim.h"
+#include "sm90_cpu_emu.h"
+typedef void* tzk_stream_t;
+#define TZK_REQUIRE(cond, ...) do { if (!(cond)) return 1; } while (0)
+#define TZK_CHECK_LAUNCH(name) do {} while (0)
+#else
+#include <cuda.h>
+#include "tzk_common.cuh"
+#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(1024) type name[]
+#define TZK_UNPAREN(...) __VA_ARGS__
+#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#endif
+
+namespace {
+#ifndef TZK_CPU_SHIM
+#include "tzk_sm90_ptx.h"
+#endif
+#include "tzk_tma.h"
+namespace tzk_itc {      // what tzk_interact_tc.cuh expects from its includer
+__device__ __forceinline__ uint32_t cvt_tf32(float x) { return tf32_bits(x); }
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) { ::mma_tf32(c, a, b); }
+}  // namespace tzk_itc
+#include "tzk_interact_tc.cuh"
+
+// a float4 this kernel wrote earlier (another thread of the CTA, before a __syncthreads): through L2, not the
+// read-only path
+__device__ __forceinline__ float4 load_l2(const float* p) {
+#ifdef TZK_CPU_SHIM
+  return *reinterpret_cast<const float4*>(p);
+#else
+  return __ldcg(reinterpret_cast<const float4*>(p));
+#endif
+}
+
+// ======================================================================================================================
+// Input gradient of the wide layer fused with the backward of the DLRM interaction that produced its input (DLRM-Criteo:
+// X = [351 pairs | 0 | dense 16 | sparse 416], 784 columns).  Per CTA of FB_M samples:
+//   1. dX[FB_M x 784] = dZ W, in chunks of 32 columns: dZ's fragments are split once and stay in registers (K = 64), W^T
+//      hi / lo chunks arrive by TMA through the stage ring.  The pass-through columns (352 ..) are stored straight into
+//      d_dense / d_sparse; the pair columns (0 .. 351) go to a shared-memory tile.  They run second so that the
+//      tile is complete when the ring drains.
+//   2. per sample, one warp: S from the pair columns, dE = S E + pass-through (tzk_itc::bwd_sample), the pass-through
+//      read back from d_dense / d_sparse (written by this CTA in step 1, so an L2 hit).
+// dX never reaches global memory.  The MMA order and the per-k-step accumulation are gemm3x_kernel's, so dX and with it
+// dE are bit for bit what gemm3x_kernel (dgrad) followed by dot_interact27_bwd_tc_kernel computes.
+constexpr int FB_M = 64;                      // samples per CTA
+constexpr int FB_THREADS = 512;               // 16 warps: 4 along the samples x 4 along a 32-column chunk
+constexpr int FB_WARPS = FB_THREADS / 32;
+constexpr int FB_CHUNKS = (tzk_itc::kRow + 31) / 32;   // 25: the last one reads W^T rows 784 .. 799 as zeros
+constexpr int FB_PAIR_CHUNKS = tzk_itc::kInter / 32;   // 11: columns 0 .. 351
+constexpr int FB_BOX = 32 * 128;              // one W^T box: 32 dX columns x 32 k = 4 KB
+constexpr int FB_STAGE = 4 * FB_BOX;          // hi k 0..31 | hi k 32..63 | lo k 0..31 | lo k 32..63
+constexpr int FB_STAGES = 3;
+constexpr int FB_LDP = 360;                   // row stride of the pair tile: 8 mod 32 words -> conflict-free float2 stores
+constexpr int FB_P_OFF = FB_STAGES * FB_STAGE;
+constexpr int FB_S_OFF = FB_P_OFF + FB_M * FB_LDP * 4;
+constexpr int FB_IJ_OFF = FB_S_OFF + FB_WARPS * 32 * tzk_itc::kSS * 4;
+constexpr int FB_BAR_OFF = FB_IJ_OFF + tzk_itc::kInter * 2;
+constexpr int FB_SMEM = FB_BAR_OFF + FB_STAGES * 8;    // 215 768 B: one CTA per SM
+
+struct FbParams {
+  const float* dz; int64_t ld_dz;
+  const float* dense; int64_t ld_dense;
+  const float* sparse; int64_t ld_sparse;
+  float* d_dense; int64_t ld_ddense;
+  float* d_sparse; int64_t ld_dsparse;
+  int64_t M;
+};
+
+__global__ void __launch_bounds__(FB_THREADS, 1)
+interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
+                         FbParams p) {
+  TZK_DYN_SMEM(uint8_t, smem);
+  float* P = reinterpret_cast<float*>(smem + FB_P_OFF);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + FB_BAR_OFF);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int64_t m0 = (int64_t)blockIdx.x * FB_M;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < FB_STAGES; ++s) mbar_init(full + s, 1);
+    fence_mbarrier_init();
+  }
+  float* S = reinterpret_cast<float*>(smem + FB_S_OFF) + warp * (32 * tzk_itc::kSS);
+  unsigned short* pair_ij = reinterpret_cast<unsigned short*>(smem + FB_IJ_OFF);
+  tzk_itc::init_pair_ij(pair_ij);
+  for (int i = lane; i < 32 * tzk_itc::kSS; i += 32) S[i] = 0.f;   // diagonal and padding stay zero
+  __syncthreads();
+  // chunk c covers dX columns 32 col_chunk(c) ..: the pass-through chunks first, then the pair chunks
+  auto col_chunk = [](int c) { return (c + FB_PAIR_CHUNKS) % FB_CHUNKS; };
+  auto load = [&](int c) {                        // thread 0 only
+    uint8_t* sb = smem + (c % FB_STAGES) * FB_STAGE;
+    uint64_t* bar = full + c % FB_STAGES;
+    const int n0 = col_chunk(c) * 32;
+    mbar_expect_tx(bar, FB_STAGE);
+    tma_load_2d(sb, &map_whi, bar, 0, n0);
+    tma_load_2d(sb + FB_BOX, &map_whi, bar, 32, n0);
+    tma_load_2d(sb + 2 * FB_BOX, &map_wlo, bar, 0, n0);
+    tma_load_2d(sb + 3 * FB_BOX, &map_wlo, bar, 32, n0);
+  };
+  if (threadIdx.x == 0)
+    for (int c = 0; c < FB_STAGES; ++c) load(c);
+
+  // A = dZ rows r, r + 8 of this warp's 16, all 64 columns, split once (rows past M are zeros)
+  const int wm = warp & 3, wn = warp >> 2;
+  const int r = wm * 16 + g;
+  uint32_t ah[8][4], al[8][4];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    const int k0 = kk * 8 + t, k1 = k0 + 4;
+    const int64_t ra = m0 + r, rb = ra + 8;
+    const float a[4] = {ra < p.M ? __ldg(p.dz + ra * p.ld_dz + k0) : 0.f, rb < p.M ? __ldg(p.dz + rb * p.ld_dz + k0) : 0.f,
+                        ra < p.M ? __ldg(p.dz + ra * p.ld_dz + k1) : 0.f, rb < p.M ? __ldg(p.dz + rb * p.ld_dz + k1) : 0.f};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      ah[kk][i] = tf32_bits(a[i]);
+      al[kk][i] = tf32_bits(a[i] - __uint_as_float(ah[kk][i]));
+    }
+  }
+  const int n = wn * 8 + g;                       // this lane's B column (W^T row) within the chunk
+  for (int c = 0; c < FB_CHUNKS; ++c) {
+    const int s = c % FB_STAGES;
+    mbar_wait(full + s, (uint32_t)(c / FB_STAGES) & 1u);
+    const uint32_t* whi = reinterpret_cast<const uint32_t*>(smem + s * FB_STAGE);
+    const uint32_t* wlo = whi + 2 * FB_BOX / 4;
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t* bh_box = whi + (kk >> 2) * (FB_BOX / 4);
+      const uint32_t* bl_box = wlo + (kk >> 2) * (FB_BOX / 4);
+      const int k0 = (kk & 3) * 8 + t, k1 = k0 + 4;
+      const uint32_t bh[2] = {bh_box[swz(n, k0)], bh_box[swz(n, k1)]};
+      const uint32_t bl[2] = {bl_box[swz(n, k0)], bl_box[swz(n, k1)]};
+      float part[4] = {0.f, 0.f, 0.f, 0.f};
+      mma_tf32(part, al[kk], bh);                 // small terms first
+      mma_tf32(part, ah[kk], bl);
+      mma_tf32(part, ah[kk], bh);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[q] += part[q];
+    }
+    // c0/c1: row r, columns col, col + 1; c2/c3: row r + 8
+    const int col = col_chunk(c) * 32 + wn * 8 + 2 * t;
+    if (col < tzk_itc::kInter) {
+      *reinterpret_cast<float2*>(P + r * FB_LDP + col) = make_float2(acc[0], acc[1]);
+      *reinterpret_cast<float2*>(P + (r + 8) * FB_LDP + col) = make_float2(acc[2], acc[3]);
+    } else if (col < tzk_itc::kRow) {
+      const int e = col - tzk_itc::kInter;        // column of [dense 16 | sparse 416]
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = m0 + r + 8 * h;
+        if (row >= p.M) continue;
+        float* dst = e < tzk_itc::kD ? p.d_dense + row * p.ld_ddense + e : p.d_sparse + row * p.ld_dsparse + (e - tzk_itc::kD);
+        *reinterpret_cast<float2*>(dst) = make_float2(acc[2 * h], acc[2 * h + 1]);
+      }
+    }
+    __syncthreads();                              // every warp is done with stage s; at the end: P and the stores
+    if (threadIdx.x == 0 && c + FB_STAGES < FB_CHUNKS) load(c + FB_STAGES);
+  }
+
+  for (int i = warp; i < FB_M; i += FB_WARPS) {
+    const int64_t b = m0 + i;
+    if (b >= p.M) break;
+    float* dd = p.d_dense + b * p.ld_ddense;
+    float* ds = p.d_sparse + b * p.ld_dsparse;
+    float4 pass[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int row = g + 8 * q;
+      pass[q] = row == 0 ? load_l2(dd + 4 * t)
+              : row < tzk_itc::kN ? load_l2(ds + (row - 1) * tzk_itc::kD + 4 * t)
+              : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    tzk_itc::bwd_sample(P + i * FB_LDP, p.dense + b * p.ld_dense, p.sparse + b * p.ld_sparse, pass, pair_ij, S, dd, ds,
+                        lane);
+  }
+}
+
+// W^T hi / lo [K, 64] from W [64, ld_w] (K columns used)
+__global__ void split_wt_kernel(const float* __restrict__ w, int64_t ld_w, int K, float* __restrict__ hi,
+                                float* __restrict__ lo) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < K * 64) {
+    const int k = i >> 6, o = i & 63;
+    const float v = w[(int64_t)o * ld_w + k];
+    const float h = tf32_rna(v);
+    hi[i] = h;
+    lo[i] = tf32_rna(v - h);
+  }
+}
+
+}  // namespace
+
+extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_t ld_w, const float* dense,
+                                     int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
+                                     int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
+                                     tzk_stream_t stream) {
+  TZK_REQUIRE(M > 0, "interact_wide_bwd: M must be positive");
+  TZK_REQUIRE(ld_w >= tzk_itc::kRow, "interact_wide_bwd: w needs %d columns", tzk_itc::kRow);
+  const int64_t lds[] = {ld_dz, ld_w, ld_dense, ld_sparse, ld_ddense, ld_dsparse};
+  for (int64_t ld : lds) TZK_REQUIRE(ld % 4 == 0, "interact_wide_bwd: row strides must be multiples of 4 floats");
+  const void* ptrs[] = {dz, w, dense, sparse, d_dense, d_sparse, wt_hi, wt_lo};
+  for (const void* q : ptrs)
+    TZK_REQUIRE(q && reinterpret_cast<uintptr_t>(q) % 16 == 0, "interact_wide_bwd: NULL or not 16-B aligned pointer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  TZK_LAUNCH((split_wt_kernel), (tzk_itc::kRow * 64 + 255) / 256, 256, 0, st, w, ld_w, tzk_itc::kRow, wt_hi, wt_lo);
+  CUtensorMap mh, ml;
+  TZK_REQUIRE(!make_map(&mh, wt_hi, tzk_itc::kRow, 64, 64, 32) && !make_map(&ml, wt_lo, tzk_itc::kRow, 64, 64, 32),
+              "interact_wide_bwd: tensor-map encoding failed");
+  FbParams p;
+  p.dz = dz; p.ld_dz = ld_dz; p.dense = dense; p.ld_dense = ld_dense; p.sparse = sparse; p.ld_sparse = ld_sparse;
+  p.d_dense = d_dense; p.ld_ddense = ld_ddense; p.d_sparse = d_sparse; p.ld_dsparse = ld_dsparse; p.M = M;
+#ifndef TZK_CPU_SHIM
+  static bool configured = false;     // once: nothing but the launches happens inside a stream capture
+  if (!configured) {
+    cudaFuncSetAttribute(interact_wide_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FB_SMEM);
+    configured = true;
+  }
+#endif
+  TZK_LAUNCH((interact_wide_bwd_kernel), (unsigned)((M + FB_M - 1) / FB_M), FB_THREADS, FB_SMEM, st, mh, ml, p);
+  TZK_CHECK_LAUNCH("interact_wide_bwd_kernel");
+  return 0;
+}

@@ -268,6 +268,59 @@ class Gemm3xLinearFn(torch.autograd.Function):
         return None, dx, dw, db, None, None
 
 
+class InteractWideFn(torch.autograd.Function):
+    """relu(X @ W^T + b) with X = functional.dlrm_interaction(dense, sparse, 26, 16, aligned=True), the first layer of
+    DLRM-Criteo's final MLP.  The forward is the interaction kernel followed by gemm3x; the backward computes the
+    interaction's input gradients in one kernel from dZ and W (tzk_interact_wide_bwd) instead of writing X's gradient
+    [M, 784] to memory and reading it back, and the weight gradient with wgrad3x from the saved X."""
+
+    @staticmethod
+    def forward(ctx, lib, dense, sparse, weight, bias, in_map):
+        from .functional import _rows_contig, backend
+
+        dense, sparse = _rows_contig(dense), _rows_contig(sparse)
+        x = backend().dot_interact_fwd(dense, sparse, 26, 16, True, True, 4, 1)
+        w = torch.zeros((weight.shape[0], x.shape[1]), dtype=weight.dtype, device=weight.device)
+        for (src, dst, n) in in_map:
+            w[:, dst:dst + n].copy_(weight[:, src:src + n])
+        y = gemm3x(lib, x, w, bias, True)
+        ctx.lib, ctx.in_map, ctx.has_bias = lib, in_map, bias is not None
+        ctx.save_for_backward(dense, sparse, x, w, y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from .kernels import default_kernels
+
+        dense, sparse, x, w, y = ctx.saved_tensors
+        lib = ctx.lib
+        dz, colsum = default_kernels().act_bwd_colsum(dy.contiguous(), y, True, want_dz=True)
+        d_dense = d_sparse = dw = None
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            d_dense, d_sparse = default_kernels().interact_wide_bwd(dz, w, dense, sparse)
+        if ctx.needs_input_grad[3]:
+            full = wgrad3x(lib, x, dz)
+            dw = torch.cat([full[:, dst:dst + n] for (_, dst, n) in ctx.in_map], dim=1)
+        db = colsum if (ctx.has_bias and ctx.needs_input_grad[4]) else None
+        return (None, d_dense if ctx.needs_input_grad[1] else None, d_sparse if ctx.needs_input_grad[2] else None, dw, db,
+                None)
+
+
+def interact_wide_usable(dense: Optional[torch.Tensor], sparse: torch.Tensor, weight: torch.Tensor,
+                         num_sparse: int, dim: int) -> bool:
+    """Whether InteractWideFn covers this layer: DLRM-Criteo's shape (26 sparse features of 16 plus the bottom-MLP
+    output, all copied into the row), fp32 CUDA tensors, a 783 -> 64 weight, and the kernels the layer-by-layer path
+    would run (gemm3x for the layer, the tensor-core interaction)."""
+    return (dense is not None and num_sparse == 26 and dim == 16 and dense.is_cuda and dense.dtype == torch.float32
+            and sparse.dtype == torch.float32 and dense.dim() == 2 and tuple(dense.shape[1:]) == (16,)
+            and sparse.dim() == 2 and tuple(sparse.shape[1:]) == (416,) and dense.shape[0] == sparse.shape[0] >= 256
+            and all(t.stride(1) == 1 and t.stride(0) % 4 == 0 and t.data_ptr() % 16 == 0 for t in (dense, sparse))
+            and weight.dtype == torch.float32 and tuple(weight.shape) == (64, 783)
+            and os.environ.get("TZK_GEMM3X", "1") == "1" and os.environ.get("TZK_INTERACT_TC", "1") != "0"
+            and os.environ.get("TZK_INTERACT_TC_FWD", "1") != "0" and os.environ.get("TZK_INTERACT_TC_BWD", "1") != "0"
+            and not torch.backends.cuda.matmul.allow_tf32 and available() and _gemm3x_lib() is not None)
+
+
 def _use_gemm3x(x: torch.Tensor, weight: torch.Tensor) -> bool:
     return (os.environ.get("TZK_GEMM3X", "1") == "1" and x.is_cuda and x.dim() == 2 and x.dtype == torch.float32
             and weight.dtype == torch.float32 and x.stride(1) == 1 and x.stride(0) % 4 == 0 and x.data_ptr() % 16 == 0

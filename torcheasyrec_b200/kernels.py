@@ -722,6 +722,23 @@ class CudaKernels:
         self.launches += 1
         return d_dense, d_sparse
 
+    def interact_wide_bwd(self, dz: torch.Tensor, w: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor):
+        """(d_dense [B, 16], d_sparse [B, 416]) of DLRM-Criteo's interaction followed by a 784 -> 64 layer with weight
+        w [64, 784] (the interaction's column layout), from dz [B, 64], the gradient of the layer's pre-activation."""
+        dz, ld_z = _rows2d(dz, "dz")
+        w, ld_w = _rows2d(w, "w")
+        dense, ld_d = _rows2d(dense, "dense")
+        sparse, ld_s = _rows2d(sparse, "sparse")
+        B = dz.shape[0]
+        d_dense = torch.empty((B, 16), dtype=torch.float32, device=dz.device)
+        d_sparse = torch.empty((B, 416), dtype=torch.float32, device=dz.device)
+        wt = torch.empty((2, 784, 64), dtype=torch.float32, device=dz.device)
+        check(self._lib.tzk_interact_wide_bwd(_ptr(dz), ld_z, _ptr(w), ld_w, _ptr(dense), ld_d, _ptr(sparse), ld_s, B,
+                                              _ptr(d_dense), 16, _ptr(d_sparse), 416, _ptr(wt[0]), _ptr(wt[1]),
+                                              _stream()), "tzk_interact_wide_bwd")
+        self.launches += 2
+        return d_dense, d_sparse
+
     # ------------------------------------------------------------------ dense-tower helpers
     def bias_act(self, y: torch.Tensor, bias: Optional[torch.Tensor], relu: bool) -> torch.Tensor:
         y, ld = _rows2d(y, "y")

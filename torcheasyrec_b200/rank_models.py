@@ -339,19 +339,38 @@ class DLRM(RankModel):
         sparse = grouped[self._sparse_group_name]
         if self.dense_mlp and dense_feat is None:
             dense_feat = self.dense_mlp(grouped[self._dense_group_name])
-        # interaction + both concats of dlrm.py:113-131 in one kernel
-        # the 783-wide result travels as [B, 784]: one zero column after the 351 interaction terms puts the dense
-        # and sparse blocks (and every row) on 16-B boundaries -> 128-bit stores in the kernel and tensor-core
-        # (align4) kernels for the first final-MLP GEMM and its dX/dW twins (dense_gemm.py pads the weight)
-        all_feat, in_map = Fn.dlrm_interaction(dense_feat, sparse, self._sparse_num, self._per_sparse_dim,
-                                               with_dense=True,
-                                               with_sparse=bool(self._model_config.arch_with_sparse), aligned=True)
-        fused = self._fused_tail(batch, all_feat, in_map)
+        x = self._interact_wide(dense_feat, sparse)
+        if x is not None:           # the interaction and the first final-MLP layer in one autograd node
+            in_map, start = None, 1
+        else:
+            # interaction + both concats of dlrm.py:113-131 in one kernel
+            # the 783-wide result travels as [B, 784]: one zero column after the 351 interaction terms puts the dense
+            # and sparse blocks (and every row) on 16-B boundaries -> 128-bit stores in the kernel and tensor-core
+            # (align4) kernels for the first final-MLP GEMM and its dX/dW twins (dense_gemm.py pads the weight)
+            x, in_map = Fn.dlrm_interaction(dense_feat, sparse, self._sparse_num, self._per_sparse_dim,
+                                            with_dense=True,
+                                            with_sparse=bool(self._model_config.arch_with_sparse), aligned=True)
+            start = 0
+        fused = self._fused_tail(batch, x, in_map, start)
         if fused is not None:
             return fused
-        return self._output_to_prediction(self.output_mlp(self.final_mlp(all_feat, in_map)))
+        for i, layer in enumerate(list(self.final_mlp.mlp)[start:], start):
+            x = layer(x, in_map) if (i == 0 and in_map is not None) else layer(x)
+        return self._output_to_prediction(self.output_mlp(x))
 
-    def _fused_tail(self, batch: Batch, all_feat: torch.Tensor, in_map):
+    def _interact_wide(self, dense_feat: Optional[torch.Tensor], sparse: torch.Tensor) -> Optional[torch.Tensor]:
+        """Output of the first final-MLP layer computed together with the interaction (dense_gemm.InteractWideFn) when
+        the model has DLRM-Criteo's shape and that layer is Linear(783 -> 64) + ReLU; None otherwise."""
+        from .dense_gemm import InteractWideFn, _gemm3x_lib, interact_wide_usable
+
+        first = self.final_mlp.mlp[0].perceptron
+        if not (self._model_config.arch_with_sparse and len(first) == 2 and isinstance(first[1], nn.ReLU)
+                and interact_wide_usable(dense_feat, sparse, first[0].weight, self._sparse_num, self._per_sparse_dim)):
+            return None
+        in_map = ((0, 0, 351), (351, 352, 432))
+        return InteractWideFn.apply(_gemm3x_lib(), dense_feat, sparse, first[0].weight, first[0].bias, in_map)
+
+    def _fused_tail(self, batch: Batch, all_feat: torch.Tensor, in_map, start: int = 0):
         """Training steps on CUDA: the last Perceptron of the final MLP, the output layer and the BCE loss as ONE kernel
         that also produces their gradients (csrc/tzk_tower_tail.cuh; 18 launches of latency-bound work on DLRM-Criteo).
         The loss is handed to `loss()` through `_tail_loss`.  Default on; TZK_FUSED_TAIL=0 keeps the layer-by-layer chain."""
@@ -368,8 +387,10 @@ class DLRM(RankModel):
         label = batch.labels[self._label_name].to(torch.float32)
         w1, b1 = last[0].weight, last[0].bias
         w2, b2 = self.output_mlp.weight, self.output_mlp.bias
+        if start >= len(layers):
+            return None
         x = all_feat
-        for i, layer in enumerate(layers[:-1]):
+        for i, layer in enumerate(layers[start:-1], start):
             x = layer(x, in_map) if (i == 0 and in_map is not None) else layer(x)
         if len(layers) == 1 and in_map is not None:
             return None
