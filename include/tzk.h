@@ -47,6 +47,10 @@ extern "C" {
 /* the next two only through tzk_fused_bwd_ex / tzk_fused_bwd_apply_ex (they need tzk_opt_args) */
 #define TZK_OPT_ADAM 3            /* m=b1 m+(1-b1)g ; v=b2 v+(1-b2)g*g ; w -= lr*(m^/(sqrt(v^)+eps) + wd*w)  (ADAM) */
 #define TZK_OPT_PARTIAL_ROWWISE_ADAM 4 /* m element-wise, v one value per row from mean_d(g*g)  (PARTIAL_ROWWISE_ADAM) */
+/* the layer-wise adaptive optimizers, also _ex only; |.| = L2 norm over the row's D elements */
+#define TZK_OPT_LAMB 5            /* m, v as ADAM ; u = m^/(sqrt(v^)+eps) + wd*w ; w -= lr*(|w|/|u|)*u            (LAMB) */
+#define TZK_OPT_PARTIAL_ROWWISE_LAMB 6 /* m element-wise, v one value per row from mean_d(g*g), u and step as LAMB (PARTIAL_ROWWISE_LAMB) */
+#define TZK_OPT_LARS_SGD 7        /* lr' = lr*eta*|w|/(|g|+wd*|w|) ; m = momentum*m + lr'*(g+wd*w) ; w -= m   (LARS_SGD) */
 /* peer-memory step only (_ex entry points): no update — weights[row] = summed gradient of the row, ((int32*)state)[key]
  * = 1; `weights` is then a dense per-row partial-sum buffer, not a table (see tzk_peer_small_update) */
 #define TZK_OPT_ACCUM_OUT 100
@@ -54,9 +58,10 @@ extern "C" {
 /* Optimizer description for the _ex entry points (what tzrec/optim/optimizer_builder.py:30-97 passes to
  * apply_optimizer_in_backward; field names follow tzrec/protos/optimizer.proto:76-139).  Host struct, device
  * pointers inside.
- *   state  : SGD unused; ADAGRAD / ADAM / PARTIAL_ROWWISE_ADAM: same layout as `weights` (accumulator / first
- *            moment); ROWWISE_ADAGRAD: one float per key.
- *   state2 : ADAM: second moment, same layout as `weights`; PARTIAL_ROWWISE_ADAM: one float per key.
+ *   state  : SGD unused; ADAGRAD / ADAM / PARTIAL_ROWWISE_ADAM / LAMB / PARTIAL_ROWWISE_LAMB / LARS_SGD: same layout as
+ *            `weights` (accumulator / first moment / momentum); ROWWISE_ADAGRAD: one float per key.
+ *   state2 : ADAM / LAMB: second moment, same layout as `weights`; PARTIAL_ROWWISE_ADAM / PARTIAL_ROWWISE_LAMB: one float
+ *            per key.  `step` as well: the LAMB variants use the same bias correction as Adam.
  *   step   : device scalar holding the 1-based iteration count of this update as a float (bias correction
  *            1 - beta^t is evaluated on the device, so a captured CUDA graph can keep replaying).
  *   max_gradient > 0 clamps every element of the summed row gradient to [-max_gradient, max_gradient]
@@ -74,6 +79,10 @@ typedef struct tzk_opt_args {
                         * line, so the update reads and writes whole lines (two half-line writes cost a read-modify-write
                         * each in DRAM: profiles/README.md).  `state` is ignored.  Lookups over such an arena:
                         * tzk_pooled_gather_fwd_strided / tzk_seq_gather_fwd_strided. */
+  float momentum, eta;  /* LARS_SGD: momentum of the velocity and the trust coefficient (fbgemm's default eta = 0.001) */
+  int32_t weight_decay_mode; /* ROWWISE_ADAGRAD (tzrec WeightDecayMode): 0 NONE (weight_decay ignored); 1 L2:
+                        * s_row += mean_d((g + wd*w)^2), w = (1 - mult*wd)*w - mult*g; 2 DECOUPLE: s_row += mean_d(g*g),
+                        * w = (1 - lr*wd)*w - mult*g; mult = lr/(sqrt(s_row)+eps) */
 } tzk_opt_args;
 
 typedef void* tzk_stream_t; /* cudaStream_t */

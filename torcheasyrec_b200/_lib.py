@@ -18,7 +18,8 @@ class TzkOptArgs(ctypes.Structure):
 
     _fields_ = [("optimizer", c_int32), ("lr", c_float), ("eps", c_float), ("beta1", c_float), ("beta2", c_float),
                 ("weight_decay", c_float), ("max_gradient", c_float), ("state", c_void_p), ("state2", c_void_p),
-                ("step", c_void_p), ("weights_f16", c_int32), ("interleaved", c_int32)]
+                ("step", c_void_p), ("weights_f16", c_int32), ("interleaved", c_int32), ("momentum", c_float),
+                ("eta", c_float), ("weight_decay_mode", c_int32)]
 
 
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)

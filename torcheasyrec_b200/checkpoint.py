@@ -8,8 +8,8 @@ loads under another world size / plan.  Here:
   * model keys are the reference's: `…ebc.embedding_bags.<table>.weight`, `…ec_dict.<dim>.embeddings.<table>.weight`
     (tzrec/utils/checkpoint_util_test.py:375-396) — a ShardedTensor over the table's global [rows, D] shape whose local
     shard is a VIEW of this rank's arena slice (sharded collections), or the plain [rows, D] view (unsharded);
-  * fused sparse optimizer state: `state.<weight key>.<table>.momentum1` (+ `.momentum2` / `.iter` for the Adam
-    variants [EXT names]); dense optimizer: `state.<param fqn>.exp_avg|exp_avg_sq|step`;
+  * fused sparse optimizer state: `state.<weight key>.<table>.momentum1` (+ `.momentum2` / `.iter` for the Adam and
+    LAMB variants [EXT names]); dense optimizer: `state.<param fqn>.exp_avg|exp_avg_sq|step`;
   * `plan`: {module path: {table: {sharding_type, compute_kernel, ranks}}} like checkpoint_util.py:1145-1160.
 The arena buffers and the `shards.*` submodules never appear in a key.
 """
@@ -21,8 +21,8 @@ import torch
 import torch.distributed as dist
 
 from .distributed import TABLE_WISE, _ShardedBase
-from .embedding_modules import _ArenaCollection
-from .kernels import OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM, OPT_ROWWISE_ADAGRAD
+from .embedding_modules import ADAM_LIKE_KINDS, ELEMENTWISE_STATE_KINDS, _ArenaCollection
+from .kernels import OPT_ADAGRAD, OPT_ADAM, OPT_LAMB, OPT_LARS_SGD, OPT_ROWWISE_ADAGRAD
 
 
 def _placement(rank: int, device: torch.device) -> str:
@@ -44,9 +44,9 @@ def sharded_rows_tensor(local: Optional[torch.Tensor], row_offset: int, global_s
 
 
 def _state_names(kind: int) -> List[str]:
-    if kind in (OPT_ADAGRAD, OPT_ROWWISE_ADAGRAD):
+    if kind in (OPT_ADAGRAD, OPT_ROWWISE_ADAGRAD, OPT_LARS_SGD):
         return ["momentum1"]
-    if kind in (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM):
+    if kind in ADAM_LIKE_KINDS:
         return ["momentum1", "momentum2", "iter"]
     return []
 
@@ -60,9 +60,7 @@ def _local_state(coll: _ArenaCollection, t: int, which: str) -> Optional[torch.T
     if spec is None or buf is None or t not in coll._table_off:
         return None
     rows, dim = coll._table_rows[t], coll._table_dim[t]
-    elementwise = (spec.kind in (OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM)) if which == "momentum1" \
-        else spec.kind == OPT_ADAM
-    if elementwise:
+    if _is_elementwise(spec.kind, which):
         o = coll._table_off[t]
         return buf[o:o + rows * dim].view(rows, dim)
     k = coll._table_key[t]
@@ -112,7 +110,7 @@ def fused_optimizer_state_dict(model, group=None) -> Dict[str, object]:
 
 
 def _is_elementwise(kind: int, which: str) -> bool:
-    return (kind in (OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM)) if which == "momentum1" else kind == OPT_ADAM
+    return (kind in ELEMENTWISE_STATE_KINDS) if which == "momentum1" else kind in (OPT_ADAM, OPT_LAMB)
 
 
 def dense_optimizer_state_dict(model, optimizer: torch.optim.Optimizer) -> Dict[str, torch.Tensor]:

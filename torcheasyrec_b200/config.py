@@ -81,6 +81,10 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
         "sgd_optimizer": _f("FusedSGDOptimizer"), "adagrad_optimizer": _f("FusedAdagradOptimizer"),
         "adam_optimizer": _f("FusedAdamOptimizer"), "rowwise_adagrad_optimizer": _f("FusedRowWiseAdagradOptimizer"),
         "partial_rowwise_adam_optimizer": _f("FusedAdamOptimizer"),     # same fields (optimizer.proto:124-131)
+        "lars_sgd_optimizer": _f("FusedLarsSGDOptimizer"),
+        "lamb_optimizer": _f("FusedAdamOptimizer"),                      # FusedLAMBOptimizer: the same fields
+        "partial_rowwise_lamb_optimizer": _f("FusedAdamOptimizer"),      # FusedPartialRowWiseLAMBOptimizer: the same
+        "adadelta_optimizer": _f("FusedAdadeltaOptimizer"), "rmsprop_optimizer": _f("FusedRMSpropOptimizer"),
         "constant_learning_rate": _f("ConstantLR"),
     },
     "DenseOptimizer": {
@@ -92,6 +96,9 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     "FusedAdagradOptimizer": dict(_FUSED, initial_accumulator_value=_f(F, 0.0)),
     "FusedRowWiseAdagradOptimizer": dict(_FUSED, weight_decay=_f(F, 0.0), weight_decay_mode=_f(E, "NONE")),
     "FusedAdamOptimizer": dict(_FUSED, beta1=_f(F, 0.9), beta2=_f(F, 0.999), weight_decay=_f(F, 0.0)),
+    "FusedLarsSGDOptimizer": dict(_FUSED, momentum=_f(F, 0.9), weight_decay=_f(F, 0.0)),
+    "FusedAdadeltaOptimizer": dict(_FUSED, rho=_f(F, 0.95), eps=_f(F, 1e-6), weight_decay=_f(F, 0.0)),
+    "FusedRMSpropOptimizer": dict(_FUSED, alpha=_f(F, 0.99), eps=_f(F, 1e-8), weight_decay=_f(F, 0.0)),
     "SGDOptimizer": {"lr": _f(F, 0.002), "momentum": _f(F, 0.0), "dampening": _f(F, 0.0), "nesterov": _f(B, False),
                      "weight_decay": _f(F, 0.0)},
     "AdagradOptimizer": {"lr": _f(F, 0.002), "lr_decay": _f(F, 0.0), "weight_decay": _f(F, 0.0),

@@ -73,7 +73,7 @@ struct BwdArgs {
   // extended optimizers (tzk_opt_args): second state, Adam constants, clipping
   float* state2;
   const float* step;  // device scalar: iteration count t >= 1 of this update (bias correction)
-  float beta1, beta2, weight_decay, max_gradient;
+  float beta1, beta2, weight_decay, max_gradient;   // LARS_SGD: beta1 = momentum, beta2 = eta (no moment decays there)
   float bc1, bc2;     // 1 - beta^t, filled in by init_bias_correction() at kernel start
   // peer mode (sharded step over peer memory, tzk_peer.cu): the sorted value is src_rank * idx_span + idx and the
   // gradient row lives in the SOURCE rank's published buffer grad_peer[src_rank] (already divided by the bag length
@@ -87,15 +87,26 @@ struct BwdArgs {
   // the kernel's instructions): mul == 0 means "divisor is 1"
   FastDiv div_b, div_span;
   int32_t ld32;         // = ld_grad (< 2^31, checked on the host): row offsets are ONE 32 x 32 -> 64-bit multiply
-  int32_t pad3;
+  int32_t wd_mode;      // row-wise Adagrad weight decay mode (tzk_opt_args.weight_decay_mode; read by finish_run_norm)
 };
+
+// Optimizer family of the run kernels, a template parameter chosen on the host.  kFamNorm: the updates whose step
+// depends on norms over the whole row (LAMB, partial row-wise LAMB, LARS-SGD) and row-wise Adagrad with L2 / decoupled
+// weight decay — two passes over the row with a group reduction in between (finish_run_norm).  Keeping them out of the
+// kFamClassic instantiations leaves the register allocation of the classic optimizers' kernels as it was.
+constexpr int kFamClassic = 0;
+constexpr int kFamNorm = 1;
 // peer mode: the sources' published gradient buffers.  A kernel parameter of its own (__grid_constant__): indexing it
 // with a run-time rank must not drag the whole argument block into local memory.
 struct PeerGrads { unsigned long long p[16]; };
 
+template <int FAM = kFamClassic>
 __device__ __forceinline__ void init_bias_correction(BwdArgs& a) {
   a.bc1 = a.bc2 = 1.f;
-  if (a.optimizer == TZK_OPT_ADAM || a.optimizer == TZK_OPT_PARTIAL_ROWWISE_ADAM) {
+  const bool adam_like = FAM == kFamClassic
+                             ? (a.optimizer == TZK_OPT_ADAM || a.optimizer == TZK_OPT_PARTIAL_ROWWISE_ADAM)
+                             : (a.optimizer == TZK_OPT_LAMB || a.optimizer == TZK_OPT_PARTIAL_ROWWISE_LAMB);
+  if (adam_like) {
     const float t = a.step ? __ldg(a.step) : 1.f;
     a.bc1 = 1.f - powf(a.beta1, t);
     a.bc2 = 1.f - powf(a.beta2, t);
@@ -385,14 +396,206 @@ __device__ __forceinline__ float group_sum(float v) {
   return v;
 }
 
+// first state laid out like the weights, per optimizer family
+template <int FAM>
+__device__ __forceinline__ bool elem_state(const BwdArgs& a) {
+  if (FAM == kFamClassic) return has_elem_state(a);
+  return a.optimizer == TZK_OPT_LAMB || a.optimizer == TZK_OPT_PARTIAL_ROWWISE_LAMB || a.optimizer == TZK_OPT_LARS_SGD;
+}
+
+template <int VEC>
+__device__ __forceinline__ void unpack4(const float4& x, float (&v)[VEC]) {
+  if constexpr (VEC == 4) {
+    v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+  } else {
+    v[0] = x.x;
+  }
+}
+template <int VEC>
+__device__ __forceinline__ void load_vec(const float* p, float (&v)[VEC]) {
+  if constexpr (VEC == 4) unpack4<4>(*reinterpret_cast<const float4*>(p), v);
+  else v[0] = p[0];
+}
+template <int VEC>
+__device__ __forceinline__ void store_vec(float* p, const float (&v)[VEC]) {
+  if constexpr (VEC == 4) *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  else p[0] = v[0];
+}
+
+// finish a run of the kFamNorm optimizers (fbgemm [EXT] split_embedding_optimizer_codegen, DESIGN.md §5); |.| is the L2
+// norm over the row's D elements, mult = lr / (sqrt(s_row) + eps):
+//   LAMB                 m = b1 m + (1-b1) g ; v = b2 v + (1-b2) g^2 ; u = m^/(sqrt(v^)+eps) + wd w ; w -= lr |w|/|u| u
+//   PARTIAL_ROWWISE_LAMB m element-wise as LAMB, v one value per row from mean_d(g^2) ; u and the step as LAMB
+//   LARS_SGD             lr' = lr eta |w| / (|g| + wd |w|) ; m = momentum m + lr' (g + wd w) ; w -= m
+//   ROWWISE_ADAGRAD  L2  s_row += mean_d((g + wd w)^2) ; w = (1 - mult wd) w - mult g
+//                    DEC s_row += mean_d(g^2)          ; w = (1 - lr wd) w - mult g
+// Phase 1 widens this lane's chunks of the row into registers, updates the moments and forms u (LARS keeps g), adding
+// up |w|^2 and |u|^2 (|g|^2); one group reduction; phase 2 applies the scaled step and stores the row.  The literal
+// formulas hold for degenerate rows too (|u| = 0, or |g| + wd |w| = 0: the row becomes NaN / inf as the arithmetic says).
+template <int G, int VEC, int CH>
+__device__ __forceinline__ void finish_run_norm(const BwdArgs& a, const BwdFeat& d, int64_t row, int64_t key,
+                                                float (&acc)[CH][VEC], int lane, const float4* pre_w,
+                                                const float4* pre_s) {
+  const int op = a.optimizer;
+  const bool lamb = op == TZK_OPT_LAMB, pr_lamb = op == TZK_OPT_PARTIAL_ROWWISE_LAMB, lars = op == TZK_OPT_LARS_SGD;
+  const bool rw_adagrad = op == TZK_OPT_ROWWISE_ADAGRAD;
+  if (a.max_gradient > 0.f) {
+#pragma unroll
+    for (int ch = 0; ch < CH; ++ch)
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) acc[ch][k] = clip_grad(a, acc[ch][k]);
+  }
+  const int64_t base = d.w_off + row * d.stride;
+  float w[CH][VEC];
+#pragma unroll
+  for (int ch = 0; ch < CH; ++ch) {
+    const int c = (ch * G + lane) * VEC;
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) w[ch][k] = 0.f;
+    if (c >= d.dim) continue;
+    if (a.w_f16) {
+      const __half* wph = reinterpret_cast<const __half*>(a.weights) + base + c;
+      if constexpr (VEC == 4) {
+        const uint2 raw = *reinterpret_cast<const uint2*>(wph);
+        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&raw.x));
+        const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&raw.y));
+        w[ch][0] = lo.x; w[ch][1] = lo.y; w[ch][2] = hi.x; w[ch][3] = hi.y;
+      } else {
+        w[ch][0] = __half2float(wph[0]);
+      }
+    } else if (pre_w) {
+      unpack4<VEC>(*pre_w, w[ch]);
+    } else {
+      load_vec<VEC>(a.weights + base + c, w[ch]);
+    }
+  }
+  // the row-wise second moment / accumulator: needs the row's sum of squares before u
+  float rw_denom = 1.f;
+  if (pr_lamb || rw_adagrad) {
+    const float wd_l2 = (rw_adagrad && a.wd_mode == 1) ? a.weight_decay : 0.f;
+    float ss = 0.f;
+#pragma unroll
+    for (int ch = 0; ch < CH; ++ch) {
+      const int c = (ch * G + lane) * VEC;
+#pragma unroll
+      for (int k = 0; k < VEC; ++k)
+        if (c + k < d.dim) {
+          const float gk = acc[ch][k] + wd_l2 * w[ch][k];
+          ss += gk * gk;
+        }
+    }
+    ss = group_sum<G>(ss);
+    float v = 0.f;
+    if (lane == 0) {
+      if (rw_adagrad) {
+        v = a.state[key] + ss / (float)d.dim;
+        a.state[key] = v;
+      } else {
+        v = a.beta2 * a.state2[key] + (1.f - a.beta2) * (ss / (float)d.dim);
+        a.state2[key] = v;
+      }
+    }
+    v = __shfl_sync(group_mask_of<G>(), v, 0, G);
+    rw_denom = rw_adagrad ? sqrtf(v) + a.eps : sqrtf(v / a.bc2) + a.eps;
+  }
+  // phase 1: moments, u (in acc), |w|^2 and |u|^2 (LARS: |g|^2)
+  float ww = 0.f, uu = 0.f;
+  if (!rw_adagrad) {
+#pragma unroll
+    for (int ch = 0; ch < CH; ++ch) {
+      const int c = (ch * G + lane) * VEC;
+      if (c >= d.dim) continue;
+      if (lamb || pr_lamb) {
+        float* sp = a.state + base + c;
+        float m[VEC];
+        if (pre_s) unpack4<VEC>(*pre_s, m);
+        else load_vec<VEC>(sp, m);
+        float v[VEC];
+        if (lamb) load_vec<VEC>(a.state2 + base + c, v);
+#pragma unroll
+        for (int k = 0; k < VEC; ++k) {
+          const float gk = acc[ch][k];
+          m[k] = a.beta1 * m[k] + (1.f - a.beta1) * gk;
+          float den = rw_denom;
+          if (lamb) {
+            v[k] = a.beta2 * v[k] + (1.f - a.beta2) * gk * gk;
+            den = sqrtf(v[k] / a.bc2) + a.eps;
+          }
+          acc[ch][k] = (m[k] / a.bc1) / den + a.weight_decay * w[ch][k];
+        }
+        store_vec<VEC>(sp, m);
+        if (lamb) store_vec<VEC>(a.state2 + base + c, v);
+      }
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) {
+        ww += w[ch][k] * w[ch][k];
+        uu += acc[ch][k] * acc[ch][k];
+      }
+    }
+    ww = group_sum<G>(ww);
+    uu = group_sum<G>(uu);
+  }
+  // phase 2: the step
+  float scale = 0.f, keep = 1.f, mult = 0.f;
+  if (lamb || pr_lamb) {
+    scale = a.lr * (sqrtf(ww) / sqrtf(uu));
+  } else if (lars) {
+    const float wn = sqrtf(ww);
+    scale = a.lr * a.beta2 * wn / (sqrtf(uu) + a.weight_decay * wn);   // beta2 = eta
+  } else {
+    mult = a.lr / rw_denom;
+    keep = a.wd_mode == 1 ? 1.f - mult * a.weight_decay : 1.f - a.lr * a.weight_decay;
+  }
+#pragma unroll
+  for (int ch = 0; ch < CH; ++ch) {
+    const int c = (ch * G + lane) * VEC;
+    if (c >= d.dim) continue;
+    if (lars) {
+      float* sp = a.state + base + c;
+      float m[VEC];
+      if (pre_s) unpack4<VEC>(*pre_s, m);
+      else load_vec<VEC>(sp, m);
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) {
+        m[k] = a.beta1 * m[k] + scale * (acc[ch][k] + a.weight_decay * w[ch][k]);   // beta1 = momentum
+        w[ch][k] = w[ch][k] - m[k];
+      }
+      store_vec<VEC>(sp, m);
+    } else if (rw_adagrad) {
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) w[ch][k] = keep * w[ch][k] - mult * acc[ch][k];
+    } else {
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) w[ch][k] = w[ch][k] - scale * acc[ch][k];
+    }
+    if (a.w_f16) {      // round to nearest even, as the classic update
+      __half* wph = reinterpret_cast<__half*>(a.weights) + base + c;
+      if constexpr (VEC == 4) {
+        uint2 raw;
+        *reinterpret_cast<__half2*>(&raw.x) = __floats2half2_rn(w[ch][0], w[ch][1]);
+        *reinterpret_cast<__half2*>(&raw.y) = __floats2half2_rn(w[ch][2], w[ch][3]);
+        *reinterpret_cast<uint2*>(wph) = raw;
+      } else {
+        wph[0] = __float2half_rn(w[ch][0]);
+      }
+    } else {
+      store_vec<VEC>(a.weights + base + c, w[ch]);
+    }
+  }
+}
+
 // finish a run: `acc` holds this lane's chunk(s) of the summed gradient.  Only called with all G lanes
 // of the group active (needed for the row-wise shuffle).
 // `pre_w` / `pre_s` (CH == 1, VEC == 4, fp32 tables): the row's weight / first-state chunk of this lane, already
 // requested by the caller (next to the gradient rows instead of after them).
-template <int G, int VEC, int CH>
+template <int G, int VEC, int CH, int FAM = kFamClassic>
 __device__ __forceinline__ void finish_run(const BwdArgs& a, const BwdFeat& d, int64_t row, int64_t key,
                                            float (&acc)[CH][VEC], int lane, const float4* pre_w = nullptr,
                                            const float4* pre_s = nullptr) {
+  if constexpr (FAM == kFamNorm) {
+    finish_run_norm<G, VEC, CH>(a, d, row, key, acc, lane, pre_w, pre_s);
+    return;
+  }
   if (a.optimizer == TZK_OPT_ACCUM_OUT) {
 #pragma unroll
     for (int ch = 0; ch < CH; ++ch) {
@@ -594,7 +797,7 @@ find_long_runs_kernel(const KeyT* __restrict__ keys, int64_t n, KeyT sentinel, W
 // is consumed, so a group keeps 3*kPos independent 64-B requests in flight instead of one dependent chain.
 // One short run (<= kShortRun sorted positions starting at p, key k0, first value v0): sum its gradient rows in sorted
 // order, ONE optimizer update.  All G lanes of the group call it together.
-template <typename KeyT, int G, int VEC, int CH>
+template <typename KeyT, int G, int VEC, int CH, int FAM>
 __device__ __forceinline__ void short_run(const BwdArgs& a, const PeerGrads& gp, const BwdFeat* fd,
                                           const int32_t* __restrict__ vals, int64_t p, KeyT k0, int32_t v0, int len,
                                           int lane) {
@@ -610,7 +813,7 @@ __device__ __forceinline__ void short_run(const BwdArgs& a, const PeerGrads& gp,
     if (pre && lane * 4 < d.dim) {
       const float* wp = a.weights + d.w_off + row * d.stride + lane * 4;
       pre_w = ld_rw_f4(wp);
-      if (has_elem_state(a)) pre_s = ld_rw_f4(a.interleaved ? wp + d.dim : a.state + (d.w_off + row * d.stride + lane * 4));
+      if (elem_state<FAM>(a)) pre_s = ld_rw_f4(a.interleaved ? wp + d.dim : a.state + (d.w_off + row * d.stride + lane * 4));
     }
     float acc[CH][VEC];
 #pragma unroll
@@ -652,11 +855,11 @@ __device__ __forceinline__ void short_run(const BwdArgs& a, const PeerGrads& gp,
       }
     }
     // (one call site: the row-wise variants shuffle inside, every lane of the group must arrive at the same instruction)
-    finish_run<G, VEC, CH>(a, d, row, (int64_t)k0, acc, lane, pre ? &pre_w : nullptr,
-                           (pre && has_elem_state(a)) ? &pre_s : nullptr);
+    finish_run<G, VEC, CH, FAM>(a, d, row, (int64_t)k0, acc, lane, pre ? &pre_w : nullptr,
+                                (pre && elem_state<FAM>(a)) ? &pre_s : nullptr);
 }
 
-template <typename KeyT, int G, int VEC, int CH>
+template <typename KeyT, int G, int VEC, int CH, int FAM>
 __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrads& gp, const BwdFeat* fd,
                                                 const KeyT* __restrict__ keys,
                                                 const int32_t* __restrict__ vals, const WorkLists& wl, int cta,
@@ -676,7 +879,7 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
       const int64_t p = hp;
       const int len = hl;
       if (h + stride < n_heads) { hp = wl.head_pos[h + stride]; hl = wl.head_len[h + stride]; }   // next head, early
-      short_run<KeyT, G, VEC, CH>(a, gp, fd, vals, p, keys[p], vals[p], len, lane);
+      short_run<KeyT, G, VEC, CH, FAM>(a, gp, fd, vals, p, keys[p], vals[p], len, lane);
     }
     return;
   }
@@ -711,7 +914,7 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
       while (len <= kShortRun && p0 + len < a.n && keys[p0 + len] == key_c) ++len;
     }
     if (len > kShortRun) continue;
-    short_run<KeyT, G, VEC, CH>(a, gp, fd, vals, p0, key_c, v_c, len, lane);
+    short_run<KeyT, G, VEC, CH, FAM>(a, gp, fd, vals, p0, key_c, v_c, len, lane);
   }
 }
 
@@ -722,7 +925,7 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
 // the update — the order of the additions is fixed by the sorted positions, whoever happens to execute them.
 // These CTAs ride in the same launch as the short-run CTAs (fused_apply_kernel): tiny tables / hot ids and the big
 // tables' rows are updated side by side instead of in three dependent launches.
-template <typename KeyT, int G, int VEC, int CH>
+template <typename KeyT, int G, int VEC, int CH, int FAM>
 __device__ __forceinline__ void long_chunk_body(const BwdArgs& a, const PeerGrads& gp, const BwdFeat* fd,
                                                 const KeyT* __restrict__ keys,
                                                 const int32_t* __restrict__ vals, const WorkLists& wl, int cta,
@@ -785,7 +988,7 @@ __device__ __forceinline__ void long_chunk_body(const BwdArgs& a, const PeerGrad
     }
     if (gw == 0) {
       if (it.n_chunks == 1) {
-        finish_run<G, VEC, CH>(a, d, row, (int64_t)key, acc, lane);
+        finish_run<G, VEC, CH, FAM>(a, d, row, (int64_t)key, acc, lane);
       } else {
         float* dst = wl.partials + (int64_t)(it.pbase + it.cc) * ROWF;
 #pragma unroll
@@ -809,7 +1012,7 @@ __device__ __forceinline__ void long_chunk_body(const BwdArgs& a, const PeerGrad
 #pragma unroll
               for (int k = 0; k < VEC; ++k) acc[ch][k] += __ldcg(src + (ch * G + lane) * VEC + k);
           }
-          finish_run<G, VEC, CH>(a, d, row, (int64_t)key, acc, lane);
+          finish_run<G, VEC, CH, FAM>(a, d, row, (int64_t)key, acc, lane);
           if (lane == 0) wl.run_done[it.pbase] = 0;         // the list can be replayed (same sort, another gradient)
         }
       }
@@ -819,7 +1022,7 @@ __device__ __forceinline__ void long_chunk_body(const BwdArgs& a, const PeerGrad
 }
 
 // ---- 3 + 4 in one launch: CTAs [0, n_short) walk the sorted positions (short runs), the rest serve the long-run list
-template <typename KeyT, int G, int VEC, int CH>
+template <typename KeyT, int G, int VEC, int CH, int FAM>
 __global__ void __launch_bounds__(kThreads, CH == 1 ? 4 : 1)     // 4 CTAs / SM: 64 registers (weight / state prefetch + 2 gradient rows in flight)
 fused_apply_kernel(BwdArgs a, const int64_t* __restrict__ feat_w_off, const int64_t* __restrict__ feat_rows,
                    const int64_t* __restrict__ feat_key_base, const int32_t* __restrict__ feat_dim,
@@ -829,11 +1032,11 @@ fused_apply_kernel(BwdArgs a, const int64_t* __restrict__ feat_w_off, const int6
   extern __shared__ __align__(16) unsigned char smem_raw[];
   BwdFeat* fd = reinterpret_cast<BwdFeat*>(smem_raw);
   stage_feats(fd, feat_w_off, feat_rows, feat_key_base, feat_dim, feat_col, feat_pool, a.F, a.interleaved);
-  init_bias_correction(a);
+  init_bias_correction<FAM>(a);
   // the long-run CTAs come FIRST in the grid: they are few, each has a lot to do, and the hardware starts CTAs in
   // index order — their work overlaps the whole short-run sweep instead of trailing it
-  if ((int)blockIdx.x < n_long) long_chunk_body<KeyT, G, VEC, CH>(a, gp, fd, keys, vals, wl, blockIdx.x, n_long);
-  else run_update_body<KeyT, G, VEC, CH>(a, gp, fd, keys, vals, wl, blockIdx.x - n_long, gridDim.x - n_long);
+  if ((int)blockIdx.x < n_long) long_chunk_body<KeyT, G, VEC, CH, FAM>(a, gp, fd, keys, vals, wl, blockIdx.x, n_long);
+  else run_update_body<KeyT, G, VEC, CH, FAM>(a, gp, fd, keys, vals, wl, blockIdx.x - n_long, gridDim.x - n_long);
 }
 
 // ---- 3'. tile path: rows of <= 128 floats, 16-B aligned (vec4, one chunk per lane) -------------------------
@@ -1149,27 +1352,50 @@ WsLayout ws_layout(int64_t nnz, int64_t total_keys, int max_dim) {
 
 }  // namespace
 
-#define TZK_BWD_LAUNCH(KeyT, G_, VEC_, CH_)                                                          \
+#define TZK_BWD_LAUNCH(KeyT, G_, VEC_, CH_, FAM_)                                                    \
   do {                                                                                                \
     size_t smem_s = (size_t)F * sizeof(BwdFeat);                                                      \
     if (smem_s > 48 * 1024)                                                                           \
-      cudaFuncSetAttribute(fused_apply_kernel<KeyT, G_, VEC_, CH_>,                                   \
+      cudaFuncSetAttribute(fused_apply_kernel<KeyT, G_, VEC_, CH_, FAM_>,                             \
                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s);                 \
-    fused_apply_kernel<KeyT, G_, VEC_, CH_><<<grid_s + n_long, kThreads, smem_s, st>>>(               \
+    fused_apply_kernel<KeyT, G_, VEC_, CH_, FAM_><<<grid_s + n_long, kThreads, smem_s, st>>>(         \
         a, feat_w_off, feat_rows, feat_key_base, feat_dim, feat_col, feat_pool, (const KeyT*)keys_out, \
         vals_out, wl, n_long, gp);                                                                    \
     TZK_CHECK_LAUNCH("fused_apply_kernel");                                                           \
   } while (0)
 
-#define TZK_BWD_DISPATCH_G(KeyT, VEC_, CH_)                 \
-  switch (G) {                                              \
-    case 1: TZK_BWD_LAUNCH(KeyT, 1, VEC_, CH_); break;      \
-    case 2: TZK_BWD_LAUNCH(KeyT, 2, VEC_, CH_); break;      \
-    case 4: TZK_BWD_LAUNCH(KeyT, 4, VEC_, CH_); break;      \
-    case 8: TZK_BWD_LAUNCH(KeyT, 8, VEC_, CH_); break;      \
-    case 16: TZK_BWD_LAUNCH(KeyT, 16, VEC_, CH_); break;    \
-    default: TZK_BWD_LAUNCH(KeyT, 32, VEC_, CH_); break;    \
+#define TZK_BWD_DISPATCH_G(KeyT, VEC_, CH_, FAM_)                 \
+  switch (G) {                                                    \
+    case 1: TZK_BWD_LAUNCH(KeyT, 1, VEC_, CH_, FAM_); break;      \
+    case 2: TZK_BWD_LAUNCH(KeyT, 2, VEC_, CH_, FAM_); break;      \
+    case 4: TZK_BWD_LAUNCH(KeyT, 4, VEC_, CH_, FAM_); break;      \
+    case 8: TZK_BWD_LAUNCH(KeyT, 8, VEC_, CH_, FAM_); break;      \
+    case 16: TZK_BWD_LAUNCH(KeyT, 16, VEC_, CH_, FAM_); break;    \
+    default: TZK_BWD_LAUNCH(KeyT, 32, VEC_, CH_, FAM_); break;    \
   }
+
+// general path, every (key width, VEC, G, CH) of one optimizer family
+#define TZK_BWD_DISPATCH(FAM_)                                                                                         \
+  do {                                                                                                                 \
+    if (k64) {                                                                                                         \
+      if (vec == 4) { if (ch == 1) { TZK_BWD_DISPATCH_G(uint64_t, 4, 1, FAM_) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint64_t, 32, 4, 2, FAM_); } else { TZK_BWD_LAUNCH(uint64_t, 32, 4, 8, FAM_); } } \
+      else { if (ch == 1) { TZK_BWD_DISPATCH_G(uint64_t, 1, 1, FAM_) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint64_t, 32, 1, 2, FAM_); } else { TZK_BWD_LAUNCH(uint64_t, 32, 1, 8, FAM_); } } \
+    } else {                                                                                                           \
+      if (vec == 4) { if (ch == 1) { TZK_BWD_DISPATCH_G(uint32_t, 4, 1, FAM_) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint32_t, 32, 4, 2, FAM_); } else { TZK_BWD_LAUNCH(uint32_t, 32, 4, 8, FAM_); } } \
+      else { if (ch == 1) { TZK_BWD_DISPATCH_G(uint32_t, 1, 1, FAM_) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint32_t, 32, 1, 2, FAM_); } else { TZK_BWD_LAUNCH(uint32_t, 32, 1, 8, FAM_); } } \
+    }                                                                                                                  \
+  } while (0)
+
+// kFamNorm: the optimizers of finish_run_norm (row-wise Adagrad only with a weight decay mode and a nonzero decay;
+// without them it is the classic update)
+static bool norm_family(const tzk_opt_args& o) {
+  return o.optimizer == TZK_OPT_LAMB || o.optimizer == TZK_OPT_PARTIAL_ROWWISE_LAMB || o.optimizer == TZK_OPT_LARS_SGD ||
+         (o.optimizer == TZK_OPT_ROWWISE_ADAGRAD && o.weight_decay_mode != 0 && o.weight_decay != 0.f);
+}
+static bool elem_state_opt(int32_t optimizer) {   // first state laid out like the weights
+  return optimizer == TZK_OPT_ADAGRAD || optimizer == TZK_OPT_ADAM || optimizer == TZK_OPT_PARTIAL_ROWWISE_ADAM ||
+         optimizer == TZK_OPT_LAMB || optimizer == TZK_OPT_PARTIAL_ROWWISE_LAMB || optimizer == TZK_OPT_LARS_SGD;
+}
 
 extern "C" size_t tzk_fused_bwd_workspace_bytes(int64_t nnz, int64_t total_keys, int32_t max_dim) {
   return ws_layout(nnz, total_keys, max_dim < 1 ? 1 : max_dim).total;
@@ -1189,7 +1415,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   const int32_t optimizer = opt.optimizer;
   float* state = opt.state;
   const float lr = opt.lr, eps = opt.eps;
-  TZK_REQUIRE((optimizer >= 0 && optimizer <= TZK_OPT_PARTIAL_ROWWISE_ADAM) || optimizer == TZK_OPT_ACCUM_OUT,
+  TZK_REQUIRE((optimizer >= 0 && optimizer <= TZK_OPT_LARS_SGD) || optimizer == TZK_OPT_ACCUM_OUT,
               "fused_bwd: unknown optimizer %d", optimizer);
   TZK_REQUIRE(F >= 0 && B >= 0 && nnz >= 0, "fused_bwd: negative size");
   if (F == 0 || B == 0 || nnz == 0) return 0;
@@ -1204,8 +1430,11 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
     TZK_REQUIRE(optimizer == TZK_OPT_SGD || state != nullptr || opt.interleaved, "fused_bwd: optimizer state is NULL");
     TZK_REQUIRE(!opt.interleaved || (optimizer == TZK_OPT_ADAGRAD && !opt.weights_f16),
                 "fused_bwd: interleaved [weight | state] rows are implemented for fp32 tables with element-wise Adagrad");
-    TZK_REQUIRE((optimizer != TZK_OPT_ADAM && optimizer != TZK_OPT_PARTIAL_ROWWISE_ADAM) || (opt.state2 && opt.step),
-                "fused_bwd: Adam variants need state2 and the device step counter");
+    TZK_REQUIRE((optimizer != TZK_OPT_ADAM && optimizer != TZK_OPT_PARTIAL_ROWWISE_ADAM &&
+                 optimizer != TZK_OPT_LAMB && optimizer != TZK_OPT_PARTIAL_ROWWISE_LAMB) || (opt.state2 && opt.step),
+                "fused_bwd: Adam and LAMB variants need state2 and the device step counter");
+    TZK_REQUIRE(optimizer != TZK_OPT_ROWWISE_ADAGRAD || (opt.weight_decay_mode >= 0 && opt.weight_decay_mode <= 2),
+                "fused_bwd: weight_decay_mode %d is not NONE (0), L2 (1) or DECOUPLE (2)", opt.weight_decay_mode);
   }
   TZK_REQUIRE(F <= 2048, "fused_bwd: F=%d > 2048 keys per collection", F);
   TZK_REQUIRE(max_dim >= 1 && max_dim <= 1024, "fused_bwd: max_dim=%d out of range [1,1024]", max_dim);
@@ -1307,7 +1536,9 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   a.peer_w = 0; a.idx_span = 1; a.w_f16 = opt.weights_f16 ? 1 : 0; a.interleaved = opt.interleaved ? 1 : 0;
   a.div_b = make_fast_div(B); a.div_span = make_fast_div(1);
   TZK_REQUIRE(ld_grad >= 0 && ld_grad < ((int64_t)1 << 31), "fused_bwd: ld_grad out of range");
-  a.ld32 = (int32_t)ld_grad; a.pad3 = 0;
+  a.ld32 = (int32_t)ld_grad; a.wd_mode = opt.weight_decay_mode;
+  if (optimizer == TZK_OPT_LARS_SGD) { a.beta1 = opt.momentum; a.beta2 = opt.eta; }
+  const int fam = norm_family(opt) ? kFamNorm : kFamClassic;
   PeerGrads gp;
   for (int r = 0; r < 16; ++r) gp.p[r] = 0ull;
   if (pw) {
@@ -1323,9 +1554,8 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   const int vec = (vec_ok && peers_aligned && ((uintptr_t)weights % (a.w_f16 ? 8 : 16) == 0) &&
                    ((uintptr_t)a.grad_out % 16 == 0) &&
                    (ld_grad % 4 == 0) &&
-                   (!(optimizer == TZK_OPT_ADAGRAD || optimizer == TZK_OPT_ADAM ||
-                      optimizer == TZK_OPT_PARTIAL_ROWWISE_ADAM) || opt.interleaved || (uintptr_t)state % 16 == 0) &&
-                   (optimizer != TZK_OPT_ADAM || (uintptr_t)opt.state2 % 16 == 0))
+                   (!elem_state_opt(optimizer) || opt.interleaved || (uintptr_t)state % 16 == 0) &&
+                   ((optimizer != TZK_OPT_ADAM && optimizer != TZK_OPT_LAMB) || (uintptr_t)opt.state2 % 16 == 0))
                       ? 4 : 1;
   int need = (max_dim + vec - 1) / vec;  // chunks per row
   int G = 1;
@@ -1337,9 +1567,10 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   int grid_s = (int)std::min<int64_t>(ceil_div64(nnz, NG), kSmCountH100 * 16);
   // TZK_BWD_TILE=1 selects the tile path.  Both paths are bound by the random 64-B weight/state/gradient accesses of
   // the gradient half, and the general kernels execute fewer instructions without the three barriers per tile, so
-  // they stay the default.
+  // they stay the default.  The kFamNorm optimizers always take the general path.
   const char* tile_env = getenv("TZK_BWD_TILE");
-  const bool tile_path = tile_env && tile_env[0] == '1' && !a.w_f16 && !a.interleaved && optimizer != TZK_OPT_ACCUM_OUT;   // (fp32 tables, real updates)
+  const bool tile_path = tile_env && tile_env[0] == '1' && !a.w_f16 && !a.interleaved && optimizer != TZK_OPT_ACCUM_OUT &&
+                         fam == kFamClassic;   // (fp32 tables, real classic updates)
   if (vec == 4 && ch == 1 && tile_path) {
     // tile path: every gradient / weight / state row of a tile is requested at once, runs are reduced in shared memory
     float* carry_first = reinterpret_cast<float*>(ws + L.carry);
@@ -1387,13 +1618,8 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
 
   // general path: one launch — short runs by sorted position + the long-run list's chunk CTAs (CH compiled for 1, 2, 8)
   const int n_long = kSmCountH100 * 2;
-  if (k64) {
-    if (vec == 4) { if (ch == 1) { TZK_BWD_DISPATCH_G(uint64_t, 4, 1) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint64_t, 32, 4, 2); } else { TZK_BWD_LAUNCH(uint64_t, 32, 4, 8); } }
-    else { if (ch == 1) { TZK_BWD_DISPATCH_G(uint64_t, 1, 1) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint64_t, 32, 1, 2); } else { TZK_BWD_LAUNCH(uint64_t, 32, 1, 8); } }
-  } else {
-    if (vec == 4) { if (ch == 1) { TZK_BWD_DISPATCH_G(uint32_t, 4, 1) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint32_t, 32, 4, 2); } else { TZK_BWD_LAUNCH(uint32_t, 32, 4, 8); } }
-    else { if (ch == 1) { TZK_BWD_DISPATCH_G(uint32_t, 1, 1) } else if (ch <= 2) { TZK_BWD_LAUNCH(uint32_t, 32, 1, 2); } else { TZK_BWD_LAUNCH(uint32_t, 32, 1, 8); } }
-  }
+  if (fam == kFamNorm) TZK_BWD_DISPATCH(kFamNorm);
+  else TZK_BWD_DISPATCH(kFamClassic);
   return 0;
 }
 
@@ -1401,6 +1627,7 @@ static tzk_opt_args classic_opt(int32_t optimizer, float* state, float lr, float
   tzk_opt_args o;
   o.optimizer = optimizer; o.lr = lr; o.eps = eps; o.beta1 = 0.9f; o.beta2 = 0.999f; o.weight_decay = 0.f;
   o.max_gradient = 0.f; o.state = state; o.state2 = nullptr; o.step = nullptr; o.weights_f16 = 0; o.interleaved = 0;
+  o.momentum = 0.f; o.eta = 0.f; o.weight_decay_mode = 0;
   return o;
 }
 
@@ -1484,7 +1711,7 @@ struct SmallTab {
 };
 struct SmallPeers { unsigned long long psum[16], flags[16]; };
 
-template <int G>
+template <int G, int FAM>
 __global__ void __launch_bounds__(kThreads)
 small_table_update_kernel(BwdArgs a, const __grid_constant__ SmallPeers sp, const SmallTab* __restrict__ tabs, int n_tabs,
                           int total_rows, int W) {
@@ -1492,7 +1719,7 @@ small_table_update_kernel(BwdArgs a, const __grid_constant__ SmallPeers sp, cons
   SmallTab* st = reinterpret_cast<SmallTab*>(smem_raw);
   for (int i = threadIdx.x; i < n_tabs; i += blockDim.x) st[i] = tabs[i];
   __syncthreads();
-  init_bias_correction(a);
+  init_bias_correction<FAM>(a);
   constexpr int NG = kThreads / G;
   const int lane = threadIdx.x % G;
   for (int j = blockIdx.x * NG + threadIdx.x / G; j < total_rows; j += gridDim.x * NG) {
@@ -1530,7 +1757,7 @@ small_table_update_kernel(BwdArgs a, const __grid_constant__ SmallPeers sp, cons
     BwdFeat d;
     d.w_off = t.w_off; d.rows = t.n_local; d.key_base = t.key_base; d.dim = t.dim; d.col = 0; d.pool = 0;
     d.stride = a.interleaved ? 2 * t.dim : t.dim;
-    finish_run<G, 4, 1>(a, d, i, t.key_base + i, acc, lane);
+    finish_run<G, 4, 1, FAM>(a, d, i, t.key_base + i, acc, lane);
   }
 }
 
@@ -1545,16 +1772,23 @@ extern "C" int tzk_peer_small_update(const tzk_opt_args* opt, const uint64_t* ps
   if (n_tabs == 0 || total_rows == 0) return 0;
   TZK_REQUIRE(tabs && weights && max_dim >= 4 && max_dim <= 128 && max_dim % 4 == 0 && n_tabs <= 1024,
               "peer_small_update: dims must be multiples of 4 and <= 128");
-  TZK_REQUIRE(opt->optimizer >= 0 && opt->optimizer <= TZK_OPT_PARTIAL_ROWWISE_ADAM && !opt->weights_f16,
+  TZK_REQUIRE(opt->optimizer >= 0 && opt->optimizer <= TZK_OPT_LARS_SGD && !opt->weights_f16,
               "peer_small_update: unsupported optimizer");
   TZK_REQUIRE(opt->optimizer == TZK_OPT_SGD || opt->state, "peer_small_update: optimizer state is NULL");
+  TZK_REQUIRE(!norm_family(*opt) || !opt->interleaved, "peer_small_update: interleaved rows are Adagrad only");
+  TZK_REQUIRE((opt->optimizer != TZK_OPT_ADAM && opt->optimizer != TZK_OPT_PARTIAL_ROWWISE_ADAM &&
+               opt->optimizer != TZK_OPT_LAMB && opt->optimizer != TZK_OPT_PARTIAL_ROWWISE_LAMB) ||
+                  (opt->state2 && opt->step),
+              "peer_small_update: Adam and LAMB variants need state2 and the device step counter");
   BwdArgs a;
   a.grad_out = nullptr; a.ld_grad = 0; a.offsets = nullptr; a.weights = weights; a.state = opt->state;
   a.lr = opt->lr; a.eps = opt->eps; a.grad_scale = 1.f; a.F = 0; a.B = 1; a.optimizer = opt->optimizer; a.pooled = 0;
   a.n = total_rows; a.sentinel = 0; a.state2 = opt->state2; a.step = opt->step; a.beta1 = opt->beta1; a.beta2 = opt->beta2;
   a.weight_decay = opt->weight_decay; a.max_gradient = opt->max_gradient; a.bc1 = a.bc2 = 1.f;
   a.peer_w = 0; a.idx_span = 1; a.w_f16 = 0; a.interleaved = opt->interleaved ? 1 : 0;
-  a.div_b = make_fast_div(1); a.div_span = make_fast_div(1); a.ld32 = 0; a.pad3 = 0;
+  a.div_b = make_fast_div(1); a.div_span = make_fast_div(1); a.ld32 = 0; a.wd_mode = opt->weight_decay_mode;
+  if (opt->optimizer == TZK_OPT_LARS_SGD) { a.beta1 = opt->momentum; a.beta2 = opt->eta; }
+  const bool norm = norm_family(*opt);
   SmallPeers sp;
   for (int r = 0; r < 16; ++r) { sp.psum[r] = r < W ? psum_ptrs[r] : 0ull; sp.flags[r] = r < W ? flag_ptrs[r] : 0ull; }
   int G = 1;
@@ -1564,14 +1798,20 @@ extern "C" int tzk_peer_small_update(const tzk_opt_args* opt, const uint64_t* ps
   const size_t smem = (size_t)n_tabs * sizeof(SmallTab);
   cudaStream_t st = as_stream(stream);
   const SmallTab* tp = static_cast<const SmallTab*>(tabs);
+#define TZK_SMALL_LAUNCH(G_)                                                                                     \
+  do {                                                                                                           \
+    if (norm) small_table_update_kernel<G_, kFamNorm><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); \
+    else small_table_update_kernel<G_, kFamClassic><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); \
+  } while (0)
   switch (G) {
-    case 1: small_table_update_kernel<1><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); break;
-    case 2: small_table_update_kernel<2><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); break;
-    case 4: small_table_update_kernel<4><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); break;
-    case 8: small_table_update_kernel<8><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); break;
-    case 16: small_table_update_kernel<16><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); break;
-    default: small_table_update_kernel<32><<<grid, kThreads, smem, st>>>(a, sp, tp, n_tabs, total_rows, W); break;
+    case 1: TZK_SMALL_LAUNCH(1); break;
+    case 2: TZK_SMALL_LAUNCH(2); break;
+    case 4: TZK_SMALL_LAUNCH(4); break;
+    case 8: TZK_SMALL_LAUNCH(8); break;
+    case 16: TZK_SMALL_LAUNCH(16); break;
+    default: TZK_SMALL_LAUNCH(32); break;
   }
+#undef TZK_SMALL_LAUNCH
   TZK_CHECK_LAUNCH("small_table_update_kernel");
   return 0;
 }

@@ -20,8 +20,13 @@ import torch
 from torch import nn
 
 from . import functional as Fn
-from .kernels import (OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM, OPT_ROWWISE_ADAGRAD, OPT_SGD, POOL_MEAN, POOL_SUM,
-                      FeatureLayout, build_layout)
+from .kernels import (LARS_ETA, OPT_ADAGRAD, OPT_ADAM, OPT_LAMB, OPT_LARS_SGD, OPT_PARTIAL_ROWWISE_ADAM,
+                      OPT_PARTIAL_ROWWISE_LAMB, OPT_ROWWISE_ADAGRAD, OPT_SGD, POOL_MEAN, POOL_SUM, WD_NONE, FeatureLayout,
+                      build_layout)
+
+# kinds whose first state (`momentum1`) is laid out like the weights, and kinds with a second state and a step counter
+ELEMENTWISE_STATE_KINDS = (OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM, OPT_LAMB, OPT_PARTIAL_ROWWISE_LAMB, OPT_LARS_SGD)
+ADAM_LIKE_KINDS = (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM, OPT_LAMB, OPT_PARTIAL_ROWWISE_LAMB)
 from .sparse import JaggedTensor, KeyedJaggedTensor, KeyedTensor
 
 
@@ -67,16 +72,20 @@ class SparseOptimizerSpec:
     lr: float = 0.001
     eps: float = 1e-8                      # fbgemm TBE default (App. A.10)
     initial_accumulator_value: float = 0.0  # optimizer_builder.py:57-61
-    beta1: float = 0.9                      # Adam variants (optimizer.proto:89-131)
+    beta1: float = 0.9                      # Adam / LAMB variants (optimizer.proto:89-131)
     beta2: float = 0.999
     weight_decay: float = 0.0
     max_gradient: float = 0.0               # > 0 <=> gradient_clipping: clamp the summed row gradient
+    momentum: float = 0.9                   # LARS-SGD (FusedLarsSGDOptimizer.momentum)
+    eta: float = LARS_ETA                   # LARS-SGD trust coefficient: fbgemm's default, tzrec passes none
+    weight_decay_mode: int = WD_NONE        # row-wise Adagrad: kernels.WD_NONE / WD_L2 / WD_DECOUPLE
 
     @staticmethod
     def from_name(name: str, **kw) -> "SparseOptimizerSpec":
         kinds = {"sgd": OPT_SGD, "adagrad": OPT_ADAGRAD, "rowwise_adagrad": OPT_ROWWISE_ADAGRAD,
                  "row_wise_adagrad": OPT_ROWWISE_ADAGRAD, "adam": OPT_ADAM,
-                 "partial_rowwise_adam": OPT_PARTIAL_ROWWISE_ADAM}
+                 "partial_rowwise_adam": OPT_PARTIAL_ROWWISE_ADAM, "lamb": OPT_LAMB,
+                 "partial_rowwise_lamb": OPT_PARTIAL_ROWWISE_LAMB, "lars_sgd": OPT_LARS_SGD}
         return SparseOptimizerSpec(kind=kinds[name.lower()], **kw)
 
 
@@ -205,7 +214,7 @@ class _ArenaCollection(nn.Module):
             return self.weights.data[o:o + r * 2 * d].view(r, 2 * d)[:, d:]
         if self.opt_state is None:
             return None
-        if self._opt.kind in (OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM):
+        if self._opt.kind in ELEMENTWISE_STATE_KINDS:
             o = self._table_off[t]
             return self.opt_state[o:o + self._table_rows[t] * self._table_dim[t]].view(self._table_rows[t], -1)
         k = self._table_key[t]
@@ -332,14 +341,16 @@ class _ArenaCollection(nn.Module):
         elif spec.kind == OPT_ROWWISE_ADAGRAD:
             self.opt_state = torch.full((self.layout.total_keys,), spec.initial_accumulator_value,
                                         dtype=torch.float32, device=dev)
-        elif spec.kind in (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM):
+        elif spec.kind in ADAM_LIKE_KINDS:
             self.opt_state = torch.zeros(self.layout.arena_elems, dtype=torch.float32, device=dev)    # momentum1
-            n2 = self.layout.arena_elems if spec.kind == OPT_ADAM else self.layout.total_keys
+            n2 = self.layout.arena_elems if spec.kind in (OPT_ADAM, OPT_LAMB) else self.layout.total_keys
             self.opt_state2 = torch.zeros(n2, dtype=torch.float32, device=dev)                        # momentum2
             self.opt_step = torch.zeros((), dtype=torch.float32, device=dev)                          # iteration t
+        elif spec.kind == OPT_LARS_SGD:
+            self.opt_state = torch.zeros(self.layout.arena_elems, dtype=torch.float32, device=dev)    # momentum1
         else:
             self.opt_state = None
-        if spec.kind not in (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM):
+        if spec.kind not in ADAM_LIKE_KINDS:
             self.opt_state2, self.opt_step = None, None
 
     def opt_extras(self, bump: bool = True) -> dict:
@@ -349,11 +360,16 @@ class _ArenaCollection(nn.Module):
         if spec is None:
             return {}
         ex = {}
-        if spec.kind in (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM):
+        if spec.kind in ADAM_LIKE_KINDS:
             if bump:
                 self.opt_step.add_(1.0)
             ex.update(state2=self.opt_state2, step=self.opt_step, beta1=spec.beta1, beta2=spec.beta2,
                       weight_decay=spec.weight_decay)
+        elif spec.kind == OPT_LARS_SGD:
+            ex.update(momentum=spec.momentum, eta=spec.eta, weight_decay=spec.weight_decay)
+        elif spec.kind == OPT_ROWWISE_ADAGRAD and spec.weight_decay_mode != WD_NONE and spec.weight_decay != 0:
+            # (mode NONE, or no decay: the classic row-wise update, as fbgemm ignores weight_decay then)
+            ex.update(weight_decay=spec.weight_decay, weight_decay_mode=spec.weight_decay_mode)
         if spec.max_gradient > 0 or ex:
             ex["max_gradient"] = spec.max_gradient
         return ex

@@ -18,6 +18,9 @@ from ._lib import TzkError, check, lib
 
 POOL_SUM, POOL_MEAN = 0, 1
 OPT_SGD, OPT_ADAGRAD, OPT_ROWWISE_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM = 0, 1, 2, 3, 4
+OPT_LAMB, OPT_PARTIAL_ROWWISE_LAMB, OPT_LARS_SGD = 5, 6, 7      # the layer-wise adaptive optimizers (_ex entry points)
+WD_NONE, WD_L2, WD_DECOUPLE = 0, 1, 2    # row-wise Adagrad weight_decay_mode (tzrec WeightDecayMode)
+LARS_ETA = 0.001                         # fbgemm's default trust coefficient (tzrec passes none)
 OPT_ACCUM_OUT = 100      # peer-memory step: per-row gradient sums into a dense buffer instead of an update
 
 
@@ -159,10 +162,18 @@ def _small_linear_rows_path(K: int, N: int) -> bool:
     return t <= 128
 
 
-def _tile_path(lay: "FeatureLayout") -> bool:
+def norm_family(optimizer: int, ex: dict) -> bool:
+    """Mirrors norm_family() of csrc/tzk_bwd.cu: the updates with a norm over the row, which run on the general path."""
+    return optimizer in (OPT_LAMB, OPT_PARTIAL_ROWWISE_LAMB, OPT_LARS_SGD) or (
+        optimizer == OPT_ROWWISE_ADAGRAD and int(ex.get("weight_decay_mode", WD_NONE)) != WD_NONE
+        and float(ex.get("weight_decay", 0.0)) != 0.0)
+
+
+def _tile_path(lay: "FeatureLayout", optimizer: int = OPT_SGD, ex: Optional[dict] = None) -> bool:
     import os
 
-    return os.environ.get("TZK_BWD_TILE", "0") == "1" and bool(lay.vec_ok) and lay.max_dim <= 128 and not lay.interleaved
+    return (os.environ.get("TZK_BWD_TILE", "0") == "1" and bool(lay.vec_ok) and lay.max_dim <= 128 and not lay.interleaved
+            and not norm_family(optimizer, ex or {}))
 
 
 def _table_dtype(weights: torch.Tensor, name: str = "weights") -> bool:
@@ -181,15 +192,16 @@ def _opt_args(optimizer: int, state, lr: float, eps: float, ex: dict):
     from ._lib import TzkOptArgs
 
     st2, step = ex.get("state2"), ex.get("step")
-    if optimizer in (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM) and (st2 is None or step is None):
-        raise TzkError("Adam variants need state2 and the device step counter")
+    if optimizer in (OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM, OPT_LAMB, OPT_PARTIAL_ROWWISE_LAMB) and (st2 is None or step is None):
+        raise TzkError("Adam and LAMB variants need state2 and the device step counter")
     for t, nm in ((st2, "state2"), (step, "step")):
         if t is not None:
             _need(t, torch.float32, nm)
     return TzkOptArgs(optimizer, lr, eps, float(ex.get("beta1", 0.9)), float(ex.get("beta2", 0.999)),
                       float(ex.get("weight_decay", 0.0)), float(ex.get("max_gradient", 0.0)),
                       _ptr(state), _ptr(st2), _ptr(step), int(bool(ex.get("weights_f16", False))),
-                      int(bool(ex.get("interleaved", False))))
+                      int(bool(ex.get("interleaved", False))), float(ex.get("momentum", 0.9)),
+                      float(ex.get("eta", LARS_ETA)), int(ex.get("weight_decay_mode", WD_NONE)))
 
 
 class CudaKernels:
@@ -282,7 +294,8 @@ class CudaKernels:
     def fused_bwd(self, optimizer: int, pooled: bool, grad_out: torch.Tensor, weights: torch.Tensor,
                   state: Optional[torch.Tensor], lay: FeatureLayout, ids: torch.Tensor, offsets: torch.Tensor,
                   B: int, lr: float, eps: float, grad_scale: float = 1.0, **ex) -> None:
-        """`ex` (optional): state2, step, beta1, beta2, weight_decay, max_gradient -> tzk_fused_bwd_ex."""
+        """`ex` (optional): state2, step, beta1, beta2, weight_decay, max_gradient, momentum, eta, weight_decay_mode
+        -> tzk_fused_bwd_ex."""
         if _table_dtype(weights):
             ex = dict(ex, weights_f16=True)
         if lay.interleaved:
@@ -311,7 +324,7 @@ class CudaKernels:
                 _ptr(ws), ws.numel(), _stream()), "tzk_fused_bwd")
         # own launches next to CUB's radix sort: linearize, zero_counters, find_long_runs + the gradient half:
         # fused_apply (short runs and the long-run chunk CTAs in ONE launch), or tile_update + carry_combine
-        self.launches += 5 if _tile_path(lay) else 4
+        self.launches += 5 if _tile_path(lay, optimizer, ex) else 4
 
     def fused_bwd_workspace_bytes(self, lay: FeatureLayout, nnz: int) -> int:
         return int(self._lib.tzk_fused_bwd_workspace_bytes(nnz, lay.total_keys, lay.max_dim))
@@ -357,7 +370,7 @@ class CudaKernels:
                 _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(lay.d_key_base), _ptr(offsets), lay.num_features, B, nnz,
                 lay.total_keys, lay.max_dim, lay.vec_ok, _ptr(weights), _ptr(state), lr, eps, grad_scale,
                 _ptr(ws), ws.numel(), _stream()), "tzk_fused_bwd_apply")
-        self.launches += 2 if _tile_path(lay) else 1
+        self.launches += 2 if _tile_path(lay, optimizer, ex) else 1
 
     # ------------------------------------------------------------------ K1 / K2
     def bucketize_rw(self, ids: torch.Tensor, offsets: torch.Tensor, F: int, B: int, W: int,
@@ -620,7 +633,7 @@ class CudaKernels:
             _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(lay.d_key_base), lay.num_features, B, me, W, cap, idx_span,
             lay.total_keys, lay.max_dim, lay.vec_ok, _ptr(weights), grad_scale, _ptr(ws), ws.numel(), _stream()),
             "tzk_fused_bwd_apply_peer")
-        self.launches += 2 if _tile_path(lay) else 1
+        self.launches += 2 if _tile_path(lay, optimizer, ex) else 1
 
     # ------------------------------------------------------------------ K6
     def col_gather_sum(self, srcs: Sequence[torch.Tensor], plan: "ColPlan", rows: int,

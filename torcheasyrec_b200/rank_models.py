@@ -21,7 +21,8 @@ from .config import Message, config_to_kwargs
 from .embedding_group import EmbeddingGroup
 from .embedding_modules import SparseOptimizerSpec
 from .features import BaseFeature
-from .kernels import OPT_ADAGRAD, OPT_ADAM, OPT_PARTIAL_ROWWISE_ADAM, OPT_ROWWISE_ADAGRAD, OPT_SGD
+from .kernels import (OPT_ADAGRAD, OPT_ADAM, OPT_LAMB, OPT_LARS_SGD, OPT_PARTIAL_ROWWISE_ADAM, OPT_PARTIAL_ROWWISE_LAMB,
+                      OPT_ROWWISE_ADAGRAD, OPT_SGD, WD_DECOUPLE, WD_L2, WD_NONE)
 
 
 # --------------------------------------------------------------------------------------------------------
@@ -564,14 +565,24 @@ def sparse_optimizer_from_config(train_config: Message) -> SparseOptimizerSpec:
         return SparseOptimizerSpec(kind=OPT_ADAGRAD, lr=cfg.lr, initial_accumulator_value=cfg.initial_accumulator_value,
                                    **clip)
     if kind == "rowwise_adagrad_optimizer":
-        if cfg.weight_decay:
-            raise NotImplementedError("rowwise_adagrad weight_decay modes are not implemented")
-        return SparseOptimizerSpec(kind=OPT_ROWWISE_ADAGRAD, lr=cfg.lr, **clip)
-    if kind in ("adam_optimizer", "partial_rowwise_adam_optimizer"):
-        return SparseOptimizerSpec(kind=OPT_ADAM if kind == "adam_optimizer" else OPT_PARTIAL_ROWWISE_ADAM, lr=cfg.lr,
-                                   beta1=cfg.beta1, beta2=cfg.beta2, weight_decay=cfg.weight_decay, **clip)
-    raise NotImplementedError(f"sparse optimizer {kind} is not implemented (sgd / adagrad / rowwise_adagrad / adam / "
-                              "partial_rowwise_adam are; lars_sgd, lamb, partial_rowwise_lamb, adadelta, rmsprop are not)")
+        modes = {"NONE": WD_NONE, "L2": WD_L2, "DECOUPLE": WD_DECOUPLE}
+        mode = cfg.weight_decay_mode
+        mode = modes[mode] if isinstance(mode, str) else int(mode)      # (an enum is its name, or its number)
+        return SparseOptimizerSpec(kind=OPT_ROWWISE_ADAGRAD, lr=cfg.lr, weight_decay=cfg.weight_decay,
+                                   weight_decay_mode=mode, **clip)
+    adam_like = {"adam_optimizer": OPT_ADAM, "partial_rowwise_adam_optimizer": OPT_PARTIAL_ROWWISE_ADAM,
+                 "lamb_optimizer": OPT_LAMB, "partial_rowwise_lamb_optimizer": OPT_PARTIAL_ROWWISE_LAMB}
+    if kind in adam_like:
+        return SparseOptimizerSpec(kind=adam_like[kind], lr=cfg.lr, beta1=cfg.beta1, beta2=cfg.beta2,
+                                   weight_decay=cfg.weight_decay, **clip)
+    if kind == "lars_sgd_optimizer":        # eta: fbgemm's default (the proto has no field for it)
+        return SparseOptimizerSpec(kind=OPT_LARS_SGD, lr=cfg.lr, momentum=cfg.momentum, weight_decay=cfg.weight_decay,
+                                   **clip)
+    if kind in ("adadelta_optimizer", "rmsprop_optimizer"):
+        # the reference raises the same way: the public torchrec / fbgemm-gpu releases have no such fused kernel
+        raise RuntimeError(f"sparse {kind} is not available in the public torchrec / fbgemm-gpu releases (the "
+                           "reference needs an unreleased fbgemm-gpu wheel for it), and is not implemented here")
+    raise NotImplementedError(f"sparse optimizer {kind} is not implemented")
 
 
 def dense_optimizer_from_config(train_config: Message, params, **kw) -> torch.optim.Optimizer:
