@@ -83,6 +83,11 @@ typedef struct tzk_opt_args {
   int32_t weight_decay_mode; /* ROWWISE_ADAGRAD (tzrec WeightDecayMode): 0 NONE (weight_decay ignored); 1 L2:
                         * s_row += mean_d((g + wd*w)^2), w = (1 - mult*wd)*w - mult*g; 2 DECOUPLE: s_row += mean_d(g*g),
                         * w = (1 - lr*wd)*w - mult*g; mult = lr/(sqrt(s_row)+eps) */
+  const float* per_sample_weights; /* NULL: unweighted bags.  Else weighted bags (pooled layout, [EXT] the weighted TBE
+                        * backward, split_embedding_backward_codegen_*_weighted_exact): position l contributes
+                        * grad_scale * w[l] * grad_out row (/ L for MEAN).  tzk_fused_bwd_ex reads w[nnz] here and needs
+                        * tzk_fused_bwd_weighted_workspace_bytes; tzk_fused_bwd_apply_ex only checks it is non-NULL and
+                        * consumes the workspace of tzk_fused_bwd_sort_weighted.  The peer entry points reject it. */
 } tzk_opt_args;
 
 typedef void* tzk_stream_t; /* cudaStream_t */
@@ -144,6 +149,19 @@ int tzk_seq_gather_fwd_f16(const void* weights, const int64_t* feat_w_off, const
                            const int64_t* offsets, int32_t F, int32_t B, int32_t D, int64_t nnz, float* out,
                            tzk_stream_t stream);
 
+/* ---- K4w: weighted pooled gather  ([EXT] fbgemm TBE split_embedding_codegen_forward_weighted; torchrec's sharded
+ * lookup passes `features.weights_or_none()` as per_sample_weights — IdFeature `weighted: true`,
+ * tzrec/features/id_feature.py, tzrec/datasets/utils.py:299-342) ------------------------------------------------------
+ * out[b, feat_col[f] : +D_f] = pool_{l in bag(f,b)} per_sample_weights[l] * row(ids[l]), accumulated in fp32 in list order
+ * as acc = fmaf(w[l], row, acc) (the first term w[l0] * row), MEAN multiplies by 1/L at the end; with all-ones weights the
+ * bits equal the unweighted lookup's.  One entry point for the three arena formats: weights_f16 != 0 -> halfs (like
+ * tzk_pooled_gather_fwd_f16), else fp32 with dense rows (feat_stride NULL) or strided rows (like _strided). */
+int tzk_pooled_gather_fwd_weighted(const void* weights, int32_t weights_f16, const int64_t* feat_w_off,
+                                   const int64_t* feat_rows, const int32_t* feat_dim, const int32_t* feat_stride,
+                                   const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
+                                   const int64_t* offsets, const float* per_sample_weights, int32_t F, int32_t B,
+                                   int32_t max_dim, int32_t vec_ok, float* out, int64_t ld_out, tzk_stream_t stream);
+
 /* ---- K5: fused backward + sparse optimizer  ([EXT] TBE split_embedding_backward_codegen_*_exact,
  * installed by apply_optimizer_in_backward at tzrec/main.py:774-781; optimizer choice
  * tzrec/optim/optimizer_builder.py:30-97) -------------------------------------------------------------
@@ -189,6 +207,16 @@ int tzk_fused_bwd_apply(int32_t optimizer, int32_t pooled, const float* grad_out
                         int32_t max_dim, int32_t vec_ok, float* weights, float* state, float lr, float eps,
                         float grad_scale, void* workspace, size_t workspace_bytes, tzk_stream_t stream);
 
+/* Weighted bags ([EXT] the weighted TBE backward, split_embedding_backward_codegen_*_weighted_exact, without the
+ * gradient w.r.t. the weights): tzk_opt_args.per_sample_weights non-NULL, pooled layout only.  The workspace must have
+ * tzk_fused_bwd_weighted_workspace_bytes.  tzk_fused_bwd_sort_weighted is the id half (it also leaves the weights in
+ * sorted order in the workspace); tzk_fused_bwd_apply_ex with a non-NULL per_sample_weights is its gradient half. */
+size_t tzk_fused_bwd_weighted_workspace_bytes(int64_t nnz, int64_t total_keys, int32_t max_dim);
+int tzk_fused_bwd_sort_weighted(int32_t pooled, const int64_t* feat_rows, const int64_t* feat_key_base, const int64_t* ids,
+                                const int64_t* offsets, const float* per_sample_weights, int32_t F, int32_t B,
+                                int64_t nnz, int64_t total_keys, int32_t max_dim, void* workspace,
+                                size_t workspace_bytes, tzk_stream_t stream);
+
 /* ---- pooled-lookup backward w.r.t. a row buffer in which every row is referenced exactly once (the
  * sample owner's half of the sharded backward; our replacement of [EXT] PooledEmbeddingsAllToAll /
  * PooledEmbeddingsReduceScatter backward, App. A.6 / A.8):
@@ -230,6 +258,9 @@ int tzk_permute_lengths(const int32_t* lengths, const int32_t* perm, int32_t S_o
 int tzk_permute_ids(const int64_t* ids, const int64_t* in_offsets, const int64_t* out_offsets,
                     const int32_t* perm, int32_t S_out, int32_t B, int64_t* out_ids,
                     tzk_stream_t stream);
+/* the `weights` half of permute_2D_sparse_data: the per-sample weights of a weighted KJT, moved like its ids */
+int tzk_permute_weights(const float* weights, const int64_t* in_offsets, const int64_t* out_offsets,
+                        const int32_t* perm, int32_t S_out, int32_t B, float* out_weights, tzk_stream_t stream);
 
 /* ---- K6: regroup  ([EXT] fbgemm::permute_pooled_embs / KeyedTensor.regroup_as_dict, called at
  * tzrec/modules/embedding.py:972-976; App. A.13) ------------------------------------------------------

@@ -19,7 +19,7 @@ class TzkOptArgs(ctypes.Structure):
     _fields_ = [("optimizer", c_int32), ("lr", c_float), ("eps", c_float), ("beta1", c_float), ("beta2", c_float),
                 ("weight_decay", c_float), ("max_gradient", c_float), ("state", c_void_p), ("state2", c_void_p),
                 ("step", c_void_p), ("weights_f16", c_int32), ("interleaved", c_int32), ("momentum", c_float),
-                ("eta", c_float), ("weight_decay_mode", c_int32)]
+                ("eta", c_float), ("weight_decay_mode", c_int32), ("per_sample_weights", c_void_p)]
 
 
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
@@ -44,7 +44,14 @@ SIGNATURES = {
         [P, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, P, c_int64, P],
     ),
     "tzk_seq_gather_fwd_strided": (c_int32, [P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, c_int64, P, P]),
+    "tzk_pooled_gather_fwd_weighted": (
+        c_int32,
+        [P, c_int32, P, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, P, c_int64, P],
+    ),
     "tzk_fused_bwd_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32]),
+    "tzk_fused_bwd_weighted_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int32]),
+    "tzk_fused_bwd_sort_weighted": (
+        c_int32, [c_int32, P, P, P, P, P, c_int32, c_int32, c_int64, c_int64, c_int32, P, c_size_t, P]),
     "tzk_fused_bwd": (
         c_int32,
         [c_int32, c_int32, P, c_int64, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int64, c_int64, c_int32,
@@ -74,6 +81,7 @@ SIGNATURES = {
     "tzk_bag_grad_expand": (c_int32, [P, c_int64, P, P, P, P, c_int32, c_int32, c_int32, P, P]),
     "tzk_permute_lengths": (c_int32, [P, P, c_int32, c_int32, P, P]),
     "tzk_permute_ids": (c_int32, [P, P, P, P, c_int32, c_int32, P, P]),
+    "tzk_permute_weights": (c_int32, [P, P, P, P, c_int32, c_int32, P, P]),
     "tzk_col_gather_sum": (c_int32, [P, P, c_int32, P, P, P, c_int32, c_int64, P, c_int64, P]),
     "tzk_jagged_to_padded": (c_int32, [P, P, c_int32, c_int32, c_int32, P, P]),
     "tzk_padded_to_jagged": (c_int32, [P, P, c_int32, c_int32, c_int32, c_int64, P, P]),

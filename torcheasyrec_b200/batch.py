@@ -91,7 +91,8 @@ def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Se
     batch = Batch()
     seq_lengths: Dict[str, np.ndarray] = {}
     for dg, feats in by_group.items():
-        keys, vals, lens = [], [], []
+        keys, vals, lens, wts = [], [], [], []
+        weighted = any(f.is_sparse and f.is_weighted for f in feats)
         dense_keys, dense_dims, dense_vals = [], [], []
         for f in feats:
             if f.is_sparse:
@@ -112,6 +113,9 @@ def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Se
                 keys.append(f.name)
                 lens.append(L.astype(np.int32))
                 vals.append(_draw_ids(rng, f.num_embeddings, int(L.sum()), id_dist))
+                if weighted:      # as DataParser: weighted keys carry their weights, the others of the group 1.0
+                    n = int(L.sum())
+                    wts.append(rng.random(n, dtype=np.float32) if f.is_weighted else np.ones(n, dtype=np.float32))
             elif f.is_sequence:
                 raise NotImplementedError("dense sequence features are not generated")
             else:
@@ -120,7 +124,8 @@ def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Se
                 dense_vals.append(rng.random((B, f.value_dim), dtype=np.float32))
         if keys:
             batch.sparse_features[dg] = KeyedJaggedTensor(
-                keys, torch.from_numpy(np.concatenate(vals)), lengths=torch.from_numpy(np.concatenate(lens)), stride=B)
+                keys, torch.from_numpy(np.concatenate(vals)), lengths=torch.from_numpy(np.concatenate(lens)),
+                weights=torch.from_numpy(np.concatenate(wts)) if weighted else None, stride=B)
         if dense_keys:
             batch.dense_features[dg] = KeyedTensor(dense_keys, dense_dims, torch.from_numpy(np.concatenate(dense_vals, axis=1)))
     for name in labels:

@@ -181,6 +181,44 @@ linearize_seq_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict_
   }
 }
 
+// ---- 1w. weighted bags (per-sample weights): the sort value is the id position l, so that the weight of every sorted
+// entry can be found; bag_of[l] keeps the bag.  After the sort, sorted_bag_weight_kernel turns each sorted value back into
+// its bag and writes w[l] next to it (sw[i]) — both still in the id half, so the gradient half reads the weight of
+// sorted position i as one more coalesced 4-B load instead of a dependent random one.  The sort is stable and l grows
+// with the bag, so a run's entries keep the ascending-bag order of the unweighted sort.
+template <typename KeyT>
+__global__ void __launch_bounds__(kThreads)
+linearize_weighted_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets,
+                          const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_key_base, int F,
+                          int B, KeyT sentinel, KeyT* __restrict__ keys, int32_t* __restrict__ vals,
+                          int32_t* __restrict__ bag_of) {
+  const int64_t n_bags = (int64_t)F * B;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t bag = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; bag < n_bags; bag += stride) {
+    const int f = (int)(bag / B);
+    const int64_t s = __ldg(offsets + bag), e = __ldg(offsets + bag + 1);
+    const int64_t base = __ldg(feat_key_base + f), rows = __ldg(feat_rows + f);
+    for (int64_t l = s; l < e; ++l) {
+      int64_t id = __ldg(ids + l);
+      if ((uint64_t)id >= (uint64_t)rows) id = 0;
+      keys[l] = rows > 0 ? (KeyT)(base + id) : sentinel;
+      vals[l] = (int32_t)l;
+      bag_of[l] = (int32_t)bag;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+sorted_bag_weight_kernel(int32_t* __restrict__ vals, const int32_t* __restrict__ bag_of, const float* __restrict__ psw,
+                         int64_t n, float* __restrict__ sw) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int32_t l = vals[i];
+    vals[i] = __ldg(bag_of + l);
+    sw[i] = __ldg(psw + l);
+  }
+}
+
 // ---- 1'. peer mode: the owner reads its chunk of every source rank's wire buffers (tzk_peer.cu: destination-major,
 // fixed capacity, counts per destination) straight into the sort's input.  Slot s = (src r, j): valid while j is below
 // the count r published for this rank; the rest are padding (sentinel key: sorted last, never updated).
@@ -797,10 +835,12 @@ find_long_runs_kernel(const KeyT* __restrict__ keys, int64_t n, KeyT sentinel, W
 // is consumed, so a group keeps 3*kPos independent 64-B requests in flight instead of one dependent chain.
 // One short run (<= kShortRun sorted positions starting at p, key k0, first value v0): sum its gradient rows in sorted
 // order, ONE optimizer update.  All G lanes of the group call it together.
-template <typename KeyT, int G, int VEC, int CH, int FAM>
+// WTD: weighted bags — sw[i] is the per-sample weight of sorted position i (sorted_bag_weight_kernel); it multiplies
+// the entry's scale.
+template <typename KeyT, int G, int VEC, int CH, int FAM, bool WTD = false>
 __device__ __forceinline__ void short_run(const BwdArgs& a, const PeerGrads& gp, const BwdFeat* fd,
                                           const int32_t* __restrict__ vals, int64_t p, KeyT k0, int32_t v0, int len,
-                                          int lane) {
+                                          int lane, const float* __restrict__ sw = nullptr) {
         int f00;
     if (a.pooled) f00 = bag_feat(a, v0); else f00 = feat_of_key<KeyT>(fd, a.F, k0);
     const BwdFeat d = fd[f00];
@@ -830,6 +870,7 @@ __device__ __forceinline__ void short_run(const BwdArgs& a, const PeerGrads& gp,
         const int j = j0 + q;
         ok[q] = j < len;
         en[q] = entry_of(a, gp, fd, (j == 0 || !ok[q]) ? v0 : vals[p + j], f00);
+        if (WTD && ok[q]) en[q].scale *= __ldg(sw + p + j);
       }
 #pragma unroll
       for (int ch = 0; ch < CH; ++ch) {
@@ -859,11 +900,11 @@ __device__ __forceinline__ void short_run(const BwdArgs& a, const PeerGrads& gp,
                                 (pre && elem_state<FAM>(a)) ? &pre_s : nullptr);
 }
 
-template <typename KeyT, int G, int VEC, int CH, int FAM>
+template <typename KeyT, int G, int VEC, int CH, int FAM, bool WTD = false>
 __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrads& gp, const BwdFeat* fd,
                                                 const KeyT* __restrict__ keys,
                                                 const int32_t* __restrict__ vals, const WorkLists& wl, int cta,
-                                                int n_ctas) {
+                                                int n_ctas, const float* __restrict__ sw = nullptr) {
   constexpr int NG = kThreads / G;
   const int lane = threadIdx.x % G;
   const int64_t stride = (int64_t)n_ctas * NG;
@@ -879,7 +920,7 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
       const int64_t p = hp;
       const int len = hl;
       if (h + stride < n_heads) { hp = wl.head_pos[h + stride]; hl = wl.head_len[h + stride]; }   // next head, early
-      short_run<KeyT, G, VEC, CH, FAM>(a, gp, fd, vals, p, keys[p], vals[p], len, lane);
+      short_run<KeyT, G, VEC, CH, FAM, WTD>(a, gp, fd, vals, p, keys[p], vals[p], len, lane, sw);
     }
     return;
   }
@@ -914,7 +955,7 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
       while (len <= kShortRun && p0 + len < a.n && keys[p0 + len] == key_c) ++len;
     }
     if (len > kShortRun) continue;
-    short_run<KeyT, G, VEC, CH, FAM>(a, gp, fd, vals, p0, key_c, v_c, len, lane);
+    short_run<KeyT, G, VEC, CH, FAM, WTD>(a, gp, fd, vals, p0, key_c, v_c, len, lane, sw);
   }
 }
 
@@ -925,11 +966,11 @@ __device__ __forceinline__ void run_update_body(const BwdArgs& a, const PeerGrad
 // the update — the order of the additions is fixed by the sorted positions, whoever happens to execute them.
 // These CTAs ride in the same launch as the short-run CTAs (fused_apply_kernel): tiny tables / hot ids and the big
 // tables' rows are updated side by side instead of in three dependent launches.
-template <typename KeyT, int G, int VEC, int CH, int FAM>
+template <typename KeyT, int G, int VEC, int CH, int FAM, bool WTD = false>
 __device__ __forceinline__ void long_chunk_body(const BwdArgs& a, const PeerGrads& gp, const BwdFeat* fd,
                                                 const KeyT* __restrict__ keys,
                                                 const int32_t* __restrict__ vals, const WorkLists& wl, int cta,
-                                                int n_ctas) {
+                                                int n_ctas, const float* __restrict__ sw = nullptr) {
   constexpr int GW = 32 / G;          // lane groups per warp
   constexpr int ROWF = CH * G * VEC;  // floats per partial row
   constexpr int kLU = 4;              // independent gradient rows in flight per lane group
@@ -961,6 +1002,7 @@ __device__ __forceinline__ void long_chunk_body(const BwdArgs& a, const PeerGrad
         const int q = q0 + u * GW;
         ok[u] = q < it.end;
         en[u] = entry_of(a, gp, fd, ok[u] ? vals[q] : v0, f0);
+        if (WTD && ok[u]) en[u].scale *= __ldg(sw + q);
       }
 #pragma unroll
       for (int ch = 0; ch < CH; ++ch) {
@@ -1037,6 +1079,24 @@ fused_apply_kernel(BwdArgs a, const int64_t* __restrict__ feat_w_off, const int6
   // index order — their work overlaps the whole short-run sweep instead of trailing it
   if ((int)blockIdx.x < n_long) long_chunk_body<KeyT, G, VEC, CH, FAM>(a, gp, fd, keys, vals, wl, blockIdx.x, n_long);
   else run_update_body<KeyT, G, VEC, CH, FAM>(a, gp, fd, keys, vals, wl, blockIdx.x - n_long, gridDim.x - n_long);
+}
+
+// the same launch for weighted bags: sw = the sorted per-sample weights the id half left in the workspace
+template <typename KeyT, int G, int VEC, int CH, int FAM>
+__global__ void __launch_bounds__(kThreads, CH == 1 ? 2 : 1)    // (2 CTAs / SM: at 64 and 80 registers the weighted runs spilled)
+fused_apply_weighted_kernel(BwdArgs a, const int64_t* __restrict__ feat_w_off, const int64_t* __restrict__ feat_rows,
+                            const int64_t* __restrict__ feat_key_base, const int32_t* __restrict__ feat_dim,
+                            const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                            const KeyT* __restrict__ keys, const int32_t* __restrict__ vals, WorkLists wl, int n_long,
+                            const __grid_constant__ PeerGrads gp, const float* __restrict__ sw) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  BwdFeat* fd = reinterpret_cast<BwdFeat*>(smem_raw);
+  stage_feats(fd, feat_w_off, feat_rows, feat_key_base, feat_dim, feat_col, feat_pool, a.F, a.interleaved);
+  init_bias_correction<FAM>(a);
+  if ((int)blockIdx.x < n_long)
+    long_chunk_body<KeyT, G, VEC, CH, FAM, true>(a, gp, fd, keys, vals, wl, blockIdx.x, n_long, sw);
+  else
+    run_update_body<KeyT, G, VEC, CH, FAM, true>(a, gp, fd, keys, vals, wl, blockIdx.x - n_long, gridDim.x - n_long, sw);
 }
 
 // ---- 3'. tile path: rows of <= 128 floats, 16-B aligned (vec4, one chunk per lane) -------------------------
@@ -1355,6 +1415,16 @@ WsLayout ws_layout(int64_t nnz, int64_t total_keys, int max_dim) {
 #define TZK_BWD_LAUNCH(KeyT, G_, VEC_, CH_, FAM_)                                                    \
   do {                                                                                                \
     size_t smem_s = (size_t)F * sizeof(BwdFeat);                                                      \
+    if (sw) {                                                                                         \
+      if (smem_s > 48 * 1024)                                                                         \
+        cudaFuncSetAttribute(fused_apply_weighted_kernel<KeyT, G_, VEC_, CH_, FAM_>,                  \
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s);               \
+      fused_apply_weighted_kernel<KeyT, G_, VEC_, CH_, FAM_><<<grid_s + n_long, kThreads, smem_s, st>>>( \
+          a, feat_w_off, feat_rows, feat_key_base, feat_dim, feat_col, feat_pool, (const KeyT*)keys_out, \
+          vals_out, wl, n_long, gp, sw);                                                              \
+      TZK_CHECK_LAUNCH("fused_apply_weighted_kernel");                                                \
+      break;                                                                                          \
+    }                                                                                                 \
     if (smem_s > 48 * 1024)                                                                           \
       cudaFuncSetAttribute(fused_apply_kernel<KeyT, G_, VEC_, CH_, FAM_>,                             \
                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_s);                 \
@@ -1401,6 +1471,21 @@ extern "C" size_t tzk_fused_bwd_workspace_bytes(int64_t nnz, int64_t total_keys,
   return ws_layout(nnz, total_keys, max_dim < 1 ? 1 : max_dim).total;
 }
 
+// weighted bags: the unweighted layout, then bag_of [n] int32 (id position -> bag) and sw [n] fp32 (sorted weights)
+struct WsWeighted { size_t bag_of, sw, total; };
+static WsWeighted ws_weighted(const WsLayout& L, int64_t nnz) {
+  const int64_t n = nnz < 1 ? 1 : nnz;
+  WsWeighted W;
+  W.bag_of = L.total;
+  W.sw = align_up(W.bag_of + (size_t)n * 4, 256);
+  W.total = align_up(W.sw + (size_t)n * 4, 256);
+  return W;
+}
+
+extern "C" size_t tzk_fused_bwd_weighted_workspace_bytes(int64_t nnz, int64_t total_keys, int32_t max_dim) {
+  return ws_weighted(ws_layout(nnz, total_keys, max_dim < 1 ? 1 : max_dim), nnz).total;
+}
+
 // phases: 1 = linearize + sort (needs ids / offsets only), 2 = reduce runs + update (needs the gradient)
 static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, const float* grad_out,
                           int64_t ld_grad, const int64_t* feat_w_off, const int64_t* feat_rows,
@@ -1410,6 +1495,9 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
                           int32_t vec_ok, float* weights, float grad_scale, void* workspace,
                           size_t workspace_bytes, tzk_stream_t stream, const PeerWire* pw = nullptr,
                           const uint64_t* grad_ptrs = nullptr, int32_t* overflow = nullptr) {
+  // weighted bags (opt.per_sample_weights != NULL, pooled local layouts only): phase 1 reads the weights and leaves them
+  // sorted in the workspace, phase 2 reads them from there
+  const float* psw = opt.per_sample_weights;
   // peer mode (pw != nullptr): nnz = W * cap wire slots; phase 1 pulls the keys from the sources' wire buffers instead
   // of linearising local ids; phase 2 reads every gradient slice from grad_ptrs[src] (tzk_peer.cu, DESIGN.md §6)
   const int32_t optimizer = opt.optimizer;
@@ -1439,10 +1527,14 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   TZK_REQUIRE(F <= 2048, "fused_bwd: F=%d > 2048 keys per collection", F);
   TZK_REQUIRE(max_dim >= 1 && max_dim <= 1024, "fused_bwd: max_dim=%d out of range [1,1024]", max_dim);
   WsLayout L = ws_layout(nnz, total_keys, max_dim);
-  TZK_REQUIRE(workspace && workspace_bytes >= L.total, "fused_bwd: workspace too small (%zu < %zu)",
-              workspace_bytes, L.total);
+  const WsWeighted LW = ws_weighted(L, nnz);
+  TZK_REQUIRE(!psw || (pooled && !pw), "fused_bwd: per-sample weights need the pooled local layout");
+  const size_t ws_need = psw ? LW.total : L.total;
+  TZK_REQUIRE(workspace && workspace_bytes >= ws_need, "fused_bwd: workspace too small (%zu < %zu)", workspace_bytes,
+              ws_need);
   cudaStream_t st = as_stream(stream);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
+  float* sw = psw ? reinterpret_cast<float*>(ws + LW.sw) : nullptr;
   void* keys_in = ws + L.keys_in;
   void* keys_out = ws + L.keys_out;
   int32_t* vals_in = reinterpret_cast<int32_t*>(ws + L.vals_in);
@@ -1495,8 +1587,12 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
     if (k64) cudaFuncSetAttribute(linearize_seq_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_lin);
     else cudaFuncSetAttribute(linearize_seq_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_lin);
   }
+  int32_t* bag_of = reinterpret_cast<int32_t*>(ws + LW.bag_of);
   if (k64) {
-    if (pooled)
+    if (psw)
+      linearize_weighted_kernel<uint64_t><<<grid_lin, kThreads, 0, st>>>(
+          ids, offsets, feat_rows, feat_key_base, F, B, (uint64_t)sentinel, (uint64_t*)keys_in, vals_in, bag_of);
+    else if (pooled)
       linearize_kernel<uint64_t><<<grid_lin, kThreads, 0, st>>>(ids, offsets, feat_rows, feat_key_base, F, B,
                                                                 pooled, (uint64_t)sentinel, (uint64_t*)keys_in, vals_in);
     else
@@ -1506,7 +1602,10 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
     ce = cub_sort<uint64_t>(ws + L.cub_tmp, cub_bytes, (const uint64_t*)keys_in, (uint64_t*)keys_out, vals_in,
                             vals_out, nnz, bits, st);
   } else {
-    if (pooled)
+    if (psw)
+      linearize_weighted_kernel<uint32_t><<<grid_lin, kThreads, 0, st>>>(
+          ids, offsets, feat_rows, feat_key_base, F, B, (uint32_t)sentinel, (uint32_t*)keys_in, vals_in, bag_of);
+    else if (pooled)
       linearize_kernel<uint32_t><<<grid_lin, kThreads, 0, st>>>(ids, offsets, feat_rows, feat_key_base, F, B,
                                                                 pooled, (uint32_t)sentinel, (uint32_t*)keys_in, vals_in);
     else
@@ -1517,6 +1616,11 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
                             vals_out, nnz, bits, st);
   }
   TZK_REQUIRE(ce == cudaSuccess, "fused_bwd: radix sort failed: %s", cudaGetErrorString(ce));
+  if (psw) {
+    const int grid_w = (int)std::min<int64_t>(ceil_div64(nnz, kThreads), kSmCountH100 * 8);
+    sorted_bag_weight_kernel<<<grid_w, kThreads, 0, st>>>(vals_out, bag_of, psw, nnz, sw);
+    TZK_CHECK_LAUNCH("sorted_bag_weight_kernel");
+  }
   }
   if (phases & 1) {   // work list of the long runs (tiny tables, hot ids) for the gradient half's chunk CTAs
     zero_counters<<<1, 1, 0, st>>>(wl.counters);
@@ -1570,7 +1674,7 @@ static int fused_bwd_impl(int phases, const tzk_opt_args& opt, int32_t pooled, c
   // they stay the default.  The kFamNorm optimizers always take the general path.
   const char* tile_env = getenv("TZK_BWD_TILE");
   const bool tile_path = tile_env && tile_env[0] == '1' && !a.w_f16 && !a.interleaved && optimizer != TZK_OPT_ACCUM_OUT &&
-                         fam == kFamClassic;   // (fp32 tables, real classic updates)
+                         fam == kFamClassic && !sw;   // (fp32 tables, real classic updates, unweighted bags)
   if (vec == 4 && ch == 1 && tile_path) {
     // tile path: every gradient / weight / state row of a tile is requested at once, runs are reduced in shared memory
     float* carry_first = reinterpret_cast<float*>(ws + L.carry);
@@ -1627,7 +1731,7 @@ static tzk_opt_args classic_opt(int32_t optimizer, float* state, float lr, float
   tzk_opt_args o;
   o.optimizer = optimizer; o.lr = lr; o.eps = eps; o.beta1 = 0.9f; o.beta2 = 0.999f; o.weight_decay = 0.f;
   o.max_gradient = 0.f; o.state = state; o.state2 = nullptr; o.step = nullptr; o.weights_f16 = 0; o.interleaved = 0;
-  o.momentum = 0.f; o.eta = 0.f; o.weight_decay_mode = 0;
+  o.momentum = 0.f; o.eta = 0.f; o.weight_decay_mode = 0; o.per_sample_weights = nullptr;
   return o;
 }
 
@@ -1665,6 +1769,20 @@ extern "C" int tzk_fused_bwd_sort(int32_t pooled, const int64_t* feat_rows, cons
   return fused_bwd_impl(1, classic_opt(TZK_OPT_SGD, nullptr, 0.f, 0.f), pooled, nullptr, 0, nullptr, feat_rows,
                         nullptr, nullptr, nullptr, feat_key_base, ids, offsets, F, B, nnz, total_keys, max_dim, 0,
                         nullptr, 0.f, workspace, workspace_bytes, stream);
+}
+
+// id half of a weighted update (workspace: tzk_fused_bwd_weighted_workspace_bytes); its gradient half is
+// tzk_fused_bwd_apply_ex with opt->per_sample_weights non-NULL
+extern "C" int tzk_fused_bwd_sort_weighted(int32_t pooled, const int64_t* feat_rows, const int64_t* feat_key_base,
+                                           const int64_t* ids, const int64_t* offsets, const float* per_sample_weights,
+                                           int32_t F, int32_t B, int64_t nnz, int64_t total_keys, int32_t max_dim,
+                                           void* workspace, size_t workspace_bytes, tzk_stream_t stream) {
+  TZK_REQUIRE(per_sample_weights != nullptr || F == 0 || B == 0 || nnz == 0,
+              "fused_bwd_sort_weighted: per_sample_weights is NULL");
+  tzk_opt_args o = classic_opt(TZK_OPT_SGD, nullptr, 0.f, 0.f);
+  o.per_sample_weights = per_sample_weights;
+  return fused_bwd_impl(1, o, pooled, nullptr, 0, nullptr, feat_rows, nullptr, nullptr, nullptr, feat_key_base, ids,
+                        offsets, F, B, nnz, total_keys, max_dim, 0, nullptr, 0.f, workspace, workspace_bytes, stream);
 }
 
 extern "C" int tzk_fused_bwd_apply(int32_t optimizer, int32_t pooled, const float* grad_out, int64_t ld_grad,
@@ -1775,6 +1893,7 @@ extern "C" int tzk_peer_small_update(const tzk_opt_args* opt, const uint64_t* ps
   TZK_REQUIRE(opt->optimizer >= 0 && opt->optimizer <= TZK_OPT_LARS_SGD && !opt->weights_f16,
               "peer_small_update: unsupported optimizer");
   TZK_REQUIRE(opt->optimizer == TZK_OPT_SGD || opt->state, "peer_small_update: optimizer state is NULL");
+  TZK_REQUIRE(opt->per_sample_weights == nullptr, "peer_small_update: weighted bags are not supported on the peer step");
   TZK_REQUIRE(!norm_family(*opt) || !opt->interleaved, "peer_small_update: interleaved rows are Adagrad only");
   TZK_REQUIRE((opt->optimizer != TZK_OPT_ADAM && opt->optimizer != TZK_OPT_PARTIAL_ROWWISE_ADAM &&
                opt->optimizer != TZK_OPT_LAMB && opt->optimizer != TZK_OPT_PARTIAL_ROWWISE_LAMB) ||
@@ -1859,6 +1978,7 @@ extern "C" int tzk_fused_bwd_apply_peer(const tzk_opt_args* opt, int32_t pooled,
                                         int32_t vec_ok, float* weights, float grad_scale, void* workspace,
                                         size_t workspace_bytes, tzk_stream_t stream) {
   TZK_REQUIRE(opt != nullptr && grad_ptrs != nullptr, "fused_bwd_apply_peer: NULL argument");
+  TZK_REQUIRE(opt->per_sample_weights == nullptr, "fused_bwd_apply_peer: weighted bags are not supported on the peer step");
   PeerWire pw;
   TZK_REQUIRE(fill_wire(&pw, nullptr, nullptr, nullptr, me, W, cap, idx_span) == 0,
               "fused_bwd_apply_peer: bad wire description");

@@ -115,6 +115,20 @@ permute_ids_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ 
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
     out_ids[dst0 + i] = ids[src0 + i];
 }
+
+// the per-sample weights of a weighted KJT travel with its ids: the same segment copy over 4-B floats
+__global__ void __launch_bounds__(kThreads)
+permute_weights_kernel(const float* __restrict__ w, const int64_t* __restrict__ in_offsets,
+                       const int64_t* __restrict__ out_offsets, const int32_t* __restrict__ perm, int B,
+                       float* __restrict__ out_w) {
+  const int s = blockIdx.y;
+  const int64_t src0 = __ldg(in_offsets + (int64_t)__ldg(perm + s) * B);
+  const int64_t dst0 = __ldg(out_offsets + (int64_t)s * B);
+  const int64_t n = __ldg(out_offsets + (int64_t)(s + 1) * B) - dst0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    out_w[dst0 + i] = w[src0 + i];
+}
 }  // namespace
 
 extern "C" size_t tzk_bucketize_rw_workspace_bytes(int32_t F, int32_t B, int32_t W, int64_t nnz) {
@@ -175,5 +189,20 @@ extern "C" int tzk_permute_ids(const int64_t* ids, const int64_t* in_offsets, co
   dim3 grid(gx, S_out);
   permute_ids_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(ids, in_offsets, out_offsets, perm, B, out_ids);
   TZK_CHECK_LAUNCH("permute_ids_kernel");
+  return 0;
+}
+
+extern "C" int tzk_permute_weights(const float* weights, const int64_t* in_offsets, const int64_t* out_offsets,
+                                   const int32_t* perm, int32_t S_out, int32_t B, float* out_weights,
+                                   tzk_stream_t stream) {
+  TZK_REQUIRE(S_out >= 0 && B >= 0, "permute_weights: negative size");
+  if (S_out == 0 || B == 0) return 0;
+  TZK_REQUIRE(S_out <= 65535, "permute_weights: S_out=%d > 65535", S_out);
+  TZK_REQUIRE(in_offsets && out_offsets && perm, "permute_weights: NULL argument");
+  int gx = (int)(ceil_div64(B, kThreads) < 64 ? ceil_div64(B, kThreads) : 64);
+  dim3 grid(gx, S_out);
+  permute_weights_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(weights, in_offsets, out_offsets, perm, B,
+                                                                    out_weights);
+  TZK_CHECK_LAUNCH("permute_weights_kernel");
   return 0;
 }

@@ -41,17 +41,22 @@ struct BagStage {
   int64_t id0;     // first id (valid when len > 0)
 };
 
-template <int G, int VEC, typename WT>
-__global__ void __launch_bounds__(kThreads)
-pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restrict__ feat_w_off,
-                         const int64_t* __restrict__ feat_rows, const int32_t* __restrict__ feat_dim,
-                         const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
-                         const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F, int B,
-                         float* __restrict__ out, int64_t ld_out, const int32_t* __restrict__ feat_stride) {
+// WTD: weighted bags (per-sample weights psw[l], fbgemm's ..._forward_weighted): out = sum_l psw[l] * row(ids[l]) in list
+// order as acc = fmaf(psw[l], row, acc), the first term as psw[l0] * row — with all-ones weights every operation is exact
+// and the result has the bits of the unweighted lookup
+template <int G, int VEC, typename WT, bool WTD>
+__device__ __forceinline__ void
+pooled_gather_body(const WT* __restrict__ weights, const int64_t* __restrict__ feat_w_off,
+                   const int64_t* __restrict__ feat_rows, const int32_t* __restrict__ feat_dim,
+                   const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                   const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F, int B,
+                   float* __restrict__ out, int64_t ld_out, const int32_t* __restrict__ feat_stride,
+                   const float* __restrict__ psw) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   FeatDesc* fd = reinterpret_cast<FeatDesc*>(smem_raw);
   BagStage* st = reinterpret_cast<BagStage*>(smem_raw + align16((size_t)F * sizeof(FeatDesc)));
   int32_t* st_len = reinterpret_cast<int32_t*>(st + kItemsPerCta);
+  float* st_w = reinterpret_cast<float*>(st_len + kItemsPerCta);   // WTD: weight of the bag's first id
   for (int f = threadIdx.x; f < F; f += kThreads) {
     fd[f].w_off = feat_w_off[f];
     fd[f].rows = feat_rows[f];
@@ -95,6 +100,11 @@ pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restri
       int64_t id0[PT];
 #pragma unroll
       for (int k = 0; k < PT; ++k) id0[k] = len[k] > 0 ? __ldg(ids + s[k]) : 0;
+      float w0[PT];
+      if constexpr (WTD) {
+#pragma unroll
+        for (int k = 0; k < PT; ++k) w0[k] = len[k] > 0 ? __ldg(psw + s[k]) : 0.f;
+      }
 #pragma unroll
       for (int k = 0; k < PT; ++k) {
         const int i = threadIdx.x + k * kThreads;
@@ -102,6 +112,7 @@ pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restri
           st[i].start = s[k];
           st[i].id0 = id0[k];
           st_len[i] = len[k];
+          if constexpr (WTD) st_w[i] = w0[k];
         }
       }
     }
@@ -140,10 +151,21 @@ pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restri
                 a = ld_table_f4<WT>(weights + d.w_off + id * d.stride + c);
               }
               const int64_t s0 = st[i].start;
-              for (int l = 1; l < L; ++l) {
-                int64_t idl = __ldg(ids + s0 + l);
-                if ((uint64_t)idl >= (uint64_t)d.rows) idl = 0;
-                a = f4_add(a, ld_table_f4<WT>(weights + d.w_off + idl * d.stride + c));
+              if constexpr (WTD) {
+                a = f4_scale(a, st_w[i]);
+                for (int l = 1; l < L; ++l) {
+                  int64_t idl = __ldg(ids + s0 + l);
+                  const float wl = __ldg(psw + s0 + l);
+                  if ((uint64_t)idl >= (uint64_t)d.rows) idl = 0;
+                  const float4 r = ld_table_f4<WT>(weights + d.w_off + idl * d.stride + c);
+                  a = make_float4(fmaf(wl, r.x, a.x), fmaf(wl, r.y, a.y), fmaf(wl, r.z, a.z), fmaf(wl, r.w, a.w));
+                }
+              } else {
+                for (int l = 1; l < L; ++l) {
+                  int64_t idl = __ldg(ids + s0 + l);
+                  if ((uint64_t)idl >= (uint64_t)d.rows) idl = 0;
+                  a = f4_add(a, ld_table_f4<WT>(weights + d.w_off + idl * d.stride + c));
+                }
               }
               if (d.pool == TZK_POOL_MEAN) a = f4_scale(a, 1.0f / (float)L);
             }
@@ -166,10 +188,20 @@ pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restri
               int64_t id = st[i].id0;
               if ((uint64_t)id >= (uint64_t)d.rows) id = 0;
               acc = ld_table_f1<WT>(weights + d.w_off + id * d.stride + c);
-              for (int l = 1; l < L; ++l) {
-                int64_t idl = __ldg(ids + s0 + l);
-                if ((uint64_t)idl >= (uint64_t)d.rows) idl = 0;
-                acc += ld_table_f1<WT>(weights + d.w_off + idl * d.stride + c);
+              if constexpr (WTD) {
+                acc = st_w[i] * acc;
+                for (int l = 1; l < L; ++l) {
+                  int64_t idl = __ldg(ids + s0 + l);
+                  const float wl = __ldg(psw + s0 + l);
+                  if ((uint64_t)idl >= (uint64_t)d.rows) idl = 0;
+                  acc = fmaf(wl, ld_table_f1<WT>(weights + d.w_off + idl * d.stride + c), acc);
+                }
+              } else {
+                for (int l = 1; l < L; ++l) {
+                  int64_t idl = __ldg(ids + s0 + l);
+                  if ((uint64_t)idl >= (uint64_t)d.rows) idl = 0;
+                  acc += ld_table_f1<WT>(weights + d.w_off + idl * d.stride + c);
+                }
               }
               if (d.pool == TZK_POOL_MEAN) acc = acc * (1.0f / (float)L);
             }
@@ -180,6 +212,29 @@ pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restri
     }
     __syncthreads();  // the stage buffer is reused by the next (tile, chunk)
   }
+}
+
+template <int G, int VEC, typename WT>
+__global__ void __launch_bounds__(kThreads)
+pooled_gather_fwd_kernel(const WT* __restrict__ weights, const int64_t* __restrict__ feat_w_off,
+                         const int64_t* __restrict__ feat_rows, const int32_t* __restrict__ feat_dim,
+                         const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                         const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F, int B,
+                         float* __restrict__ out, int64_t ld_out, const int32_t* __restrict__ feat_stride) {
+  pooled_gather_body<G, VEC, WT, false>(weights, feat_w_off, feat_rows, feat_dim, feat_col, feat_pool, ids, offsets, F,
+                                        B, out, ld_out, feat_stride, nullptr);
+}
+
+template <int G, int VEC, typename WT>
+__global__ void __launch_bounds__(kThreads, 2)     // (up to 128 registers: the default allocation spilled)
+pooled_gather_fwd_weighted_kernel(const WT* __restrict__ weights, const int64_t* __restrict__ feat_w_off,
+                                  const int64_t* __restrict__ feat_rows, const int32_t* __restrict__ feat_dim,
+                                  const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                                  const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F, int B,
+                                  float* __restrict__ out, int64_t ld_out, const int32_t* __restrict__ feat_stride,
+                                  const float* __restrict__ psw) {
+  pooled_gather_body<G, VEC, WT, true>(weights, feat_w_off, feat_rows, feat_dim, feat_col, feat_pool, ids, offsets, F,
+                                       B, out, ld_out, feat_stride, psw);
 }
 
 // one lane group per id position; f found by binary search over the key boundaries offsets[f*B]
@@ -238,12 +293,25 @@ inline int pick_lanes(int max_dim, int vec) {
     default: KERNEL<32, VEC_, WT_><<<grid, kThreads, smem, st>>>(__VA_ARGS__); break;             \
   }
 
+template <int VEC, typename WT>
+static void pooled_gather_weighted_allow_smem_v(int G, size_t smem) {
+  auto k = G == 1 ? pooled_gather_fwd_weighted_kernel<1, VEC, WT> : G == 2 ? pooled_gather_fwd_weighted_kernel<2, VEC, WT>
+         : G == 4 ? pooled_gather_fwd_weighted_kernel<4, VEC, WT> : G == 8 ? pooled_gather_fwd_weighted_kernel<8, VEC, WT>
+         : G == 16 ? pooled_gather_fwd_weighted_kernel<16, VEC, WT> : pooled_gather_fwd_weighted_kernel<32, VEC, WT>;
+  cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+template <typename WT>
+static void pooled_gather_weighted_allow_smem(int G, int vec, size_t smem) {
+  if (vec == 4) pooled_gather_weighted_allow_smem_v<4, WT>(G, smem);
+  else pooled_gather_weighted_allow_smem_v<1, WT>(G, smem);
+}
+
 template <typename WT>
 static int pooled_gather_fwd_impl(const WT* weights, const int64_t* feat_w_off, const int64_t* feat_rows,
                                   const int32_t* feat_dim, const int32_t* feat_col, const int32_t* feat_pool,
                                   const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t max_dim,
                                   int32_t vec_ok, float* out, int64_t ld_out, tzk_stream_t stream,
-                                  const int32_t* feat_stride = nullptr) {
+                                  const int32_t* feat_stride = nullptr, const float* psw = nullptr) {
   TZK_REQUIRE(F >= 0 && B >= 0, "pooled_gather_fwd: negative F/B");
   if (F == 0 || B == 0) return 0;
   TZK_REQUIRE(weights && feat_w_off && feat_rows && feat_dim && feat_col && feat_pool && offsets && out,
@@ -258,8 +326,20 @@ static int pooled_gather_fwd_impl(const WT* weights, const int64_t* feat_w_off, 
   const int n_work = n_tiles * ((F + kItemsPerCta / kTB - 1) / (kItemsPerCta / kTB));
   int grid = n_work < kSmCountH100 * 8 ? n_work : kSmCountH100 * 8;
   size_t smem = align16((size_t)F * sizeof(FeatDesc)) + (size_t)kItemsPerCta * (sizeof(BagStage) + sizeof(int32_t));
-  TZK_REQUIRE(smem <= 48 * 1024, "pooled_gather_fwd: F=%d keys need %zu B of shared memory (> 48 KB)", F, smem);
-  if (vec == 4) {
+  if (psw) {      // + the first weight of every staged bag; above 48 KB the weighted kernel opts in
+    smem += (size_t)kItemsPerCta * sizeof(float);
+    if (smem > 48 * 1024) pooled_gather_weighted_allow_smem<WT>(G, vec, smem);
+  }
+  TZK_REQUIRE(psw || smem <= 48 * 1024, "pooled_gather_fwd: F=%d keys need %zu B of shared memory (> 48 KB)", F, smem);
+  if (psw) {
+    if (vec == 4) {
+      TZK_DISPATCH_G(G, 4, WT, pooled_gather_fwd_weighted_kernel, weights, feat_w_off, feat_rows, feat_dim, feat_col,
+                     feat_pool, ids, offsets, F, B, out, ld_out, feat_stride, psw)
+    } else {
+      TZK_DISPATCH_G(G, 1, WT, pooled_gather_fwd_weighted_kernel, weights, feat_w_off, feat_rows, feat_dim, feat_col,
+                     feat_pool, ids, offsets, F, B, out, ld_out, feat_stride, psw)
+    }
+  } else if (vec == 4) {
     TZK_DISPATCH_G(G, 4, WT, pooled_gather_fwd_kernel, weights, feat_w_off, feat_rows, feat_dim, feat_col,
                    feat_pool, ids, offsets, F, B, out, ld_out, feat_stride)
   } else {
@@ -355,4 +435,25 @@ extern "C" int tzk_seq_gather_fwd_strided(const float* weights, const int64_t* f
                                           const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t D,
                                           int32_t row_stride, int64_t nnz, float* out, tzk_stream_t stream) {
   return seq_gather_fwd_impl<float>(weights, feat_w_off, feat_rows, ids, offsets, F, B, D, nnz, out, stream, row_stride);
+}
+
+// Weighted bags ([EXT] fbgemm TBE split_embedding_codegen_forward_weighted, per_sample_weights of the sharded lookup): one
+// entry point for the three arena formats — weights_f16 selects halfs, feat_stride (nullable) strided fp32 rows.
+extern "C" int tzk_pooled_gather_fwd_weighted(const void* weights, int32_t weights_f16, const int64_t* feat_w_off,
+                                              const int64_t* feat_rows, const int32_t* feat_dim,
+                                              const int32_t* feat_stride, const int32_t* feat_col,
+                                              const int32_t* feat_pool, const int64_t* ids, const int64_t* offsets,
+                                              const float* per_sample_weights, int32_t F, int32_t B, int32_t max_dim,
+                                              int32_t vec_ok, float* out, int64_t ld_out, tzk_stream_t stream) {
+  TZK_REQUIRE(F == 0 || B == 0 || per_sample_weights != nullptr,
+              "pooled_gather_fwd_weighted: per_sample_weights is NULL");
+  if (weights_f16) {
+    TZK_REQUIRE(feat_stride == nullptr, "pooled_gather_fwd_weighted: strided (interleaved) tables are fp32");
+    return pooled_gather_fwd_impl<__half>(static_cast<const __half*>(weights), feat_w_off, feat_rows, feat_dim, feat_col,
+                                          feat_pool, ids, offsets, F, B, max_dim, vec_ok, out, ld_out, stream, nullptr,
+                                          per_sample_weights);
+  }
+  return pooled_gather_fwd_impl<float>(static_cast<const float*>(weights), feat_w_off, feat_rows, feat_dim, feat_col,
+                                       feat_pool, ids, offsets, F, B, max_dim, vec_ok, out, ld_out, stream, feat_stride,
+                                       per_sample_weights);
 }

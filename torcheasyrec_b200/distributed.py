@@ -459,6 +459,14 @@ class _ShardedBase(nn.Module):
         raise KeyError(name)
 
 
+def reject_weighted(features: KeyedJaggedTensor) -> None:
+    """Sharded pooled lookups do not carry per-sample weights yet (the bucketize / push kernels would have to move them
+    with the ids): a weighted KJT raises instead of being pooled as a plain sum.  Host-side, no device sync."""
+    if features.weights_or_none() is not None:
+        raise NotImplementedError("weighted id features (per-sample weights) on a sharded EmbeddingBagCollection are not "
+                                  "supported yet; use an unsharded collection")
+
+
 class ShardedEmbeddingBagCollection(_ShardedBase):
     """forward(KJT of the local batch) -> KeyedTensor [B, sum D], same values as the unsharded collection."""
 
@@ -466,6 +474,7 @@ class ShardedEmbeddingBagCollection(_ShardedBase):
         return self._configs
 
     def forward(self, features: KeyedJaggedTensor) -> KeyedTensor:
+        reject_weighted(features)
         if self._maybe_enable_peer(features):
             return self.forward(features)
         keys, lens, vals = [], [], []

@@ -385,9 +385,10 @@ class _ArenaCollection(nn.Module):
     def feature_names(self) -> List[str]:
         return self._feature_names
 
-    def _bwd_workspace(self, k, nnz: int) -> torch.Tensor:
+    def _bwd_workspace(self, k, nnz: int, weighted: bool = False) -> torch.Tensor:
         """Private fused-backward workspace (the sorted keys live here between forward and backward)."""
-        need = k.fused_bwd_workspace_bytes(self.layout, nnz)
+        need = k.fused_bwd_workspace_bytes(self.layout, nnz, weighted=True) if weighted else \
+            k.fused_bwd_workspace_bytes(self.layout, nnz)
         ws = getattr(self, "_bwd_ws", None)
         if ws is None or ws.numel() < need or ws.device != self.weights.device:
             ws = torch.empty(max(need, 256), dtype=torch.uint8, device=self.weights.device)
@@ -424,7 +425,7 @@ class _ArenaCollection(nn.Module):
         return kjt.permute([pos[f] for f in self._feature_names])
 
 
-def _early_sort(ctx, mod, pooled: bool, ids, offsets, B, want_grad: bool) -> None:
+def _early_sort(ctx, mod, pooled: bool, ids, offsets, B, want_grad: bool, psw=None) -> None:
     """Enqueue the id-only half of the fused backward (linearize + radix sort) on the module's side stream right
     away: it overlaps the rest of the forward pass and the dense backward instead of sitting on the critical path
     (the role TrainPipelineSparseDist's data-dist stream plays in the reference, tzrec/utils/dist_util.py:221-303).
@@ -444,17 +445,20 @@ def _early_sort(ctx, mod, pooled: bool, ids, offsets, B, want_grad: bool) -> Non
             and hasattr(k, "fused_bwd_sort") and mod.optimizer is not None
             and not getattr(mod, "_early_busy", False)      # one outstanding lookup per module owns the workspace
             and os.environ.get("TZK_EARLY_SORT", "1") != "0"):
-        ws = mod._bwd_workspace(k, ids.numel())
+        ws = mod._bwd_workspace(k, ids.numel(), weighted=psw is not None)
         side = mod._side_stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
-            k.fused_bwd_sort(pooled, mod.layout, ids, offsets, B, ws)
+            if psw is None:
+                k.fused_bwd_sort(pooled, mod.layout, ids, offsets, B, ws)
+            else:
+                k.fused_bwd_sort(pooled, mod.layout, ids, offsets, B, ws, per_sample_weights=psw)
         ctx.early = (ws, side)
         mod._early_busy = True
         mod._early_owner = weakref.ref(ctx)
 
 
-def _fused_backward(ctx, mod, pooled: bool, grad, ids, offsets, who: str) -> None:
+def _fused_backward(ctx, mod, pooled: bool, grad, ids, offsets, who: str, psw=None) -> None:
     spec = mod.optimizer
     if spec is None:
         raise RuntimeError(f"{who}.backward: no sparse optimizer set (call set_optimizer); tables are updated "
@@ -467,6 +471,8 @@ def _fused_backward(ctx, mod, pooled: bool, grad, ids, offsets, who: str) -> Non
         mod._early_busy = False
         cur = torch.cuda.current_stream()
         extras = mod.opt_extras()          # (advances the device step counter on `cur`)
+        if psw is not None:
+            extras["per_sample_weights"] = psw
         if os.environ.get("TZK_ASYNC_APPLY", "1") != "0":
             # The gradient half stays on the side stream (it is already ordered after the sort there) and the rest of
             # the backward pass — whatever autograd schedules after this node, e.g. the bottom MLP of DLRM — runs
@@ -478,7 +484,7 @@ def _fused_backward(ctx, mod, pooled: bool, grad, ids, offsets, who: str) -> Non
                                   ids.numel(), ctx.B, spec.lr, spec.eps, mod.grad_scale, ws, **extras)
             # keeps the buffers the side-stream kernel reads away from the allocator until the join (autograd drops
             # the saved tensors as soon as this node returns)
-            mod._pending_apply = (grad, offsets, ids)
+            mod._pending_apply = (grad, offsets, ids, psw)
 
             def _join(mod=mod, cur=cur, side=side):
                 cur.wait_stream(side)
@@ -493,24 +499,34 @@ def _fused_backward(ctx, mod, pooled: bool, grad, ids, offsets, who: str) -> Non
             k.fused_bwd_apply(spec.kind, pooled, grad, mod.weights.data, mod.opt_state, mod.layout, offsets,
                               ids.numel(), ctx.B, spec.lr, spec.eps, mod.grad_scale, ws, **extras)
     else:
+        extras = mod.opt_extras()
+        if psw is not None:
+            extras["per_sample_weights"] = psw
         k.fused_bwd(spec.kind, pooled, grad, mod.weights.data, mod.opt_state, mod.layout, ids, offsets, ctx.B,
-                    spec.lr, spec.eps, mod.grad_scale, **mod.opt_extras())
+                    spec.lr, spec.eps, mod.grad_scale, **extras)
 
 
 class _PooledLookup(torch.autograd.Function):
+    """psw: the KJT's per-sample weights (weighted bags, as torchrec's sharded lookup passes weights_or_none() to the
+    TBE), or None.  They are data: no gradient flows to them."""
+
     @staticmethod
-    def forward(ctx, hook, mod, ids, offsets, B):
-        out = Fn.backend().pooled_gather_fwd(mod.weights.data, mod.layout, ids, offsets, B)
+    def forward(ctx, hook, mod, ids, offsets, B, psw=None):
+        k = Fn.backend()
+        if psw is None:
+            out = k.pooled_gather_fwd(mod.weights.data, mod.layout, ids, offsets, B)
+        else:
+            out = k.pooled_gather_fwd(mod.weights.data, mod.layout, ids, offsets, B, per_sample_weights=psw)
         ctx.mod, ctx.B = mod, B
-        ctx.save_for_backward(ids, offsets)
-        _early_sort(ctx, mod, True, ids, offsets, B, hook is not None)
+        ctx.save_for_backward(ids, offsets, psw)
+        _early_sort(ctx, mod, True, ids, offsets, B, hook is not None, psw)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        ids, offsets = ctx.saved_tensors
-        _fused_backward(ctx, ctx.mod, True, Fn._rows_contig(grad_out), ids, offsets, "EmbeddingBagCollection")
-        return None, None, None, None, None
+        ids, offsets, psw = ctx.saved_tensors
+        _fused_backward(ctx, ctx.mod, True, Fn._rows_contig(grad_out), ids, offsets, "EmbeddingBagCollection", psw)
+        return None, None, None, None, None, None
 
 
 class _SeqLookup(torch.autograd.Function):
@@ -544,7 +560,11 @@ class EmbeddingBagCollection(_ArenaCollection):
         kjt = self._select(kjt)
         B = kjt.stride()
         hook = self._hook_tensor() if torch.is_grad_enabled() else None
-        return _PooledLookup.apply(hook, self, kjt.values(), kjt.offsets(), B)
+        psw = kjt.weights_or_none()
+        if psw is not None and psw.requires_grad:
+            raise NotImplementedError("EmbeddingBagCollection: per-sample weights that require grad (feature "
+                                      "processors) are not supported; the weights of a weighted id feature are data")
+        return _PooledLookup.apply(hook, self, kjt.values(), kjt.offsets(), B, psw)
 
     def forward(self, features: KeyedJaggedTensor) -> KeyedTensor:
         return KeyedTensor(self._embedding_names, self._lengths_per_key, self.pooled_values(features))

@@ -170,6 +170,8 @@ def _tensors_of(batch: Batch) -> List[torch.Tensor]:
     for k in sorted(batch.sparse_features):
         kjt = batch.sparse_features[k]
         out += [kjt.values(), kjt.lengths()]
+        if kjt.weights_or_none() is not None:      # weighted id features: replay must see the new weights too
+            out.append(kjt.weights_or_none())
     for k in sorted(batch.dense_features):
         out.append(batch.dense_features[k].values())
     for k in sorted(batch.labels):

@@ -183,7 +183,10 @@ def kjt_permute(kjt, indices: List[int]):
     lpk = kjt.length_per_key()
     out_nnz = sum(lpk[i] for i in indices)
     new_ids = backend().permute_ids(kjt.values(), kjt.offsets(), new_off, perm, B, out_nnz)
-    out = KeyedJaggedTensor([kjt.keys()[i] for i in indices], new_ids, lengths=new_len, offsets=new_off, stride=B)
+    w = kjt.weights_or_none()
+    new_w = None if w is None else backend().permute_weights(w, kjt.offsets(), new_off, perm, B, out_nnz)
+    out = KeyedJaggedTensor([kjt.keys()[i] for i in indices], new_ids, lengths=new_len, offsets=new_off, weights=new_w,
+                            stride=B)
     out._length_per_key = [lpk[i] for i in indices]
     return out
 

@@ -173,7 +173,7 @@ def _tile_path(lay: "FeatureLayout", optimizer: int = OPT_SGD, ex: Optional[dict
     import os
 
     return (os.environ.get("TZK_BWD_TILE", "0") == "1" and bool(lay.vec_ok) and lay.max_dim <= 128 and not lay.interleaved
-            and not norm_family(optimizer, ex or {}))
+            and not norm_family(optimizer, ex or {}) and (ex or {}).get("per_sample_weights") is None)
 
 
 def _table_dtype(weights: torch.Tensor, name: str = "weights") -> bool:
@@ -197,11 +197,14 @@ def _opt_args(optimizer: int, state, lr: float, eps: float, ex: dict):
     for t, nm in ((st2, "state2"), (step, "step")):
         if t is not None:
             _need(t, torch.float32, nm)
+    psw = ex.get("per_sample_weights")
+    if psw is not None:
+        _need(psw, torch.float32, "per_sample_weights")
     return TzkOptArgs(optimizer, lr, eps, float(ex.get("beta1", 0.9)), float(ex.get("beta2", 0.999)),
                       float(ex.get("weight_decay", 0.0)), float(ex.get("max_gradient", 0.0)),
                       _ptr(state), _ptr(st2), _ptr(step), int(bool(ex.get("weights_f16", False))),
                       int(bool(ex.get("interleaved", False))), float(ex.get("momentum", 0.9)),
-                      float(ex.get("eta", LARS_ETA)), int(ex.get("weight_decay_mode", WD_NONE)))
+                      float(ex.get("eta", LARS_ETA)), int(ex.get("weight_decay_mode", WD_NONE)), _ptr(psw))
 
 
 class CudaKernels:
@@ -238,7 +241,9 @@ class CudaKernels:
 
     # ------------------------------------------------------------------ K4
     def pooled_gather_fwd(self, weights: torch.Tensor, lay: FeatureLayout, ids: torch.Tensor,
-                          offsets: torch.Tensor, B: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                          offsets: torch.Tensor, B: int, out: Optional[torch.Tensor] = None,
+                          per_sample_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """per_sample_weights (fp32 [nnz], nullable): weighted bags, out = pool_l w[l] * row(ids[l])."""
         f16 = _table_dtype(weights)
         _need(ids, torch.int64, "ids")
         _need(offsets, torch.int64, "offsets")
@@ -248,6 +253,18 @@ class CudaKernels:
         if out is None:
             out = torch.empty((B, lay.total_dim), dtype=torch.float32, device=weights.device)
         out, ld = _rows2d(out, "out")
+        if per_sample_weights is not None:
+            _need(per_sample_weights, torch.float32, "per_sample_weights")
+            if per_sample_weights.numel() != ids.numel():
+                raise TzkError(f"per_sample_weights has {per_sample_weights.numel()} entries, ids {ids.numel()}")
+            if f16 and lay.stride is not None:
+                raise TzkError("strided (interleaved) tables are fp32")
+            check(self._lib.tzk_pooled_gather_fwd_weighted(
+                _ptr(weights), int(f16), _ptr(lay.d_w_off), _ptr(lay.d_rows), _ptr(lay.d_dim), _ptr(lay.d_stride),
+                _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(ids), _ptr(offsets), _ptr(per_sample_weights), F, B,
+                lay.max_dim, lay.vec_ok, _ptr(out), ld, _stream()), "tzk_pooled_gather_fwd_weighted")
+            self.launches += 1
+            return out
         if lay.stride is not None:
             if f16:
                 raise TzkError("strided (interleaved) tables are fp32")
@@ -294,8 +311,11 @@ class CudaKernels:
     def fused_bwd(self, optimizer: int, pooled: bool, grad_out: torch.Tensor, weights: torch.Tensor,
                   state: Optional[torch.Tensor], lay: FeatureLayout, ids: torch.Tensor, offsets: torch.Tensor,
                   B: int, lr: float, eps: float, grad_scale: float = 1.0, **ex) -> None:
-        """`ex` (optional): state2, step, beta1, beta2, weight_decay, max_gradient, momentum, eta, weight_decay_mode
-        -> tzk_fused_bwd_ex."""
+        """`ex` (optional): state2, step, beta1, beta2, weight_decay, max_gradient, momentum, eta, weight_decay_mode,
+        per_sample_weights (weighted bags, fp32 [nnz]) -> tzk_fused_bwd_ex."""
+        psw = ex.get("per_sample_weights")
+        if psw is not None and psw.numel() != ids.numel():
+            raise TzkError(f"per_sample_weights has {psw.numel()} entries, ids {ids.numel()}")
         if _table_dtype(weights):
             ex = dict(ex, weights_f16=True)
         if lay.interleaved:
@@ -307,7 +327,7 @@ class CudaKernels:
             _need(state, torch.float32, "state")
         F = lay.num_features
         nnz = ids.numel()
-        nb = self._lib.tzk_fused_bwd_workspace_bytes(nnz, lay.total_keys, lay.max_dim)
+        nb = self.fused_bwd_workspace_bytes(lay, nnz, weighted=psw is not None)
         ws = self._workspace("bwd", nb, weights.device)
         if ex:
             oa = _opt_args(optimizer, state, lr, eps, ex)
@@ -322,22 +342,36 @@ class CudaKernels:
                 _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(lay.d_key_base), _ptr(ids), _ptr(offsets), F, B, nnz,
                 lay.total_keys, lay.max_dim, lay.vec_ok, _ptr(weights), _ptr(state), lr, eps, grad_scale,
                 _ptr(ws), ws.numel(), _stream()), "tzk_fused_bwd")
-        # own launches next to CUB's radix sort: linearize, zero_counters, find_long_runs + the gradient half:
-        # fused_apply (short runs and the long-run chunk CTAs in ONE launch), or tile_update + carry_combine
-        self.launches += 5 if _tile_path(lay, optimizer, ex) else 4
+        # own launches next to CUB's radix sort: linearize, zero_counters, find_long_runs (+ sorted_bag_weight for
+        # weighted bags) + the gradient half: fused_apply (short runs and the long-run chunk CTAs in ONE launch), or
+        # tile_update + carry_combine
+        self.launches += (5 if _tile_path(lay, optimizer, ex) else 4) + (psw is not None)
 
-    def fused_bwd_workspace_bytes(self, lay: FeatureLayout, nnz: int) -> int:
-        return int(self._lib.tzk_fused_bwd_workspace_bytes(nnz, lay.total_keys, lay.max_dim))
+    def fused_bwd_workspace_bytes(self, lay: FeatureLayout, nnz: int, weighted: bool = False) -> int:
+        fn = self._lib.tzk_fused_bwd_weighted_workspace_bytes if weighted else self._lib.tzk_fused_bwd_workspace_bytes
+        return int(fn(nnz, lay.total_keys, lay.max_dim))
 
     def fused_bwd_sort(self, pooled: bool, lay: FeatureLayout, ids: torch.Tensor, offsets: torch.Tensor, B: int,
-                       ws: torch.Tensor) -> None:
+                       ws: torch.Tensor, per_sample_weights: Optional[torch.Tensor] = None) -> None:
         """First half of fused_bwd (linearize + radix sort of (table,row) keys): needs only the ids, so callers run
-        it on a side stream while the forward pass is still going.  `ws` must stay untouched until fused_bwd_apply."""
+        it on a side stream while the forward pass is still going.  `ws` must stay untouched until fused_bwd_apply.
+        per_sample_weights: weighted bags (tzk_fused_bwd_sort_weighted); the apply then gets the same tensor."""
         _need(ids, torch.int64, "ids")
         _need(offsets, torch.int64, "offsets")
         nnz = ids.numel()
-        if ws.numel() < self.fused_bwd_workspace_bytes(lay, nnz):
+        psw = per_sample_weights
+        if ws.numel() < self.fused_bwd_workspace_bytes(lay, nnz, weighted=psw is not None):
             raise TzkError("fused_bwd_sort: workspace too small")
+        if psw is not None:
+            _need(psw, torch.float32, "per_sample_weights")
+            if psw.numel() != nnz:
+                raise TzkError(f"per_sample_weights has {psw.numel()} entries, ids {nnz}")
+            check(self._lib.tzk_fused_bwd_sort_weighted(
+                int(pooled), _ptr(lay.d_rows), _ptr(lay.d_key_base), _ptr(ids), _ptr(offsets), _ptr(psw),
+                lay.num_features, B, nnz, lay.total_keys, lay.max_dim, _ptr(ws), ws.numel(), _stream()),
+                "tzk_fused_bwd_sort_weighted")
+            self.launches += 4
+            return
         check(self._lib.tzk_fused_bwd_sort(int(pooled), _ptr(lay.d_rows), _ptr(lay.d_key_base), _ptr(ids),
                                            _ptr(offsets), lay.num_features, B, nnz, lay.total_keys, lay.max_dim,
                                            _ptr(ws), ws.numel(), _stream()), "tzk_fused_bwd_sort")
@@ -435,6 +469,19 @@ class CudaKernels:
         out = torch.empty(out_nnz, dtype=torch.int64, device=ids.device)
         check(self._lib.tzk_permute_ids(_ptr(ids), _ptr(in_offsets), _ptr(out_offsets), _ptr(perm),
                                         perm.numel(), B, _ptr(out), _stream()), "tzk_permute_ids")
+        self.launches += 1
+        return out
+
+    def permute_weights(self, weights: torch.Tensor, in_offsets: torch.Tensor, out_offsets: torch.Tensor,
+                        perm: torch.Tensor, B: int, out_nnz: int) -> torch.Tensor:
+        """The per-sample weights of a weighted KJT, moved like its ids (permute_ids)."""
+        _need(weights, torch.float32, "weights")
+        _need(in_offsets, torch.int64, "in_offsets")
+        _need(out_offsets, torch.int64, "out_offsets")
+        _need(perm, torch.int32, "perm")
+        out = torch.empty(out_nnz, dtype=torch.float32, device=weights.device)
+        check(self._lib.tzk_permute_weights(_ptr(weights), _ptr(in_offsets), _ptr(out_offsets), _ptr(perm),
+                                            perm.numel(), B, _ptr(out), _stream()), "tzk_permute_weights")
         self.launches += 1
         return out
 

@@ -527,8 +527,11 @@ def enable_peer_exchange(sm, batch_size: int, ids_per_feature: Optional[Dict[str
             per_f = [int(ids_per_feature.get(name, batch_size)) for name in g.feature_names]
         states.append(PeerState(g, sm.plan, grp, batch_size, per_f))
     pooled = sm._pooled
+    from .distributed import reject_weighted
 
     def forward(features):
+        if pooled:
+            reject_weighted(features)
         keys, lens, vals = [], [], []
         out = {}
         for g, st in zip(sm.groups, states):
