@@ -465,6 +465,34 @@ int tzk_fused_bwd_apply_peer(const tzk_opt_args* opt, int32_t pooled, const uint
                              int32_t max_dim, int32_t vec_ok, float* weights, float grad_scale, void* workspace,
                              size_t workspace_bytes, tzk_stream_t stream);
 
+/* ---- weighted bags on the peer step ([EXT] torchrec's sharded lookup passes features.weights_or_none() to the TBE on
+ * every sharding type).  The per-sample weights never leave the sample's rank: its gather pools w[l] * row, its
+ * bucketize records the weight of every wire slot in a LOCAL buffer, its push sends w * g (/ L).  The owner's update is
+ * the unweighted one (grad_scale 1/W).  Pooled layouts, push transport only; the pull transport
+ * (tzk_fused_bwd_apply_peer) and tzk_peer_small_update keep requiring opt->per_sample_weights == NULL.
+ *   peer_pooled_gather_fwd_weighted : tzk_peer_pooled_gather_fwd / _sel (feat_sel NULL: every feature) with the
+ *                            arithmetic of tzk_pooled_gather_fwd_weighted: acc = w[l0] * row, then fmaf(w[l], row, acc)
+ *                            in list order, MEAN * 1/L — the same bits as the unsharded weighted lookup.
+ *   peer_bucketize_weighted: tzk_peer_bucketize (pooled != 0) + wire_w[r * cap + slot] = per_sample_weights[l], wire_w a
+ *                            local float buffer of W * cap entries.
+ *   peer_push_grad_weighted: tzk_peer_push_grad (pooled != 0) with every slice scaled by ((1/L for MEAN) * wire_w[s]). */
+int tzk_peer_pooled_gather_fwd_weighted(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
+                                        const int64_t* feat_block, const int32_t* feat_owner, const int32_t* feat_dim,
+                                        const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
+                                        const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t max_dim,
+                                        float* out, int64_t ld_out, const float* mirror, const int64_t* feat_mirror_off,
+                                        const float* per_sample_weights, const int32_t* feat_sel, int32_t n_sel,
+                                        tzk_stream_t stream);
+int tzk_peer_bucketize_weighted(const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t W,
+                                const int64_t* feat_block, const int32_t* feat_owner, const int64_t* feat_rows,
+                                const int64_t* rf_key_base, int32_t pooled, int64_t cap, int64_t* wire_key,
+                                int32_t* wire_idx, int32_t* counts, void* workspace, size_t workspace_bytes,
+                                const float* per_sample_weights, float* wire_w, tzk_stream_t stream);
+int tzk_peer_push_grad_weighted(const uint64_t* recv_ptrs, const float* grad, int64_t ld_grad, const int32_t* feat_col,
+                                const int32_t* feat_pool, const int64_t* offsets, const int32_t* wire_idx,
+                                const int32_t* counts, int32_t me, int32_t W, int64_t cap, int32_t B, int32_t D,
+                                int32_t pooled, const float* wire_w, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

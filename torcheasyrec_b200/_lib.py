@@ -137,6 +137,12 @@ SIGNATURES = {
         c_int32,
         [P, c_int32, P, c_int64, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, c_int64, c_int32, c_int64,
          c_int32, c_int32, P, c_float, P, c_size_t, P]),
+    "tzk_peer_pooled_gather_fwd_weighted": (
+        c_int32, [P, P, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, P, c_int64, P, P, P, P, c_int32, P]),
+    "tzk_peer_bucketize_weighted": (
+        c_int32, [P, P, c_int32, c_int32, c_int32, P, P, P, P, c_int32, c_int64, P, P, P, P, c_size_t, P, P, P]),
+    "tzk_peer_push_grad_weighted": (
+        c_int32, [P, P, c_int64, P, P, P, P, P, c_int32, c_int32, c_int64, c_int32, c_int32, c_int32, P, P]),
 }
 
 _lib = None

@@ -22,6 +22,9 @@
 //             concurrently (different streams) use different flag arrays / epochs.
 //   dense     peer_allreduce_mean_kernel: the replicated dense gradients, summed in rank order straight out of every
 //             rank's published flat buffer (bit-identical on every rank; replaces the DDP all-reduce, SURVEY C5).
+//   weighted  (per-sample weights of weighted id features; pooled, push transport) the weights never leave the sample's
+//             rank: the gather pools w * row, the scatter records each wire slot's weight in a local buffer, the push
+//             sends w * g (/ L).  Each weighted kernel is the unweighted one's body with a compile-time switch.
 //
 // This file compiles for the host too (TZK_CPU_SHIM, tests/test_peer_exchange_model.py runs the kernels' source on
 // std::threads), so it uses plain CUDA + warp shuffles only; the barrier (PTX) is excluded from that build.
@@ -84,16 +87,18 @@ __device__ __forceinline__ int owner_of(int64_t id, int64_t block, int owner, in
 // ---- forward: requester-side gather over peer memory ------------------------------------------------------------
 // A CTA owns 32 consecutive samples x all features (its output block is contiguous); a bag is served by G lanes,
 // one 16-B load per lane per row; U bags per lane group are in flight because a remote row costs an NVLink round trip.
-template <int G>
-__global__ void __launch_bounds__(kThreads)
-peer_pooled_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off, const int64_t* __restrict__ feat_rows,
-                              const int64_t* __restrict__ feat_block, const int32_t* __restrict__ feat_owner,
-                              const int32_t* __restrict__ feat_dim, const int32_t* __restrict__ feat_col,
-                              const int32_t* __restrict__ feat_pool, const int64_t* __restrict__ ids,
-                              const int64_t* __restrict__ offsets, int F, int B, int W, float* __restrict__ out,
-                              int64_t ld_out, const float* __restrict__ mirror,
-                              const int64_t* __restrict__ feat_mirror_off, const int32_t* __restrict__ feat_sel,
-                              int n_sel) {
+// WTD: weighted bags (per-sample weights psw[l], the sample's own rank holds them): out = sum_l psw[l] * row(ids[l]) in
+// list order as acc = fmaf(psw[l], row, acc), the first term psw[l0] * row, MEAN then * 1/L — the arithmetic of
+// tzk_gather.cu's pooled_gather_fwd_weighted_kernel, so the bits equal the unsharded weighted lookup's.
+template <int G, bool WTD>
+__device__ __forceinline__ void
+peer_pooled_gather_body(const Peers& tables, const int64_t* __restrict__ rf_w_off, const int64_t* __restrict__ feat_rows,
+                        const int64_t* __restrict__ feat_block, const int32_t* __restrict__ feat_owner,
+                        const int32_t* __restrict__ feat_dim, const int32_t* __restrict__ feat_col,
+                        const int32_t* __restrict__ feat_pool, const int64_t* __restrict__ ids,
+                        const int64_t* __restrict__ offsets, int F, int B, int W, float* __restrict__ out,
+                        int64_t ld_out, const float* __restrict__ mirror, const int64_t* __restrict__ feat_mirror_off,
+                        const int32_t* __restrict__ feat_sel, int n_sel, const float* __restrict__ psw) {
   // feat_sel (nullable): this launch serves only the listed features (e.g. the mirrored ones, or the ones whose rows
   // cross NVLink — two launches on two streams overlap the local and the remote half of the lookup)
   constexpr int NG = kThreads / G, TB = 32, U = 8;
@@ -148,6 +153,11 @@ peer_pooled_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_
       int64_t id0[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) id0[u] = len[u] > 0 ? __ldg(ids + s[u]) : 0;
+      float w0[U];                        // WTD: the first weight of each bag, loaded next to its first id
+      if constexpr (WTD) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) w0[u] = len[u] > 0 ? __ldg(psw + s[u]) : 0.f;
+      }
       float4 acc[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -168,8 +178,17 @@ peer_pooled_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_
           float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
           if (len[u] > 0) {
             a = (c == lane * 4) ? acc[u] : ld_peer_f4(row_ptr(f, d, id0[u]) + c);
-            for (int l = 1; l < len[u]; ++l)
-              a = f4_add(a, ld_peer_f4(row_ptr(f, d, __ldg(ids + s[u] + l)) + c));
+            if constexpr (WTD) {
+              a = make_float4(a.x * w0[u], a.y * w0[u], a.z * w0[u], a.w * w0[u]);
+              for (int l = 1; l < len[u]; ++l) {
+                const float wl = __ldg(psw + s[u] + l);
+                const float4 r = ld_peer_f4(row_ptr(f, d, __ldg(ids + s[u] + l)) + c);
+                a = make_float4(fmaf(wl, r.x, a.x), fmaf(wl, r.y, a.y), fmaf(wl, r.z, a.z), fmaf(wl, r.w, a.w));
+              }
+            } else {
+              for (int l = 1; l < len[u]; ++l)
+                a = f4_add(a, ld_peer_f4(row_ptr(f, d, __ldg(ids + s[u] + l)) + c));
+            }
             if (d.pool == 1) {
               const float inv = 1.0f / (float)len[u];
               a = make_float4(a.x * inv, a.y * inv, a.z * inv, a.w * inv);
@@ -180,6 +199,35 @@ peer_pooled_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_
       }
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+peer_pooled_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off, const int64_t* __restrict__ feat_rows,
+                              const int64_t* __restrict__ feat_block, const int32_t* __restrict__ feat_owner,
+                              const int32_t* __restrict__ feat_dim, const int32_t* __restrict__ feat_col,
+                              const int32_t* __restrict__ feat_pool, const int64_t* __restrict__ ids,
+                              const int64_t* __restrict__ offsets, int F, int B, int W, float* __restrict__ out,
+                              int64_t ld_out, const float* __restrict__ mirror,
+                              const int64_t* __restrict__ feat_mirror_off, const int32_t* __restrict__ feat_sel,
+                              int n_sel) {
+  peer_pooled_gather_body<G, false>(tables, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
+                                    ids, offsets, F, B, W, out, ld_out, mirror, feat_mirror_off, feat_sel, n_sel,
+                                    nullptr);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+peer_pooled_gather_fwd_weighted_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off,
+                                       const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                                       const int32_t* __restrict__ feat_owner, const int32_t* __restrict__ feat_dim,
+                                       const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                                       const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F,
+                                       int B, int W, float* __restrict__ out, int64_t ld_out,
+                                       const float* __restrict__ mirror, const int64_t* __restrict__ feat_mirror_off,
+                                       const int32_t* __restrict__ feat_sel, int n_sel, const float* __restrict__ psw) {
+  peer_pooled_gather_body<G, true>(tables, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
+                                   ids, offsets, F, B, W, out, ld_out, mirror, feat_mirror_off, feat_sel, n_sel, psw);
 }
 
 // un-pooled (sequence) lookup: one lane group per id position, feature by binary search over the segment starts
@@ -415,12 +463,15 @@ peer_bkt_scan_kernel(int32_t* __restrict__ tile_counts, int64_t n_tiles, int W, 
   }
 }
 
-__global__ void __launch_bounds__(kThreads)
-peer_bkt_scatter_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets,
-                        const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
-                        const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ rf_key_base, int F, int B,
-                        int W, int pooled, int64_t cap, const int32_t* __restrict__ tile_base,
-                        int64_t* __restrict__ wire_key, int32_t* __restrict__ wire_idx) {
+// WTD (pooled): also wire_w[slot] = psw[l], the weight of the id in that slot — read only by this rank's own push
+template <bool WTD>
+__device__ __forceinline__ void
+peer_bkt_scatter_body(const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets,
+                      const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                      const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ rf_key_base, int F, int B,
+                      int W, int pooled, int64_t cap, const int32_t* __restrict__ tile_base,
+                      int64_t* __restrict__ wire_key, int32_t* __restrict__ wire_idx, const float* __restrict__ psw,
+                      float* __restrict__ wire_w) {
   TZK_DYN_SMEM(unsigned char, smem_raw);
   BktFeat* fd = reinterpret_cast<BktFeat*>(smem_raw);
   int32_t* sbase = reinterpret_cast<int32_t*>(fd + F);            // [W][kThreads]: next slot of (destination, thread)
@@ -486,9 +537,31 @@ peer_bkt_scatter_kernel(const int64_t* __restrict__ ids, const int64_t* __restri
       if (slot < cap) {               // ids beyond the wire capacity are dropped; the overflow flag reports it
         wire_key[(int64_t)r * cap + slot] = __ldg(rf_key_base + (int64_t)r * F + f) + loc;
         wire_idx[(int64_t)r * cap + slot] = pooled ? (int32_t)bag : (int32_t)l;
+        if constexpr (WTD) wire_w[(int64_t)r * cap + slot] = __ldg(psw + l);
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(kThreads)
+peer_bkt_scatter_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets,
+                        const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                        const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ rf_key_base, int F, int B,
+                        int W, int pooled, int64_t cap, const int32_t* __restrict__ tile_base,
+                        int64_t* __restrict__ wire_key, int32_t* __restrict__ wire_idx) {
+  peer_bkt_scatter_body<false>(ids, offsets, feat_rows, feat_block, feat_owner, rf_key_base, F, B, W, pooled, cap,
+                               tile_base, wire_key, wire_idx, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads, 1)     // (the default register heuristic spilled the per-destination bases)
+peer_bkt_scatter_weighted_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets,
+                                 const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                                 const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ rf_key_base, int F,
+                                 int B, int W, int64_t cap, const int32_t* __restrict__ tile_base,
+                                 int64_t* __restrict__ wire_key, int32_t* __restrict__ wire_idx,
+                                 const float* __restrict__ psw, float* __restrict__ wire_w) {
+  peer_bkt_scatter_body<true>(ids, offsets, feat_rows, feat_block, feat_owner, rf_key_base, F, B, W, 1, cap, tile_base,
+                              wire_key, wire_idx, psw, wire_w);
 }
 
 // ---- publish the pooled-output gradient: dst = grad (MEAN bags pre-divided by their length, so that the owner needs
@@ -518,12 +591,16 @@ peer_publish_grad_kernel(const float* __restrict__ grad, int64_t ld_grad, const 
 // 64-B rows at the destination, so the NVLink writes are long coalesced bursts (posted, no round trip) while the
 // scattered 64-B reads stay in local HBM.  The slice comes straight from the pooled-output gradient (no staging copy);
 // MEAN bags are divided by their length here, so the owner's update needs nothing but the row.
-template <int G>
-__global__ void __launch_bounds__(kThreads)
-peer_push_grad_kernel(const __grid_constant__ Peers recv, const float* __restrict__ grad, int64_t ld_grad,
-                      const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
-                      const int64_t* __restrict__ offsets, const int32_t* __restrict__ wire_idx,
-                      const int32_t* __restrict__ counts, int me, int W, int64_t cap, int B, int D, int pooled) {
+// WTD (pooled): the slot's per-sample weight wire_w[s] (tzk_peer_bucketize_weighted) joins the scale.  The order is
+// sc = (1/L) * w (SUM: 1 * w), then slice * sc — the unsharded weighted update's entry scale (grad_scale/L) * w with
+// grad_scale = 1; the owner's update multiplies by its 1/W after that.  All-ones weights leave every bit unchanged.
+template <int G, bool WTD>
+__device__ __forceinline__ void
+peer_push_grad_body(const Peers& recv, const float* __restrict__ grad, int64_t ld_grad,
+                    const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                    const int64_t* __restrict__ offsets, const int32_t* __restrict__ wire_idx,
+                    const int32_t* __restrict__ counts, int me, int W, int64_t cap, int B, int D, int pooled,
+                    const float* __restrict__ wire_w) {
   constexpr int NG = kThreads / G;
   const int lane = threadIdx.x % G;
   const int64_t n = (int64_t)W * cap;
@@ -532,6 +609,8 @@ peer_push_grad_kernel(const __grid_constant__ Peers recv, const float* __restric
     const int64_t j = s - (int64_t)r * cap;
     if (j >= __ldg(counts + r)) continue;
     const int32_t idx = __ldg(wire_idx + s);
+    float w = 1.f;
+    if constexpr (WTD) w = __ldg(wire_w + s);                  // (independent of idx: in flight next to it)
     const float* src;
     float sc = 1.f;
     if (pooled) {
@@ -541,6 +620,7 @@ peer_push_grad_kernel(const __grid_constant__ Peers recv, const float* __restric
         const int64_t L = __ldg(offsets + idx + 1) - __ldg(offsets + idx);
         sc = 1.0f / (float)L;                       // L >= 1: the slot exists
       }
+      if constexpr (WTD) sc *= w;
     } else {
       src = grad + (int64_t)idx * ld_grad;
     }
@@ -551,6 +631,27 @@ peer_push_grad_kernel(const __grid_constant__ Peers recv, const float* __restric
       *reinterpret_cast<float4*>(dst + c) = v;
     }
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+peer_push_grad_kernel(const __grid_constant__ Peers recv, const float* __restrict__ grad, int64_t ld_grad,
+                      const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                      const int64_t* __restrict__ offsets, const int32_t* __restrict__ wire_idx,
+                      const int32_t* __restrict__ counts, int me, int W, int64_t cap, int B, int D, int pooled) {
+  peer_push_grad_body<G, false>(recv, grad, ld_grad, feat_col, feat_pool, offsets, wire_idx, counts, me, W, cap, B, D,
+                                pooled, nullptr);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+peer_push_grad_weighted_kernel(const __grid_constant__ Peers recv, const float* __restrict__ grad, int64_t ld_grad,
+                               const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                               const int64_t* __restrict__ offsets, const int32_t* __restrict__ wire_idx,
+                               const int32_t* __restrict__ counts, int me, int W, int64_t cap, int B, int D,
+                               const float* __restrict__ wire_w) {
+  peer_push_grad_body<G, true>(recv, grad, ld_grad, feat_col, feat_pool, offsets, wire_idx, counts, me, W, cap, B, D, 1,
+                               wire_w);
 }
 
 // ---- dense gradients: out = mean over ranks of src_r, summed in rank order (the same bits on every rank) --------------
@@ -615,7 +716,7 @@ static int peer_pooled_gather_fwd_impl(const uint64_t* table_ptrs, const int64_t
                                        const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t max_dim,
                                        float* out, int64_t ld_out, const float* mirror,
                                        const int64_t* feat_mirror_off, const int32_t* feat_sel, int32_t n_sel,
-                                       void* stream) {
+                                       void* stream, const float* psw = nullptr) {
   Peers t;
   if (fill(&t, table_ptrs, W) || F <= 0 || B <= 0 || max_dim <= 0 || (max_dim % 4) || (ld_out % 4)) return 1;
   if (feat_sel && (n_sel < 0 || n_sel > F)) return 1;
@@ -627,10 +728,20 @@ static int peer_pooled_gather_fwd_impl(const uint64_t* table_ptrs, const int64_t
   TZK_LAUNCH((peer_pooled_gather_fwd_kernel<G>), grid, kThreads, smem, st, t, rf_w_off, feat_rows, feat_block,         \
              feat_owner, feat_dim, feat_col, feat_pool, ids, offsets, F, B, W, out, ld_out, mirror, feat_mirror_off,   \
              feat_sel, n_sel)
-  if (max_dim <= 16) TZK_PEER_LAUNCH(4);
+#define TZK_PEER_LAUNCH_W(G)                                                                                           \
+  TZK_LAUNCH((peer_pooled_gather_fwd_weighted_kernel<G>), grid, kThreads, smem, st, t, rf_w_off, feat_rows,            \
+             feat_block, feat_owner, feat_dim, feat_col, feat_pool, ids, offsets, F, B, W, out, ld_out, mirror,        \
+             feat_mirror_off, feat_sel, n_sel, psw)
+  if (psw) {
+    if (max_dim <= 16) TZK_PEER_LAUNCH_W(4);
+    else if (max_dim <= 32) TZK_PEER_LAUNCH_W(8);
+    else if (max_dim <= 64) TZK_PEER_LAUNCH_W(16);
+    else TZK_PEER_LAUNCH_W(32);
+  } else if (max_dim <= 16) TZK_PEER_LAUNCH(4);
   else if (max_dim <= 32) TZK_PEER_LAUNCH(8);
   else if (max_dim <= 64) TZK_PEER_LAUNCH(16);
   else TZK_PEER_LAUNCH(32);
+#undef TZK_PEER_LAUNCH_W
 #undef TZK_PEER_LAUNCH
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
@@ -660,6 +771,22 @@ extern "C" int tzk_peer_pooled_gather_fwd_sel(const uint64_t* table_ptrs, const 
   return peer_pooled_gather_fwd_impl(table_ptrs, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
                                      ids, offsets, F, B, W, max_dim, out, ld_out, mirror, feat_mirror_off, feat_sel, n_sel,
                                      stream);
+}
+
+// Weighted bags (per_sample_weights [nnz] of this rank's own batch): the same lookup, pooled as
+// tzk_pooled_gather_fwd_weighted does.  feat_sel nullable (NULL: every feature, as tzk_peer_pooled_gather_fwd).
+extern "C" int tzk_peer_pooled_gather_fwd_weighted(const uint64_t* table_ptrs, const int64_t* rf_w_off,
+                                                   const int64_t* feat_rows, const int64_t* feat_block,
+                                                   const int32_t* feat_owner, const int32_t* feat_dim,
+                                                   const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
+                                                   const int64_t* offsets, int32_t F, int32_t B, int32_t W,
+                                                   int32_t max_dim, float* out, int64_t ld_out, const float* mirror,
+                                                   const int64_t* feat_mirror_off, const float* per_sample_weights,
+                                                   const int32_t* feat_sel, int32_t n_sel, void* stream) {
+  if (!per_sample_weights) return 1;
+  return peer_pooled_gather_fwd_impl(table_ptrs, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
+                                     ids, offsets, F, B, W, max_dim, out, ld_out, mirror, feat_mirror_off, feat_sel, n_sel,
+                                     stream, per_sample_weights);
 }
 
 extern "C" int tzk_peer_seq_gather_fwd(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
@@ -739,11 +866,11 @@ extern "C" size_t tzk_peer_bucketize_workspace_bytes(int32_t F, int32_t B, int32
 // ids of the local batch -> this rank's wire buffers.  Destination r's entries start at r * cap, in (feature, bag,
 // position) order; wire_key = rf_key_base[r * F + f] + owner-local row, wire_idx = bag index (pooled) or id position
 // (sequence).  counts [W + 1]: ids per destination (clamped to cap) and, in counts[W], 1 if any destination overflowed.
-extern "C" int tzk_peer_bucketize(const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t W,
-                                  const int64_t* feat_block, const int32_t* feat_owner, const int64_t* feat_rows,
-                                  const int64_t* rf_key_base, int32_t pooled, int64_t cap, int64_t* wire_key,
-                                  int32_t* wire_idx, int32_t* counts, void* workspace, size_t workspace_bytes,
-                                  void* stream) {
+static int peer_bucketize_impl(const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t W,
+                               const int64_t* feat_block, const int32_t* feat_owner, const int64_t* feat_rows,
+                               const int64_t* rf_key_base, int32_t pooled, int64_t cap, int64_t* wire_key,
+                               int32_t* wire_idx, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream,
+                               const float* psw = nullptr, float* wire_w = nullptr) {
   if (F <= 0 || B <= 0 || W < 1 || W > kMaxPeers || cap <= 0 || cap * W >= ((int64_t)1 << 31)) return 1;
   if (!offsets || !feat_block || !feat_rows || !rf_key_base || !wire_key || !wire_idx || !counts || !workspace)
     return 1;
@@ -756,9 +883,36 @@ extern "C" int tzk_peer_bucketize(const int64_t* ids, const int64_t* offsets, in
              feat_owner, F, B, W, tile_counts, counts);
   TZK_LAUNCH((peer_bkt_scan_kernel), (unsigned)W, 1024, (size_t)32 * 4, st, tile_counts, tiles, W, cap, counts);
   const size_t smem_s = (size_t)F * sizeof(BktFeat) + (size_t)W * kThreads * 4 + (size_t)W * 8 * 4;
-  TZK_LAUNCH((peer_bkt_scatter_kernel), (unsigned)tiles, kThreads, smem_s, st, ids, offsets, feat_rows, feat_block,
-             feat_owner, rf_key_base, F, B, W, pooled, cap, tile_counts, wire_key, wire_idx);
+  if (wire_w) {
+    TZK_LAUNCH((peer_bkt_scatter_weighted_kernel), (unsigned)tiles, kThreads, smem_s, st, ids, offsets, feat_rows,
+               feat_block, feat_owner, rf_key_base, F, B, W, cap, tile_counts, wire_key, wire_idx, psw, wire_w);
+  } else {
+    TZK_LAUNCH((peer_bkt_scatter_kernel), (unsigned)tiles, kThreads, smem_s, st, ids, offsets, feat_rows, feat_block,
+               feat_owner, rf_key_base, F, B, W, pooled, cap, tile_counts, wire_key, wire_idx);
+  }
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+extern "C" int tzk_peer_bucketize(const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t W,
+                                  const int64_t* feat_block, const int32_t* feat_owner, const int64_t* feat_rows,
+                                  const int64_t* rf_key_base, int32_t pooled, int64_t cap, int64_t* wire_key,
+                                  int32_t* wire_idx, int32_t* counts, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  return peer_bucketize_impl(ids, offsets, F, B, W, feat_block, feat_owner, feat_rows, rf_key_base, pooled, cap, wire_key,
+                             wire_idx, counts, workspace, workspace_bytes, stream);
+}
+
+// Weighted bags (pooled only): tzk_peer_bucketize plus wire_w [W * cap] (this rank's local memory, not symmetric), the
+// per-sample weight of the id in every wire slot, written next to its key and bag.  Only this rank's push reads it.
+extern "C" int tzk_peer_bucketize_weighted(const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t W,
+                                           const int64_t* feat_block, const int32_t* feat_owner,
+                                           const int64_t* feat_rows, const int64_t* rf_key_base, int32_t pooled,
+                                           int64_t cap, int64_t* wire_key, int32_t* wire_idx, int32_t* counts,
+                                           void* workspace, size_t workspace_bytes, const float* per_sample_weights,
+                                           float* wire_w, void* stream) {
+  if (!pooled || !per_sample_weights || !wire_w) return 1;
+  return peer_bucketize_impl(ids, offsets, F, B, W, feat_block, feat_owner, feat_rows, rf_key_base, pooled, cap, wire_key,
+                             wire_idx, counts, workspace, workspace_bytes, stream, per_sample_weights, wire_w);
 }
 
 extern "C" int tzk_peer_publish_grad(const float* grad, int64_t ld_grad, const int32_t* feat_col, const int32_t* feat_dim,
@@ -786,6 +940,29 @@ extern "C" int tzk_peer_push_grad(const uint64_t* recv_ptrs, const float* grad, 
 #define TZK_PEER_LAUNCH(G)                                                                                           \
   TZK_LAUNCH((peer_push_grad_kernel<G>), grid_for((slots + kThreads / G - 1) / (kThreads / G)), kThreads, 0, st, p,  \
              grad, ld_grad, feat_col, feat_pool, offsets, wire_idx, counts, me, W, cap, B, D, pooled)
+  if (D <= 16) TZK_PEER_LAUNCH(4);
+  else if (D <= 32) TZK_PEER_LAUNCH(8);
+  else if (D <= 64) TZK_PEER_LAUNCH(16);
+  else TZK_PEER_LAUNCH(32);
+#undef TZK_PEER_LAUNCH
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+// Weighted bags (pooled only): tzk_peer_push_grad with every slice scaled by its slot's weight wire_w[s]
+// (tzk_peer_bucketize_weighted), folded into the MEAN 1/L — the pushed row is w * g (/ L).
+extern "C" int tzk_peer_push_grad_weighted(const uint64_t* recv_ptrs, const float* grad, int64_t ld_grad,
+                                           const int32_t* feat_col, const int32_t* feat_pool, const int64_t* offsets,
+                                           const int32_t* wire_idx, const int32_t* counts, int32_t me, int32_t W,
+                                           int64_t cap, int32_t B, int32_t D, int32_t pooled, const float* wire_w,
+                                           void* stream) {
+  Peers p;
+  if (fill(&p, recv_ptrs, W) || me < 0 || me >= W || cap <= 0 || B <= 0 || D <= 0 || (D % 4) || (ld_grad % 4)) return 1;
+  if (!pooled || !wire_w || !grad || !wire_idx || !counts || !feat_col || !feat_pool || !offsets) return 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int64_t slots = (int64_t)W * cap;
+#define TZK_PEER_LAUNCH(G)                                                                                           \
+  TZK_LAUNCH((peer_push_grad_weighted_kernel<G>), grid_for((slots + kThreads / G - 1) / (kThreads / G)), kThreads, 0, \
+             st, p, grad, ld_grad, feat_col, feat_pool, offsets, wire_idx, counts, me, W, cap, B, D, wire_w)
   if (D <= 16) TZK_PEER_LAUNCH(4);
   else if (D <= 32) TZK_PEER_LAUNCH(8);
   else if (D <= 64) TZK_PEER_LAUNCH(16);

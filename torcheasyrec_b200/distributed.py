@@ -460,11 +460,13 @@ class _ShardedBase(nn.Module):
 
 
 def reject_weighted(features: KeyedJaggedTensor) -> None:
-    """Sharded pooled lookups do not carry per-sample weights yet (the bucketize / push kernels would have to move them
-    with the ids): a weighted KJT raises instead of being pooled as a plain sum.  Host-side, no device sync."""
+    """The NCCL exchange of sharded pooled lookups does not carry per-sample weights (its all-to-alls would have to
+    move them with the ids): a weighted KJT raises instead of being pooled as a plain sum.  The peer exchange keeps
+    the weights on the sample's rank and supports them.  Host-side, no device sync."""
     if features.weights_or_none() is not None:
-        raise NotImplementedError("weighted id features (per-sample weights) on a sharded EmbeddingBagCollection are not "
-                                  "supported yet; use an unsharded collection")
+        raise NotImplementedError("weighted id features (per-sample weights) on a sharded EmbeddingBagCollection need "
+                                  "exchange=\"peer\" (the NCCL exchange does not carry them); or use an unsharded "
+                                  "collection")
 
 
 class ShardedEmbeddingBagCollection(_ShardedBase):
@@ -474,7 +476,8 @@ class ShardedEmbeddingBagCollection(_ShardedBase):
         return self._configs
 
     def forward(self, features: KeyedJaggedTensor) -> KeyedTensor:
-        reject_weighted(features)
+        if getattr(self, "_exchange", "nccl") != "peer":     # (the peer exchange's forward takes the weights)
+            reject_weighted(features)
         if self._maybe_enable_peer(features):
             return self.forward(features)
         keys, lens, vals = [], [], []

@@ -545,8 +545,10 @@ class CudaKernels:
                                feat_owner: torch.Tensor, lay: FeatureLayout, ids: torch.Tensor, offsets: torch.Tensor,
                                B: int, W: int, out: Optional[torch.Tensor] = None, mirror: Optional[torch.Tensor] = None,
                                feat_mirror_off: Optional[torch.Tensor] = None,
-                               feat_sel: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """`feat_sel` (device int32 indices): serve only these features (their output columns); `out` is then required."""
+                               feat_sel: Optional[torch.Tensor] = None,
+                               per_sample_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`feat_sel` (device int32 indices): serve only these features (their output columns); `out` is then required.
+        `per_sample_weights` (fp32 [nnz], nullable): weighted bags, pooled as pooled_gather_fwd pools them."""
         _need(ids, torch.int64, "ids")
         _need(offsets, torch.int64, "offsets")
         F = lay.num_features
@@ -557,6 +559,20 @@ class CudaKernels:
         if out is None:
             out = torch.empty((B, lay.total_dim), dtype=torch.float32, device=ids.device)
         out, ld = _rows2d(out, "out")
+        psw = per_sample_weights
+        if psw is not None and ids.numel():      # (no ids: every bag is empty, the unweighted launch writes the zeros)
+            _need(psw, torch.float32, "per_sample_weights")
+            if psw.numel() != ids.numel():
+                raise TzkError(f"per_sample_weights has {psw.numel()} entries, ids {ids.numel()}")
+            if feat_sel is not None:
+                _need(feat_sel, torch.int32, "feat_sel")
+            check(self._lib.tzk_peer_pooled_gather_fwd_weighted(
+                tables.ptrs, _ptr(rf_w_off), _ptr(feat_rows), _ptr(feat_block), _ptr(feat_owner), _ptr(lay.d_dim),
+                _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(ids), _ptr(offsets), F, B, W, (lay.max_dim + 3) // 4 * 4,
+                _ptr(out), ld, _ptr(mirror), _ptr(feat_mirror_off), _ptr(psw), _ptr(feat_sel),
+                0 if feat_sel is None else feat_sel.numel(), _stream()), "tzk_peer_pooled_gather_fwd_weighted")
+            self.launches += 1
+            return out
         if feat_sel is not None:
             _need(feat_sel, torch.int32, "feat_sel")
             check(self._lib.tzk_peer_pooled_gather_fwd_sel(
@@ -602,8 +618,10 @@ class CudaKernels:
 
     def peer_bucketize(self, ids: torch.Tensor, offsets: torch.Tensor, F: int, B: int, W: int, feat_block: torch.Tensor,
                        feat_owner: torch.Tensor, feat_rows: torch.Tensor, rf_key_base: torch.Tensor, pooled: bool,
-                       cap: int, wire_key: torch.Tensor, wire_idx: torch.Tensor, counts: torch.Tensor) -> None:
-        """ids of the local batch -> this rank's own wire buffers (see tzk_peer_bucketize in include/tzk.h)."""
+                       cap: int, wire_key: torch.Tensor, wire_idx: torch.Tensor, counts: torch.Tensor,
+                       per_sample_weights: Optional[torch.Tensor] = None, wire_w: Optional[torch.Tensor] = None) -> None:
+        """ids of the local batch -> this rank's own wire buffers (see tzk_peer_bucketize in include/tzk.h).  Weighted
+        bags (pooled): `per_sample_weights` [nnz] and `wire_w` (local fp32 [W * cap]) receive every slot's weight."""
         _need(ids, torch.int64, "ids")
         _need(offsets, torch.int64, "offsets")
         _need(wire_key, torch.int64, "wire_key")
@@ -613,6 +631,21 @@ class CudaKernels:
             raise TzkError("peer_bucketize: wire buffers smaller than W * cap")
         nb = self._lib.tzk_peer_bucketize_workspace_bytes(F, B, W)
         ws = self._workspace(("peer_bkt", F, B, W), nb, ids.device)
+        psw = per_sample_weights
+        if psw is not None and ids.numel():      # (no ids: no slot is filled, so no weight is read)
+            _need(psw, torch.float32, "per_sample_weights")
+            if wire_w is None:
+                raise TzkError("peer_bucketize: weighted bags need wire_w")
+            _need(wire_w, torch.float32, "wire_w")
+            if not pooled or psw.numel() != ids.numel() or wire_w.numel() < W * cap:
+                raise TzkError("peer_bucketize: per-sample weights need the pooled layout, one weight per id and "
+                               "W * cap wire_w entries")
+            check(self._lib.tzk_peer_bucketize_weighted(
+                _ptr(ids), _ptr(offsets), F, B, W, _ptr(feat_block), _ptr(feat_owner), _ptr(feat_rows),
+                _ptr(rf_key_base), int(pooled), cap, _ptr(wire_key), _ptr(wire_idx), _ptr(counts), _ptr(ws), ws.numel(),
+                _ptr(psw), _ptr(wire_w), _stream()), "tzk_peer_bucketize_weighted")
+            self.launches += 3
+            return
         check(self._lib.tzk_peer_bucketize(_ptr(ids), _ptr(offsets), F, B, W, _ptr(feat_block), _ptr(feat_owner),
                                            _ptr(feat_rows), _ptr(rf_key_base), int(pooled), cap, _ptr(wire_key),
                                            _ptr(wire_idx), _ptr(counts), _ptr(ws), ws.numel(), _stream()),
@@ -632,11 +665,23 @@ class CudaKernels:
         self.launches += 1
 
     def peer_push_grad(self, recv, grad: torch.Tensor, lay: FeatureLayout, offsets: torch.Tensor, wire_idx: torch.Tensor,
-                       counts: torch.Tensor, me: int, W: int, cap: int, B: int, pooled: bool) -> None:
-        """This rank's gradient slices -> the owners' receive buffers, wire order (see tzk_peer_push_grad)."""
+                       counts: torch.Tensor, me: int, W: int, cap: int, B: int, pooled: bool,
+                       wire_w: Optional[torch.Tensor] = None) -> None:
+        """This rank's gradient slices -> the owners' receive buffers, wire order (see tzk_peer_push_grad).  `wire_w`
+        (weighted bags, pooled; filled by peer_bucketize): every slice is pushed as w * g (/ L)."""
         grad, ld = _rows2d(grad, "grad")
         _need(wire_idx, torch.int32, "wire_idx")
         _need(counts, torch.int32, "counts")
+        if wire_w is not None:
+            _need(wire_w, torch.float32, "wire_w")
+            if not pooled or wire_w.numel() < W * cap:
+                raise TzkError("peer_push_grad: wire_w needs the pooled layout and W * cap entries")
+            check(self._lib.tzk_peer_push_grad_weighted(
+                recv.ptrs, _ptr(grad), ld, _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(offsets), _ptr(wire_idx),
+                _ptr(counts), me, W, cap, B, lay.dim[0], int(pooled), _ptr(wire_w), _stream()),
+                "tzk_peer_push_grad_weighted")
+            self.launches += 1
+            return
         check(self._lib.tzk_peer_push_grad(recv.ptrs, _ptr(grad), ld, _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(offsets),
                                            _ptr(wire_idx), _ptr(counts), me, W, cap, B, lay.dim[0], int(pooled),
                                            _stream()), "tzk_peer_push_grad")

@@ -295,19 +295,41 @@ class PeerState(PeerBase):
             tabs=torch.from_numpy(tabs.view(np.uint8).copy()).to(dev) if rows else torch.zeros(8, dtype=torch.uint8, device=dev),
             psum=self._alloc(self.mirror.numel(), torch.float32), flags=self._alloc(max(k, 1), torch.int32), ws=None)
 
-    def _small_ws(self, nnz: int) -> torch.Tensor:
+    def _small_ws(self, nnz: int, weighted: bool = False) -> torch.Tensor:
         k = Fn.backend()
-        need = k.fused_bwd_workspace_bytes(self.small["layout"], max(nnz, self.max_nnz))
+        n = max(nnz, self.max_nnz)
+        # (weighted bags: the id half also leaves the bag of every id and the sorted weights in the workspace)
+        need = (k.fused_bwd_workspace_bytes(self.small["layout"], n, weighted=True) if weighted
+                else k.fused_bwd_workspace_bytes(self.small["layout"], n))
         ws = self.small["ws"]
         if ws is None or ws.numel() < need:
             ws = self.small["ws"] = torch.empty(max(need, 256), dtype=torch.uint8, device=self.device)
         return ws
 
+    # ---- weighted bags ---------------------------------------------------------------------------------------------
+    def _weights(self, psw: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+        """The per-sample weights this step uses: None for un-pooled collections (they ignore weights, like the nobag
+        TBE).  They never leave this rank: its gather pools w * row and its push sends w * g (/ L); the owners' update
+        is the unweighted one.  Host-side checks only (no device sync)."""
+        if psw is None or not self.pooled:
+            return None
+        if psw.requires_grad:
+            raise NotImplementedError("sharded EmbeddingBagCollection: per-sample weights that require grad (feature "
+                                      "processors) are not supported; the weights of a weighted id feature are data")
+        if self.bwd_mode != "push":
+            raise NotImplementedError("weighted id features on a sharded EmbeddingBagCollection need the push transport "
+                                      "of the peer exchange (TZK_PEER_BWD=push, the default): with pull the owners "
+                                      "would need every source's weights")
+        return psw
+
     # ---- forward ---------------------------------------------------------------------------------------------------
-    def gather(self, ids: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
+    def gather(self, ids: torch.Tensor, offsets: torch.Tensor, psw: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """psw: the local batch's per-sample weights (weighted bags) or None."""
         g, k = self.g, Fn.backend()
         if ids.numel() > self.max_nnz:
             raise RuntimeError(f"peer exchange is sized for {self.max_nnz} ids per step, got {ids.numel()}")
+        psw = self._weights(psw)
+        wkw = {} if psw is None else {"per_sample_weights": psw}
         sel = self._split_lists() if self.pooled else None
         if sel is not None:
             # two launches over complementary feature lists: the one whose rows cross NVLink starts first, on its own
@@ -319,7 +341,7 @@ class PeerState(PeerBase):
             def remote():
                 k.peer_pooled_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
                                          g.local.layout, ids, offsets, self.B, self.W, out, self.mirror,
-                                         self.feat_mirror_off, feat_sel=sel[1])
+                                         self.feat_mirror_off, feat_sel=sel[1], **wkw)
 
             if gs is not None:
                 gs.wait_stream(cur)
@@ -330,7 +352,7 @@ class PeerState(PeerBase):
             k.peer_mirror_refresh(self.tables, self.W, *self._seg, self.mirror)
             k.peer_pooled_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
                                      g.local.layout, ids, offsets, self.B, self.W, out, self.mirror, self.feat_mirror_off,
-                                     feat_sel=sel[0])
+                                     feat_sel=sel[0], **wkw)
             if gs is not None:
                 cur.wait_stream(gs)
             return out
@@ -339,7 +361,7 @@ class PeerState(PeerBase):
         if self.pooled:
             return k.peer_pooled_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
                                             g.local.layout, ids, offsets, self.B, self.W, None, self.mirror,
-                                            self.feat_mirror_off)
+                                            self.feat_mirror_off, **wkw)
         return k.peer_seq_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
                                      g.local.layout, ids, offsets, self.B, self.W, self.mirror, self.feat_mirror_off)
 
@@ -377,25 +399,39 @@ class PeerState(PeerBase):
             self._ws = torch.empty(max(need, 256), dtype=torch.uint8, device=self.device)
         return self._ws
 
-    def prep(self, ids: torch.Tensor, offsets: torch.Tensor) -> None:
-        """Id half of the backward (side stream): bucketize -> barrier A -> pull + sort at the owner."""
+    def prep(self, ids: torch.Tensor, offsets: torch.Tensor, psw: Optional[torch.Tensor] = None) -> None:
+        """Id half of the backward (side stream): bucketize -> barrier A -> pull + sort at the owner.  psw (weighted
+        bags): the bucketize also records every wire slot's weight in `wire_w` for this rank's push, and the small
+        tables' sort keeps the weights in sorted order."""
         g, k = self.g, Fn.backend()
+        psw = self._weights(psw)
+        wkw = {}
+        if psw is not None:
+            if getattr(self, "wire_w", None) is None:    # local memory (only this rank's push reads it): no collective
+                self.wire_w = torch.zeros(max(self.W * self.cap, 1), dtype=torch.float32, device=self.device)
+            wkw = {"per_sample_weights": psw, "wire_w": self.wire_w}
 
         def run():
             if self._prep_pending:            # a forward pass without a backward: peers may still be pulling
                 self._barrier(self.site_c)
             k.peer_bucketize(ids, offsets, g.F, self.B, self.W, self.feat_block_wire, g.feat_owner, self.feat_rows,
-                             self.rf_key_base, self.pooled, self.cap, self.wire_key.t, self.wire_idx.t, self.counts.t)
+                             self.rf_key_base, self.pooled, self.cap, self.wire_key.t, self.wire_idx.t, self.counts.t,
+                             **wkw)
             if self.small is not None:        # small tables: this rank's own ids, sorted by (table, row)
                 self.small["flags"].t.zero_()
-                k.fused_bwd_sort(self.pooled, self.small["layout"], ids, offsets, self.B, self._small_ws(ids.numel()))
+                if psw is not None:
+                    k.fused_bwd_sort(self.pooled, self.small["layout"], ids, offsets, self.B,
+                                     self._small_ws(ids.numel(), weighted=True), per_sample_weights=psw)
+                else:
+                    k.fused_bwd_sort(self.pooled, self.small["layout"], ids, offsets, self.B,
+                                     self._small_ws(ids.numel()))
             self._barrier(self.site_a)
             k.fused_bwd_sort_peer(self.wire_key, self.wire_idx, self.counts, self.me, self.W, self.cap,
                                   0 if self.bwd_mode == "push" else self.idx_span, g.local.layout, g.overflow,
                                   self._workspace())
             self._prep_pending = True
 
-        self._keep = (ids, offsets)           # the side stream reads them: keep them away from the allocator
+        self._keep = (ids, offsets, psw)      # the side stream reads them: keep them away from the allocator
         self._on_side(run)
 
     # ---- backward --------------------------------------------------------------------------------------------------
@@ -414,13 +450,18 @@ class PeerState(PeerBase):
         # main stream only pushes the big tables' rows and crosses barrier B.
         accum_side = (sm is not None and push and os.environ.get("TZK_PEER_ACCUM_SIDE", "1") != "0"
                       and self._side_stream() is not None)
+        psw = self._keep[2] if self._keep is not None else None    # this step's weights (prep), or None
 
         def accumulate_small():
             from .kernels import OPT_ACCUM_OUT
 
             gr = grad if self.pooled else grad.reshape(-1, g.dim)
             nnz = int(self._keep[0].numel()) if self._keep is not None else 0
-            if nnz:
+            if nnz and psw is not None:     # weighted bags: each entry scaled by (1/W / L) * w before the per-row sums
+                k.fused_bwd_apply(OPT_ACCUM_OUT, self.pooled, gr, sm["psum"].t, sm["flags"].t, sm["layout"], offsets, nnz,
+                                  self.B, 0.0, 0.0, 1.0 / self.W, self._small_ws(nnz, weighted=True),
+                                  per_sample_weights=psw)
+            elif nnz:
                 k.fused_bwd_apply(OPT_ACCUM_OUT, self.pooled, gr, sm["psum"].t, sm["flags"].t, sm["layout"], offsets, nnz,
                                   self.B, 0.0, 0.0, 1.0 / self.W, self._small_ws(nnz))
 
@@ -431,12 +472,17 @@ class PeerState(PeerBase):
                 accumulate_small()
                 self._barrier(self.site_b2)   # every rank's partial sums are complete
             self._on_side(side_accum)         # (forks after everything enqueued so far: the gradient exists)
-            self._pending_accum = (grad, offsets)   # the side stream reads them: away from the allocator until the join
+            # the side stream reads them: away from the allocator until the join
+            self._pending_accum = (grad, offsets, psw)
         if push:
             if not self.pooled:
                 grad = grad.reshape(-1, g.dim)
-            k.peer_push_grad(self.recv, grad, lay, offsets, self.wire_idx.t, self.counts.t, self.me, self.W, self.cap,
-                             self.B, self.pooled)
+            if psw is not None:               # pushed rows are w * g (/ L); wire_w was filled by this step's prep
+                k.peer_push_grad(self.recv, grad, lay, offsets, self.wire_idx.t, self.counts.t, self.me, self.W,
+                                 self.cap, self.B, self.pooled, wire_w=self.wire_w)
+            else:
+                k.peer_push_grad(self.recv, grad, lay, offsets, self.wire_idx.t, self.counts.t, self.me, self.W,
+                                 self.cap, self.B, self.pooled)
         elif self.pooled:
             ld = g.total_dim
             k.peer_publish_grad(grad, lay, offsets, self.B, self.grad.t.view(self.B, ld))
@@ -497,12 +543,14 @@ PeerState.join_pending = _peer_join_pending
 
 
 class _PeerLookup(torch.autograd.Function):
+    """psw: the KJT's per-sample weights (weighted bags) or None; data, no gradient flows to them."""
+
     @staticmethod
-    def forward(ctx, hook, st: PeerState, ids, offsets):
-        out = st.gather(ids, offsets)
+    def forward(ctx, hook, st: PeerState, ids, offsets, psw=None):
+        out = st.gather(ids, offsets, psw)
         ctx.st = None
         if hook is not None:                  # (also with zero local ids: the barriers are collective)
-            st.prep(ids, offsets)
+            st.prep(ids, offsets, psw)
             ctx.st = st
             ctx.save_for_backward(offsets)
         return out
@@ -512,7 +560,7 @@ class _PeerLookup(torch.autograd.Function):
         if ctx.st is not None:
             (offsets,) = ctx.saved_tensors
             ctx.st.backward(Fn._rows_contig(grad_out) if ctx.st.pooled else grad_out.contiguous(), offsets)
-        return None, None, None, None
+        return None, None, None, None, None
 
 
 def enable_peer_exchange(sm, batch_size: int, ids_per_feature: Optional[Dict[str, int]] = None) -> List[PeerState]:
@@ -527,18 +575,21 @@ def enable_peer_exchange(sm, batch_size: int, ids_per_feature: Optional[Dict[str
             per_f = [int(ids_per_feature.get(name, batch_size)) for name in g.feature_names]
         states.append(PeerState(g, sm.plan, grp, batch_size, per_f))
     pooled = sm._pooled
-    from .distributed import reject_weighted
 
     def forward(features):
-        if pooled:
-            reject_weighted(features)
+        # weighted id features: each rank's weights stay with its samples (pooled collections, push transport; the
+        # checks are host-side, before any launch)
+        psw = features.weights_or_none() if pooled else None
+        if psw is not None and states:
+            states[0]._weights(psw)
         keys, lens, vals = [], [], []
         out = {}
         for g, st in zip(sm.groups, states):
             kjt = g.local._select(features)
             if kjt.stride() != st.B:
                 raise RuntimeError(f"peer exchange was sized for batch {st.B}, got {kjt.stride()}")
-            res = _PeerLookup.apply(sm._hook_tensor(kjt.values().device), st, kjt.values(), kjt.offsets())
+            res = _PeerLookup.apply(sm._hook_tensor(kjt.values().device), st, kjt.values(), kjt.offsets(),
+                                    kjt.weights_or_none() if pooled else None)
             if pooled:
                 vals.append(res)
                 keys += g.embedding_names
