@@ -493,6 +493,22 @@ int tzk_peer_push_grad_weighted(const uint64_t* recv_ptrs, const float* grad, in
                                 const int32_t* counts, int32_t me, int32_t W, int64_t cap, int32_t B, int32_t D,
                                 int32_t pooled, const float* wire_w, tzk_stream_t stream);
 
+/* ---- DLRM-Criteo interaction in BF16 (train_config.mixed_precision "BF16"; csrc/tzk_interact_bf16.cuh).  bf16 values
+ * cross the ABI as their 16-bit patterns.  N = 27 rows of 16 (dense + 26 sparse features); the row
+ * X = [351 pairs | 0 | 16 dense | 416 sparse] is 784 bf16, the reference's 783 columns with one zero after the pairs.
+ *   fwd_bf16: pairs = bf16_rn(F F^T) (products exact, fp32 accumulation, mma.sync m16n8k16) over F = [dense ; bf16_rn(sparse)];
+ *             the copied columns are dense as it is and bf16_rn(sparse).
+ *   bwd_bf16: from dX (bf16), with G the pair gradient in the upper triangle and g1 = bf16_rn(G F), g2 = bf16_rn(G^T F),
+ *             s = fp32(g1 + g2): d_dense = bf16_rn(bf16_rn(s) + dX_dense), d_sparse = s + dX_sparse (fp32) — autograd's
+ *             rounding points under torch.autocast(dtype=torch.bfloat16).
+ * Rows: dense / d_dense 8-B aligned with ld a multiple of 4, sparse / d_sparse 16-B aligned with ld a multiple of 4,
+ * X / dX 16-B aligned with ld a multiple of 8; anything else is rejected. */
+int tzk_dot_interact27_fwd_bf16(const uint16_t* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t B,
+                                uint16_t* out, int64_t ld_out, tzk_stream_t stream);
+int tzk_dot_interact27_bwd_bf16(const uint16_t* d_out, int64_t ld_dout, const uint16_t* dense, int64_t ld_dense,
+                                const float* sparse, int64_t ld_sparse, int64_t B, uint16_t* d_dense, int64_t ld_ddense,
+                                float* d_sparse, int64_t ld_dsparse, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

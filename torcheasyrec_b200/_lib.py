@@ -143,6 +143,9 @@ SIGNATURES = {
         c_int32, [P, P, c_int32, c_int32, c_int32, P, P, P, P, c_int32, c_int64, P, P, P, P, c_size_t, P, P, P]),
     "tzk_peer_push_grad_weighted": (
         c_int32, [P, P, c_int64, P, P, P, P, P, c_int32, c_int32, c_int64, c_int32, c_int32, c_int32, P, P]),
+    "tzk_dot_interact27_fwd_bf16": (c_int32, [P, c_int64, P, c_int64, c_int64, P, c_int64, P]),
+    "tzk_dot_interact27_bwd_bf16": (
+        c_int32, [P, c_int64, P, c_int64, P, c_int64, c_int64, P, c_int64, P, c_int64, P]),
 }
 
 _lib = None

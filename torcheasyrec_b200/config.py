@@ -74,8 +74,10 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
         "is_profiling": _f(B, False), "use_tensorboard": _f(B, True), "cudnn_allow_tf32": _f(B, True),
         "cuda_matmul_allow_tf32": _f(B, False), "global_embedding_constraints": _f("ParameterConstraints"),
         "mixed_precision": _f(S), "gradient_accumulation_steps": _f(I), "fine_tune_checkpoint": _f(S),
-        "tensorboard_summaries": _f(S, rep=True),
+        "tensorboard_summaries": _f(S, rep=True), "grad_scaler": _f("GradScaler"),
     },
+    "GradScaler": {"init_scale": _f(F, 65536.0), "growth_factor": _f(F, 2.0), "backoff_factor": _f(F, 0.5),
+                   "growth_interval": _f(I, 2000)},
     "EvalConfig": {"num_steps": _f(I), "log_step_count_steps": _f(I, 100)},
     "SparseOptimizer": {
         "sgd_optimizer": _f("FusedSGDOptimizer"), "adagrad_optimizer": _f("FusedAdagradOptimizer"),

@@ -8,8 +8,10 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["tzk_core.cu", "tzk_gather.cu", "tzk_bwd.cu", "tzk_dist.cu", "tzk_dense.cu", "tzk_tower.cu", "tzk_din.cu", "tzk_peer.cu", "tzk_interact_wide.cu"]
-HEADERS = ["tzk_common.cuh", "tzk_tower_bwd2.cuh", "tzk_interact_tc.cuh", "tzk_tower_tail.cuh", "tzk_sm90_ptx.h", "tzk_tma.h", os.path.join("..", "..", "include", "tzk.h")]
+SOURCES = ["tzk_core.cu", "tzk_gather.cu", "tzk_bwd.cu", "tzk_dist.cu", "tzk_dense.cu", "tzk_tower.cu", "tzk_din.cu", "tzk_peer.cu", "tzk_interact_wide.cu",
+           "tzk_interact_bf16.cu"]
+HEADERS = ["tzk_common.cuh", "tzk_tower_bwd2.cuh", "tzk_interact_tc.cuh", "tzk_tower_tail.cuh", "tzk_interact_bf16.cuh",
+"tzk_sm90_ptx.h", "tzk_tma.h", os.path.join("..", "..", "include", "tzk.h")]
 LIB = os.path.join(HERE, "libtzk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [

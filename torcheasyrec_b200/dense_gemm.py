@@ -6,6 +6,11 @@ algorithm: same fp32 inputs/outputs, fp32-equivalent accuracy.  cuBLASLt (>= 12.
 fp32 compute type and for plain fp32 when it offers no algorithm for that; which kernels it runs is its choice per GPU.
 Falls back to torch.nn.functional.linear whenever the library or the device is unavailable (set TZK_DENSE_GEMM=torch to force
 the fallback).
+
+Under torch.autocast (train_config.mixed_precision) the fp32 GEMM kernels step aside: `linear` is autocast's own F.linear
+(lower-precision list), the fused interaction + wide layer and the fused tower tail give way to the layer-by-layer torch
+chain, and the BCE kernel stays (autocast runs BCE-with-logits in fp32).  DLRM-Criteo's interaction under bf16 autocast
+has a kernel of its own, InteractBf16Fn.
 """
 
 import ctypes
@@ -14,6 +19,8 @@ from typing import Optional
 
 import torch
 from torch import nn
+
+from .functional import autocast_dtype
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "csrc", "libtzk_gemm.so")
@@ -83,7 +90,8 @@ class _LinearFn(torch.autograd.Function):
     bias+ReLU and ReLU-backward+bias-gradient are one tzk kernel each instead of four ATen passes.
     `x` may carry zero columns beyond W's in_features (width rounded up to a multiple of 4 by the producer):
     16-B aligned rows are what lets cuBLASLt pick the tensor-core kernels instead of the align1 SIMT ones —
-    e.g. DLRM's 783-wide final-MLP input travels as [B, 784]."""
+    e.g. DLRM's 783-wide final-MLP input travels as [B, 784].  fp32 only: under autocast `linear` runs autocast's
+    F.linear instead."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, relu, in_map):
@@ -135,7 +143,8 @@ class _LinearFn(torch.autograd.Function):
 
 class _SmallLinearFn(torch.autograd.Function):
     """y = act(x @ W^T + b) for K, N <= 64: one tzk launch forward, one (+ partial reduction) backward
-    (csrc/tzk_tower.cu) instead of the 4-10 library launches such a layer costs as GEMM + element-wise passes."""
+    (csrc/tzk_tower.cu) instead of the 4-10 library launches such a layer costs as GEMM + element-wise passes.
+    fp32 only: under autocast `linear` runs autocast's F.linear instead."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, relu):
@@ -223,7 +232,8 @@ def wgrad3x(lib, x, dz, slabs=SLABS):
 
 
 class Gemm3xLinearFn(torch.autograd.Function):
-    """Same contract as dense_gemm._LinearFn.apply(x, weight, bias, relu, in_map) with `lib` in front."""
+    """Same contract as dense_gemm._LinearFn.apply(x, weight, bias, relu, in_map) with `lib` in front.  fp32 only: under
+    autocast `linear` runs autocast's F.linear instead."""
 
     @staticmethod
     def forward(ctx, lib, x, weight, bias, relu, in_map):
@@ -272,7 +282,8 @@ class InteractWideFn(torch.autograd.Function):
     """relu(X @ W^T + b) with X = functional.dlrm_interaction(dense, sparse, 26, 16, aligned=True), the first layer of
     DLRM-Criteo's final MLP.  The forward is the interaction kernel followed by gemm3x; the backward computes the
     interaction's input gradients in one kernel from dZ and W (tzk_interact_wide_bwd) instead of writing X's gradient
-    [M, 784] to memory and reading it back, and the weight gradient with wgrad3x from the saved X."""
+    [M, 784] to memory and reading it back, and the weight gradient with wgrad3x from the saved X.  fp32 only: under
+    autocast interact_wide_usable() is False and the layer runs as autocast's F.linear."""
 
     @staticmethod
     def forward(ctx, lib, dense, sparse, weight, bias, in_map):
@@ -306,12 +317,52 @@ class InteractWideFn(torch.autograd.Function):
                 None)
 
 
+class InteractBf16Fn(torch.autograd.Function):
+    """X [B, 784] bf16 = [351 pairs | 0 | dense | bf16(sparse)], DLRM-Criteo's interaction under bf16 autocast
+    (csrc/tzk_interact_bf16.cuh), from the bottom MLP's bf16 output [B, 16] and the pooled embeddings [B, 416] fp32.  The
+    rounding points are those of dlrm.py:113-131 under autocast: bf16 pairs from fp32 accumulation, bf16 copies, and in
+    the backward d_dense in bf16 and d_sparse in fp32 (include/tzk.h).  The first final-MLP layer consumes X as autocast's
+    F.linear with the weight spread by IN_MAP."""
+
+    IN_MAP = ((0, 0, 351), (351, 352, 432))
+
+    @staticmethod
+    def forward(ctx, dense, sparse):
+        from .kernels import default_kernels
+
+        ctx.save_for_backward(dense, sparse)
+        return default_kernels().dot_interact27_fwd_bf16(dense, sparse)
+
+    @staticmethod
+    def backward(ctx, dx):
+        from .kernels import default_kernels
+
+        dense, sparse = ctx.saved_tensors
+        if not (dx.stride(1) == 1 and dx.stride(0) % 8 == 0 and dx.data_ptr() % 16 == 0):
+            dx = dx.contiguous()
+        d_dense, d_sparse = default_kernels().dot_interact27_bwd_bf16(dx, dense, sparse)
+        return (d_dense if ctx.needs_input_grad[0] else None), (d_sparse if ctx.needs_input_grad[1] else None)
+
+
+def interact_bf16_usable(dense: Optional[torch.Tensor], sparse: torch.Tensor, num_sparse: int, dim: int) -> bool:
+    """Whether InteractBf16Fn covers this interaction: bf16 autocast on CUDA, DLRM-Criteo's shape (26 sparse features of
+    16 plus a bf16 bottom-MLP output [B, 16]), rows aligned for the kernel's vector loads.  TZK_INTERACT_BF16=0 selects
+    the torch formulation instead."""
+    return (dense is not None and sparse.is_cuda and autocast_dtype(sparse) == torch.bfloat16 and num_sparse == 26
+            and dim == 16 and dense.dtype == torch.bfloat16 and sparse.dtype == torch.float32 and dense.dim() == 2
+            and sparse.dim() == 2 and tuple(dense.shape[1:]) == (16,) and tuple(sparse.shape[1:]) == (416,)
+            and dense.shape[0] == sparse.shape[0] >= 1
+            and dense.stride(1) == 1 and dense.stride(0) % 4 == 0 and dense.data_ptr() % 8 == 0
+            and sparse.stride(1) == 1 and sparse.stride(0) % 4 == 0 and sparse.data_ptr() % 16 == 0
+            and os.environ.get("TZK_INTERACT_BF16", "1") != "0")
+
+
 def interact_wide_usable(dense: Optional[torch.Tensor], sparse: torch.Tensor, weight: torch.Tensor,
                          num_sparse: int, dim: int) -> bool:
     """Whether InteractWideFn covers this layer: DLRM-Criteo's shape (26 sparse features of 16 plus the bottom-MLP
     output, all copied into the row), fp32 CUDA tensors, a 783 -> 64 weight, and the kernels the layer-by-layer path
-    would run (gemm3x for the layer, the tensor-core interaction)."""
-    return (dense is not None and num_sparse == 26 and dim == 16 and dense.is_cuda and dense.dtype == torch.float32
+    would run (gemm3x for the layer, the tensor-core interaction), and autocast off."""
+    return (dense is not None and autocast_dtype(sparse) is None and num_sparse == 26 and dim == 16 and dense.is_cuda and dense.dtype == torch.float32
             and sparse.dtype == torch.float32 and dense.dim() == 2 and tuple(dense.shape[1:]) == (16,)
             and sparse.dim() == 2 and tuple(sparse.shape[1:]) == (416,) and dense.shape[0] == sparse.shape[0] >= 256
             and all(t.stride(1) == 1 and t.stride(0) % 4 == 0 and t.data_ptr() % 16 == 0 for t in (dense, sparse))
@@ -338,7 +389,8 @@ def _small(x: torch.Tensor, weight: torch.Tensor) -> bool:
 
 
 class _BceFn(torch.autograd.Function):
-    """mean BCE-with-logits; the forward kernel also writes dloss/dlogits, backward only scales it."""
+    """mean BCE-with-logits; the forward kernel also writes dloss/dlogits, backward only scales it.  Kept under autocast:
+    binary_cross_entropy_with_logits is on autocast's fp32 list, so bce_with_logits() hands it fp32 logits."""
 
     @staticmethod
     def forward(ctx, logits, labels):
@@ -356,7 +408,8 @@ class _BceFn(torch.autograd.Function):
 
 
 class _TowerTailFn(torch.autograd.Function):
-    """(loss, logits) = BCE(Linear(relu(Linear(y1)))) with every gradient computed in the forward kernel."""
+    """(loss, logits) = BCE(Linear(relu(Linear(y1)))) with every gradient computed in the forward kernel.  fp32 only:
+    under autocast tower_tail_usable() is False and the two layers run as autocast's F.linear."""
 
     @staticmethod
     def forward(ctx, y1, w1, b1, w2, b2, labels):
@@ -377,8 +430,9 @@ class _TowerTailFn(torch.autograd.Function):
 
 
 def tower_tail_usable(y1: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, labels: torch.Tensor) -> bool:
-    """The fused tail covers fp32 CUDA towers ending K -> N (ReLU) -> 1 with K, N <= 64 and a float label per row."""
-    return (y1.is_cuda and y1.dim() == 2 and y1.dtype == torch.float32 and w1.dtype == torch.float32
+    """The fused tail covers fp32 CUDA towers ending K -> N (ReLU) -> 1 with K, N <= 64 and a float label per row, with
+    autocast off."""
+    return (autocast_dtype(y1) is None and y1.is_cuda and y1.dim() == 2 and y1.dtype == torch.float32 and w1.dtype == torch.float32
             and w1.shape[1] == y1.shape[1] <= 64 and w1.shape[0] <= 64 and tuple(w2.shape) == (1, w1.shape[0])
             and labels.dtype == torch.float32 and labels.numel() == y1.shape[0] >= 1 and y1.stride(1) == 1)
 
@@ -389,11 +443,29 @@ def tower_tail_bce(y1, w1, b1, w2, b2, labels):
 
 
 def bce_with_logits(logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
-    """F.binary_cross_entropy_with_logits(logits, labels) (mean); fused fwd+bwd kernel on CUDA fp32 inputs."""
+    """F.binary_cross_entropy_with_logits(logits, labels) (mean); fused fwd+bwd kernel on CUDA fp32 inputs.  Under
+    autocast the logits are cast to fp32 first, as autocast's fp32 list does for this op."""
+    if autocast_dtype(logits) is not None:
+        logits, labels = logits.float(), labels.float()
     if (logits.is_cuda and logits.dtype == torch.float32 and labels.dtype == torch.float32 and logits.numel() >= 1
             and os.environ.get("TZK_SMALL_LINEAR", "1") != "0"):
         return _BceFn.apply(logits, labels)
     return torch.nn.functional.binary_cross_entropy_with_logits(logits, labels)
+
+
+def _spread_weight(weight: torch.Tensor, width: int, in_map) -> torch.Tensor:
+    """[N, K] -> [N, width]: column src of `weight` at column dst for every (src, dst, n) of `in_map` (default: the K
+    columns first), zeros elsewhere; differentiable, so the gradient reaches `weight`."""
+    N, K = weight.shape
+    cols, c = [], 0
+    for (src, dst, n) in (in_map or ((0, 0, K),)):
+        if dst > c:
+            cols.append(weight.new_zeros((N, dst - c)))
+        cols.append(weight[:, src:src + n])
+        c = dst + n
+    if width > c:
+        cols.append(weight.new_zeros((N, width - c)))
+    return torch.cat(cols, dim=1)
 
 
 def padded_width(n: int) -> int:
@@ -410,8 +482,19 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], 
            in_map=None) -> torch.Tensor:
     """act(F.linear(x, weight, bias)).  `x` may be wider than in_features: zero-padded at the end (width =
     padded_width(in_features)) or, with `in_map` = ((src_col, dst_col, n), ...), with zero columns in between —
-    column src of the weight multiplies column dst of x."""
+    column src of the weight multiplies column dst of x.
+
+    Under autocast this is autocast's own F.linear (lower-precision list: inputs and weight cast, fp32 accumulation);
+    a wider `x` meets the weight spread to its columns through differentiable ops, so the zero columns contribute
+    nothing and the weight gradient is the reference's."""
     K = weight.shape[1]
+    if autocast_dtype(x) is not None:
+        if x.dim() == 2 and (x.shape[1] != K or in_map is not None):
+            if in_map is None and x.shape[1] != padded_width(K):
+                raise RuntimeError(f"linear: input width {x.shape[1]} does not match in_features {K}")
+            weight = _spread_weight(weight, x.shape[1], in_map)
+        y = torch.nn.functional.linear(x, weight, bias)
+        return torch.relu(y) if relu else y
     if in_map is None and _small(x, weight):
         return _SmallLinearFn.apply(x, weight, bias, relu)
     if x.dim() == 2 and (x.shape[1] != K or in_map is not None):

@@ -17,7 +17,7 @@ from .batch import Batch, synthetic_batch
 from .config import Message, edit_config, load_pipeline_config
 from .features import BaseFeature, create_features
 from .rank_models import (RankModel, TrainWrapper, create_model, dense_optimizer_from_config,
-                          sparse_optimizer_from_config)
+                          mixed_precision_to_dtype, sparse_optimizer_from_config)
 from .sparse import KeyedJaggedTensor, KeyedTensor
 
 
@@ -91,7 +91,12 @@ class Pipeline:
         if self.device.type == "cuda" and capturable:
             kw = dict(capturable=True, fused=True)
         self.dense_optimizer = dense_optimizer_from_config(self.cfg.train_config, self.model.dense_parameters(), **kw)
-        self.train_wrapper = TrainWrapper(self.model)
+        tc = self.cfg.train_config
+        self.mixed_dtype = mixed_precision_to_dtype(tc.mixed_precision)
+        if self.mixed_dtype is not None and tc.HasField("grad_scaler"):
+            raise NotImplementedError("train_config.grad_scaler: loss scaling over the fused sparse update is not "
+                                      "implemented (mixed_precision without grad_scaler is)")
+        self.train_wrapper = TrainWrapper(self.model, self.mixed_dtype, self.device.type)
         torch.backends.cuda.matmul.allow_tf32 = bool(self.cfg.train_config.cuda_matmul_allow_tf32)
 
     def _table_constraints(self) -> Dict[str, List[str]]:

@@ -31,6 +31,18 @@ def use_backend(b):
         _backend = prev
 
 
+def autocast_dtype(t: torch.Tensor) -> Optional[torch.dtype]:
+    """The dtype torch.autocast casts to on `t`'s device type, or None when autocast is off there.
+
+    Autocast never sees a custom autograd.Function, so every hand-written dense path asks this first.  Under autocast a
+    path either keeps its fp32 kernel, where autocast itself would run that op in fp32 on the same inputs, or steps
+    aside to the reference's torch formulation, which autocast then applies to (train_config.mixed_precision)."""
+    dt = t.device.type
+    if dt in ("cuda", "cpu") and torch.is_autocast_enabled(dt):
+        return torch.get_autocast_dtype(dt)
+    return None
+
+
 def _rows_contig(t: torch.Tensor) -> torch.Tensor:
     if t.dim() == 2 and (t.shape[1] <= 1 or t.stride(1) == 1) and (t.shape[0] <= 1 or t.stride(0) >= t.shape[1]):
         return t
@@ -207,7 +219,14 @@ class _FM(torch.autograd.Function):
 
 
 def factorization_machine(feature: torch.Tensor) -> torch.Tensor:
-    """[B, N, D] -> [B, D]  (tzrec/modules/fm.py:28-42)."""
+    """[B, N, D] -> [B, D]  (tzrec/modules/fm.py:28-42).
+
+    Under autocast an fp32 input keeps the kernel: sum and mul are on no lower-precision list (CUDA autocast runs sum in
+    fp32, CPU autocast leaves both alone), so autocast computes the reference in fp32 too.  Any other input dtype takes
+    the reference's torch formulation."""
+    if autocast_dtype(feature) is not None and feature.dtype != torch.float32:
+        s = torch.sum(feature, dim=1)
+        return 0.5 * (s * s - torch.sum(feature * feature, dim=1))
     B, N, D = feature.shape
     return _FM.apply(_rows_contig(feature.reshape(B, N * D)), N, D)
 
@@ -230,8 +249,26 @@ class _DotInteract(torch.autograd.Function):
         return d_dense, d_sparse, None, None, None, None, None, None
 
 
+_triu_cache = {}
+
+
+def _torch_dot_interaction(features: torch.Tensor) -> torch.Tensor:
+    """tzrec/modules/interaction.py:80-91 as stated there: bmm, then the strict upper triangle, row-major."""
+    N = features.shape[1]
+    key = (N, str(features.device))
+    iu = _triu_cache.get(key)
+    if iu is None:      # cached: no index build inside a captured step
+        iu = _triu_cache[key] = torch.triu_indices(N, N, offset=1, device=features.device)
+    z = torch.bmm(features, torch.transpose(features, 1, 2))
+    return z[:, iu[0], iu[1]]
+
+
 def dot_interaction(features: torch.Tensor) -> torch.Tensor:
-    """InteractionArch.forward (tzrec/modules/interaction.py:80-91): [B,N,D] -> [B, N(N-1)/2]."""
+    """InteractionArch.forward (tzrec/modules/interaction.py:80-91): [B,N,D] -> [B, N(N-1)/2].
+
+    Under autocast this is the reference's torch formulation: bmm is on autocast's lower-precision list."""
+    if autocast_dtype(features) is not None:
+        return _torch_dot_interaction(features)
     B, N, D = features.shape
     return _DotInteract.apply(None, features.reshape(B, N * D), N, D, False, False)
 
@@ -244,7 +281,22 @@ def dlrm_interaction(dense_feat: Optional[torch.Tensor], sparse_feat: torch.Tens
     aligned=False -> the reference's exact column layout [P | dense | sparse].
     aligned=True  -> (tensor, in_map): zero columns are inserted after the P interaction terms and at the row end so
     that every block and every row starts on a 16-B boundary; `in_map` = [(src_col, dst_col, length), ...] tells the
-    consuming Linear where the reference's columns live (dense_gemm.linear pads its weight accordingly)."""
+    consuming Linear where the reference's columns live (dense_gemm.linear pads its weight accordingly).
+
+    Under autocast this is the reference's torch formulation in the reference's layout (with aligned=True the map is
+    None): autocast rounds the bmm to its dtype and the concatenations promote back to fp32, as in dlrm.py.  DLRM-Criteo
+    under bf16 autocast has its own kernel (dense_gemm.InteractBf16Fn)."""
+    if autocast_dtype(sparse_feat) is not None:
+        B = sparse_feat.shape[0]
+        feat = sparse_feat.reshape(-1, num_sparse, dim)
+        if dense_feat is not None:
+            feat = torch.cat([dense_feat.unsqueeze(1), feat], dim=1)
+        x = _torch_dot_interaction(feat)
+        if with_dense and dense_feat is not None:
+            x = torch.cat([x, dense_feat], dim=-1)
+        if with_sparse:
+            x = torch.cat([x, sparse_feat.reshape(B, -1)], dim=-1)
+        return (x, None) if aligned else x
     if not aligned:
         return _DotInteract.apply(dense_feat, sparse_feat, num_sparse, dim, with_dense, with_sparse, 1, 0)
     n = num_sparse + (dense_feat is not None)
@@ -286,14 +338,52 @@ class _JaggedSoftmaxWsum(torch.autograd.Function):
         return d_s, d_k, None, None
 
 
+def _segments(offsets: torch.Tensor, n: int) -> torch.Tensor:
+    """Sample index of each of the n jagged rows."""
+    B = offsets.numel() - 1
+    return torch.repeat_interleave(torch.arange(B, device=offsets.device), offsets[1:] - offsets[:-1], output_size=n)
+
+
 def din_attn_input(query: torch.Tensor, seq: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
     """[N, 4*Ds] input of DIN's attention MLP for jagged sequence rows: [q | k | q - k | q * k]
-    (tzrec/modules/sequence.py:113-116 without the padded [B, T, Ds] broadcast)."""
+    (tzrec/modules/sequence.py:113-116 without the padded [B, T, Ds] broadcast).
+
+    Under autocast fp32 inputs keep the kernel: pad, cat, sub and mul are on no lower-precision list, so autocast
+    computes the reference in fp32 as the kernel does.  Other input dtypes take the torch formulation over the jagged
+    rows."""
+    if autocast_dtype(seq) is not None and (query.dtype != torch.float32 or seq.dtype != torch.float32):
+        q = torch.nn.functional.pad(query, (0, seq.shape[1] - query.shape[1]))[_segments(offsets, seq.shape[0])]
+        return torch.cat([q, seq, q - seq, q * seq], dim=-1)
     return _DinAttnInput.apply(query, seq, offsets)
+
+
+def _torch_jagged_softmax_wsum(scores, seq, offsets, max_len: int, dtype) -> torch.Tensor:
+    """tzrec/modules/sequence.py:124-128 under autocast, over jagged rows: softmax in fp32 (CUDA autocast's softmax is on
+    its fp32 list; a CPU bf16 softmax also accumulates in fp32 and rounds once), then matmul on the lower-precision list:
+    bf16 probabilities times bf16 rows, fp32 accumulation, one rounding of the result.  Padded positions of the
+    reference carry probability exactly 0, so leaving them out changes only the summation order."""
+    N, B = seq.shape[0], offsets.numel() - 1
+    seg = _segments(offsets, N)
+    s = scores.float()
+    if max_len > 0:
+        pos = torch.arange(N, device=seq.device) - offsets[:-1][seg]
+        s = s.masked_fill(pos >= max_len, float("-inf"))
+    m = torch.full((B,), float("-inf"), device=seq.device).scatter_reduce(0, seg, s.detach(), "amax")
+    e = torch.exp(s - m[seg])
+    z = torch.zeros(B, device=seq.device).index_add(0, seg, e)
+    p = (e / z[seg]).to(dtype)
+    out = torch.zeros((B, seq.shape[1]), device=seq.device).index_add(0, seg, p.float()[:, None] * seq.to(dtype).float())
+    return out.to(dtype)
 
 
 def jagged_softmax_weighted_sum(scores: torch.Tensor, seq: torch.Tensor, offsets: torch.Tensor,
                                 max_len: int = 0) -> torch.Tensor:
     """[B, Ds]: per sample softmax over its (first max_len) scores, then the weighted sum of its rows
-    (tzrec/modules/sequence.py:118-128; a sample without rows gives zeros like the masked padded version)."""
+    (tzrec/modules/sequence.py:118-128; a sample without rows gives zeros like the masked padded version).
+
+    Under autocast the weighted sum is a lower-precision matmul in the reference, so this takes the torch formulation
+    (_torch_jagged_softmax_wsum) instead of the fp32 kernel."""
+    dt = autocast_dtype(seq)
+    if dt is not None:
+        return _torch_jagged_softmax_wsum(scores, seq, offsets, int(max_len), dt)
     return _JaggedSoftmaxWsum.apply(scores, seq, offsets, int(max_len))

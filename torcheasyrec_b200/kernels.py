@@ -141,6 +141,17 @@ def _rows2d(t: torch.Tensor, name: str) -> Tuple[torch.Tensor, int]:
     return t, ld
 
 
+def _rows2d_dtype(t: torch.Tensor, dtype, name: str) -> Tuple[torch.Tensor, int]:
+    """_rows2d for another element type (the bf16 interaction's operands)."""
+    if not t.is_cuda:
+        raise TzkError(f"{name}: expected a CUDA tensor (no CPU fallback)")
+    if t.dtype != dtype or t.dim() != 2:
+        raise TzkError(f"{name}: expected a 2-D {dtype} tensor")
+    if t.shape[1] > 1 and t.stride(1) != 1:
+        raise TzkError(f"{name}: rows must be contiguous")
+    return t, (t.stride(0) if t.shape[0] > 1 else max(t.shape[1], 1))
+
+
 def _unvalidated_switch(name: str) -> bool:
     """Mirrors unvalidated_switch() of csrc/tzk_common.cuh: `name`=0/1 decides, else TZK_EXPERIMENTAL=1 turns it on."""
     e = os.environ.get(name, "")
@@ -824,6 +835,38 @@ class CudaKernels:
         check(self._lib.tzk_dot_interact_bwd(_ptr(dense), ld_d, _ptr(sparse), ld_s, _ptr(d_out), ld_o, B, Ns, D,
                                              int(copy_dense), int(copy_sparse), p_pad, _ptr(d_dense), D,
                                              _ptr(d_sparse), Ns * D, _stream()), "tzk_dot_interact_bwd")
+        self.launches += 1
+        return d_dense, d_sparse
+
+    def dot_interact27_fwd_bf16(self, dense: torch.Tensor, sparse: torch.Tensor) -> torch.Tensor:
+        """X [B, 784] bf16 = [351 pairs | 0 | dense | bf16(sparse)] of DLRM-Criteo's interaction under bf16 autocast, from
+        dense [B, 16] bf16 and sparse [B, 416] fp32 (tzk_dot_interact27_fwd_bf16)."""
+        dense, ld_d = _rows2d_dtype(dense, torch.bfloat16, "dense")
+        sparse, ld_s = _rows2d(sparse, "sparse")
+        B = sparse.shape[0]
+        if tuple(dense.shape) != (B, 16) or tuple(sparse.shape) != (B, 416):
+            raise TzkError(f"dot_interact27_fwd_bf16: expected dense [B, 16] and sparse [B, 416], got "
+                           f"{tuple(dense.shape)} and {tuple(sparse.shape)}")
+        out = torch.empty((B, 784), dtype=torch.bfloat16, device=sparse.device)
+        check(self._lib.tzk_dot_interact27_fwd_bf16(_ptr(dense), ld_d, _ptr(sparse), ld_s, B, _ptr(out), 784, _stream()),
+              "tzk_dot_interact27_fwd_bf16")
+        self.launches += 1
+        return out
+
+    def dot_interact27_bwd_bf16(self, d_out: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor):
+        """(d_dense [B, 16] bf16, d_sparse [B, 416] fp32) from dX [B, 784] bf16 (tzk_dot_interact27_bwd_bf16)."""
+        d_out, ld_o = _rows2d_dtype(d_out, torch.bfloat16, "d_out")
+        dense, ld_d = _rows2d_dtype(dense, torch.bfloat16, "dense")
+        sparse, ld_s = _rows2d(sparse, "sparse")
+        B = sparse.shape[0]
+        if tuple(d_out.shape) != (B, 784) or tuple(dense.shape) != (B, 16) or tuple(sparse.shape) != (B, 416):
+            raise TzkError(f"dot_interact27_bwd_bf16: expected dX [B, 784], dense [B, 16] and sparse [B, 416], got "
+                           f"{tuple(d_out.shape)}, {tuple(dense.shape)} and {tuple(sparse.shape)}")
+        d_dense = torch.empty((B, 16), dtype=torch.bfloat16, device=sparse.device)
+        d_sparse = torch.empty((B, 416), dtype=torch.float32, device=sparse.device)
+        check(self._lib.tzk_dot_interact27_bwd_bf16(_ptr(d_out), ld_o, _ptr(dense), ld_d, _ptr(sparse), ld_s, B,
+                                                    _ptr(d_dense), 16, _ptr(d_sparse), 416, _stream()),
+              "tzk_dot_interact27_bwd_bf16")
         self.launches += 1
         return d_dense, d_sparse
 

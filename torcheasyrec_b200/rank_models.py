@@ -8,6 +8,7 @@ Dense towers stay plain PyTorch exactly as in the reference (parameter names are
 
 from typing import Any, Dict, List, Optional
 
+import contextlib
 import os
 
 import torch
@@ -343,6 +344,12 @@ class DLRM(RankModel):
         x = self._interact_wide(dense_feat, sparse)
         if x is not None:           # the interaction and the first final-MLP layer in one autograd node
             in_map, start = None, 1
+        elif self._interact_bf16_ok(dense_feat, sparse):
+            # bf16 autocast: X [B, 784] bf16 straight from the tensor-core kernel; the first final-MLP layer is
+            # autocast's F.linear over it with the weight spread by in_map (dense_gemm.linear)
+            from .dense_gemm import InteractBf16Fn
+
+            x, in_map, start = InteractBf16Fn.apply(dense_feat, sparse), InteractBf16Fn.IN_MAP, 0
         else:
             # interaction + both concats of dlrm.py:113-131 in one kernel
             # the 783-wide result travels as [B, 784]: one zero column after the 351 interaction terms puts the dense
@@ -371,15 +378,24 @@ class DLRM(RankModel):
         in_map = ((0, 0, 351), (351, 352, 432))
         return InteractWideFn.apply(_gemm3x_lib(), dense_feat, sparse, first[0].weight, first[0].bias, in_map)
 
+    def _interact_bf16_ok(self, dense_feat: Optional[torch.Tensor], sparse: torch.Tensor) -> bool:
+        """DLRM-Criteo's glue under bf16 autocast (dense_gemm.InteractBf16Fn); every other shape or dtype takes the torch
+        formulation of Fn.dlrm_interaction."""
+        from .dense_gemm import interact_bf16_usable
+
+        return bool(self._model_config.arch_with_sparse) and interact_bf16_usable(dense_feat, sparse, self._sparse_num,
+                                                                                   self._per_sparse_dim)
+
     def _fused_tail(self, batch: Batch, all_feat: torch.Tensor, in_map, start: int = 0):
         """Training steps on CUDA: the last Perceptron of the final MLP, the output layer and the BCE loss as ONE kernel
         that also produces their gradients (csrc/tzk_tower_tail.cuh; 18 launches of latency-bound work on DLRM-Criteo).
-        The loss is handed to `loss()` through `_tail_loss`.  Default on; TZK_FUSED_TAIL=0 keeps the layer-by-layer chain."""
+        The loss is handed to `loss()` through `_tail_loss`.  Default on; TZK_FUSED_TAIL=0 keeps the layer-by-layer chain.
+        fp32 only: under autocast the layers run one by one as autocast's F.linear."""
         from .dense_gemm import tower_tail_bce, tower_tail_usable
 
         self._tail_loss = None
         layers = list(self.final_mlp.mlp)
-        if (not self.training or not torch.is_grad_enabled() or not all_feat.is_cuda or self._num_class != 1
+        if (not self.training or Fn.autocast_dtype(all_feat) is not None or not torch.is_grad_enabled() or not all_feat.is_cuda or self._num_class != 1
                 or not layers or self._label_name not in batch.labels or os.environ.get("TZK_FUSED_TAIL", "1") == "0"):
             return None
         last = layers[-1].perceptron
@@ -601,15 +617,38 @@ def dense_optimizer_from_config(train_config: Message, params, **kw) -> torch.op
     raise NotImplementedError(kind)
 
 
-class TrainWrapper(nn.Module):
-    """tzrec/models/model.py:271-297: forward(batch) -> (total_loss, (losses, predictions, batch))."""
+_MIXED_PRECISION_TO_DTYPE = {"BF16": torch.bfloat16, "FP16": torch.float16}
 
-    def __init__(self, model: RankModel) -> None:
+
+def mixed_precision_to_dtype(mixed_precision: Optional[str]) -> Optional[torch.dtype]:
+    """train_config.mixed_precision -> autocast dtype (tzrec/acc/utils.py:267-286): empty means off, an unknown value
+    raises."""
+    if not mixed_precision:
+        return None
+    if mixed_precision not in _MIXED_PRECISION_TO_DTYPE:
+        raise ValueError(f"Unknown mixed_precision: {mixed_precision}, "
+                         f"available types: {list(_MIXED_PRECISION_TO_DTYPE.keys())}")
+    return _MIXED_PRECISION_TO_DTYPE[mixed_precision]
+
+
+class TrainWrapper(nn.Module):
+    """tzrec/models/model.py:271-297: forward(batch) -> (total_loss, (losses, predictions, batch)), with `predict` and
+    `loss` under torch.autocast(device type, mixed_dtype) when a mixed-precision dtype is given.
+
+    The autocast weight-cast cache is off: a captured step (engine.GraphedTrainStep) then holds no cast tensor across
+    replays, and the eager and the captured step run the same casts.  The cast values are the same either way; only a
+    weight used twice in one forward is cast twice."""
+
+    def __init__(self, model: RankModel, mixed_dtype: Optional[torch.dtype] = None, device_type: str = "cuda") -> None:
         super().__init__()
         self.model = model
+        self.mixed_dtype, self.device_type = mixed_dtype, device_type
 
     def forward(self, batch: Batch):
-        predictions = self.model.predict(batch)
-        losses = self.model.loss(predictions, batch)
-        total = torch.stack(list(losses.values())).sum()
+        ctx = contextlib.nullcontext() if self.mixed_dtype is None else \
+            torch.autocast(self.device_type, dtype=self.mixed_dtype, cache_enabled=False)
+        with ctx:
+            predictions = self.model.predict(batch)
+            losses = self.model.loss(predictions, batch)
+            total = torch.stack(list(losses.values())).sum()
         return total, (losses, {k: v.detach() for k, v in predictions.items()}, batch)
