@@ -321,6 +321,20 @@ int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_
                           int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
                           int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
                           tzk_stream_t stream);
+/* The forward of the same pair of layers: y [M,64] = relu(X w^T + bias) with X = [351 pairs | 0 | dense | sparse] the
+ * interaction's output, and pairs [M,352] = X's first 352 columns (column 351 zero), which the weight gradient needs.
+ * X itself is never written.  w [64, ld_w] in the interaction's column layout (ld_w >= 784), bias nullable; w_hi / w_lo:
+ * [64, 784] scratch (the TF32 split of w).  Bit for bit tzk_dot_interact_fwd (p_pad = 1) followed by libtzk_gemm3x.so's
+ * forward.  Row strides multiples of 4 floats, every pointer but bias 16-B aligned. */
+int tzk_interact_wide_fwd(const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse, const float* w,
+                          int64_t ld_w, const float* bias, int64_t M, float* y, int64_t ld_y, float* pairs,
+                          int64_t ld_pairs, float* w_hi, float* w_lo, tzk_stream_t stream);
+/* Weight gradient of the layer, dw [64, 784] = dz [M,64]^T X in X's column layout, with X read from pairs, dense and
+ * sparse; bit for bit libtzk_gemm3x.so's tzk_wgrad3x on X with the same `slabs`.  partial: slabs * 896 * 64 floats of
+ * scratch.  Row strides multiples of 4 floats, every pointer 16-B aligned. */
+int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const float* pairs, int64_t ld_pairs, const float* dense,
+                            int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, int32_t slabs,
+                            float* partial, float* dw, int64_t ld_dw, tzk_stream_t stream);
 
 /* ---- dense-tower helpers (callers of the path: tzrec/modules/mlp.py:20-84, Perceptron = Linear -> ReLU) ----
  * The tower GEMMs stay library calls; these fuse the element-wise passes around them.

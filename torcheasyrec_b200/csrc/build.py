@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["tzk_core.cu", "tzk_gather.cu", "tzk_bwd.cu", "tzk_dist.cu", "tzk_dense.cu", "tzk_tower.cu", "tzk_din.cu", "tzk_peer.cu", "tzk_interact_wide.cu",
            "tzk_interact_bf16.cu"]
 HEADERS = ["tzk_common.cuh", "tzk_tower_bwd2.cuh", "tzk_interact_tc.cuh", "tzk_tower_tail.cuh", "tzk_interact_bf16.cuh",
-"tzk_sm90_ptx.h", "tzk_tma.h", os.path.join("..", "..", "include", "tzk.h")]
+"tzk_sm90_ptx.h", "tzk_tma.h", "tzk_wgrad3x.cuh", os.path.join("..", "..", "include", "tzk.h")]
 LIB = os.path.join(HERE, "libtzk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
@@ -65,7 +65,7 @@ def build_gemm3x(force: bool = False) -> str:
     """libtzk_gemm3x.so: hand-written TMA + mma.sync 3xTF32 GEMMs of the wide tower layer (forward, dgrad, wgrad)."""
     src = os.path.join(HERE, "tzk_gemm3x.cu")
     lib = os.path.join(HERE, "libtzk_gemm3x.so")
-    deps = [src] + [os.path.join(HERE, h) for h in ("tzk_sm90_ptx.h", "tzk_tma.h")]
+    deps = [src] + [os.path.join(HERE, h) for h in ("tzk_sm90_ptx.h", "tzk_tma.h", "tzk_wgrad3x.cuh")]
     if force or _mtime(lib) < max(_mtime(d) for d in deps):
         subprocess.run([NVCC, *FLAGS, "-shared", src, "-o", lib + ".tmp"], check=True)
         os.replace(lib + ".tmp", lib)

@@ -157,126 +157,7 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__
   }
 }
 
-// ======================================================================================================================
-// Weight gradient of the same layer:  dW[n, k] = sum_m dZ[m, n] * X[m, k]   (n < 64, k < K = 784, m < M = batch).
-// Work item = (column tile j of 128 X columns, row slab s); each CTA owns one item and computes the [64 x 128] block
-// dZ[slab]^T X[slab, tile] with A = dZ^T and B = X straight from the row-major boxes, streaming the slab in chunks of
-// 32 rows (4 k-steps of 8).  Warp w: n rows 16 (w % 4) .. +16, X columns 64 (w / 4) .. +64.  The partial block goes to
-// `partial`; wgrad_reduce_kernel adds the slabs in a fixed order and transposes into dW[64, K].  X is read exactly once
-// over all items (tiles read disjoint columns); dZ is re-read by the 7 column tiles from L2.
-// Per stage: X (4 boxes of 32 rows x 128 B = 16 KB) | dZ (2 boxes = 8 KB).
-constexpr int WG_ROWS = 32;                         // batch rows per chunk = 4 k-steps
-constexpr int WG_BOX = WG_ROWS * 128;               // one TMA box: 32 rows x 32 floats = 4 KB
-constexpr int WG_A = 4 * WG_BOX, WG_B = 2 * WG_BOX; // 16 KB, 8 KB
-constexpr int WG_STAGE = WG_A + WG_B;               // 24 KB
-constexpr int WG_STAGES = 4;                        // 96 KB: two CTAs per SM
-
-struct WgParams {
-  float* partial;      // [slabs, k_tiles * 128, 64]
-  int64_t M;           // batch rows
-  int64_t slab_rows;   // multiple of 32
-  int k_tiles;         // ceil(K / 128)
-};
-
-__global__ void __launch_bounds__(NUM_THREADS, 2)
-wgrad3x_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_dz, WgParams p) {
-  TZK_DYN_SMEM(uint8_t, smem);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int jt = blockIdx.x % p.k_tiles;                  // column tile of X
-  const int64_t slab = blockIdx.x / p.k_tiles;
-  const int64_t row0 = slab * p.slab_rows;
-  const int64_t rows = (p.M - row0 < p.slab_rows) ? p.M - row0 : p.slab_rows;
-  const int num_c = (int)((rows + WG_ROWS - 1) / WG_ROWS);  // rows past M are zero-filled by the TMA
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) mbar_init(full + s, 1);
-    fence_mbarrier_init();
-  }
-  __syncthreads();
-  auto load = [&](int c) {                                // thread 0 only
-    uint8_t* sb = smem + (c % WG_STAGES) * WG_STAGE;
-    uint64_t* bar = full + c % WG_STAGES;
-    const int r = (int)(row0 + (int64_t)c * WG_ROWS);
-    mbar_expect_tx(bar, WG_A + WG_B);
-#pragma unroll
-    for (int b = 0; b < 4; ++b) tma_load_2d(sb + b * WG_BOX, &map_x, bar, jt * 128 + b * 32, r);
-#pragma unroll
-    for (int b = 0; b < 2; ++b) tma_load_2d(sb + WG_A + b * WG_BOX, &map_dz, bar, b * 32, r);
-  };
-  if (threadIdx.x == 0)
-    for (int c = 0; c < WG_STAGES && c < num_c; ++c) load(c);
-
-  const int n0 = (warp & 3) * 16 + g;                     // this lane's n rows n0 and n0 + 8
-  const int kc0 = (warp >> 2) * 64 + g;                   // this lane's X column in n8 tile nt: kc0 + 8 nt
-  float acc[8][4], part[8][4];
-#pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) acc[nt][q] = 0.f;
-  for (int c = 0; c < num_c; ++c) {
-    const int s = c % WG_STAGES;
-    mbar_wait(full + s, (uint32_t)(c / WG_STAGES) & 1u);
-    const float* xs = reinterpret_cast<const float*>(smem + s * WG_STAGE);
-    const float* zs = reinterpret_cast<const float*>(smem + s * WG_STAGE + WG_A);
-    // element (m, col) of a [32 rows x 128 floats] operand held as 32-column boxes
-    auto at = [](const float* base, int m, int col) { return base[(col >> 5) * (WG_BOX / 4) + swz(m, col & 31)]; };
-#pragma unroll
-    for (int ks = 0; ks < WG_ROWS / 8; ++ks) {
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) part[nt][q] = 0.f;
-      const int m = ks * 8 + t;                           // batch rows m (a0, a1, b0) and m + 4 (a2, a3, b1)
-      const float a[4] = {at(zs, m, n0), at(zs, m, n0 + 8), at(zs, m + 4, n0), at(zs, m + 4, n0 + 8)};
-      uint32_t ah[4], al[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        ah[i] = tf32_bits(a[i]);
-        al[i] = tf32_bits(a[i] - __uint_as_float(ah[i]));
-      }
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        const float b[2] = {at(xs, m, kc0 + 8 * nt), at(xs, m + 4, kc0 + 8 * nt)};
-        uint32_t bh[2], bl[2];
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          bh[i] = tf32_bits(b[i]);
-          bl[i] = tf32_bits(b[i] - __uint_as_float(bh[i]));
-        }
-        mma_tf32(part[nt], al, bh);
-        mma_tf32(part[nt], ah, bl);
-        mma_tf32(part[nt], ah, bh);
-      }
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[nt][q] += part[nt][q];
-    }
-    __syncthreads();
-    if (threadIdx.x == 0 && c + WG_STAGES < num_c) load(c + WG_STAGES);
-  }
-  // c0/c1: n row n0, X columns 2t, 2t+1 of the n8 tile; c2/c3: n row n0 + 8
-  float* out = p.partial + ((int64_t)slab * p.k_tiles + jt) * 128 * 64;
-#pragma unroll
-  for (int nt = 0; nt < 8; ++nt) {
-    const int kcol = (warp >> 2) * 64 + nt * 8 + 2 * t;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) out[(int64_t)(kcol + (q & 1)) * 64 + n0 + 8 * (q >> 1)] = acc[nt][q];
-  }
-}
-
-// dW[n, k] = sum over slabs (fixed order) of partial[s, k, n]; one thread per (k, n), n fastest for the reads
-__global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int slabs, int k_pad, int K, float* __restrict__ dw,
-                                    int64_t ld_dw) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= K * 64) return;
-  const int k = i >> 6, n = i & 63;
-  float acc = 0.f;
-  for (int s = 0; s < slabs; ++s) acc += partial[((int64_t)s * k_pad + k) * 64 + n];
-  dw[(int64_t)n * ld_dw + k] = acc;
-}
+#include "tzk_wgrad3x.cuh"   // wgrad3x_kernel, wgrad_reduce_kernel
 
 __global__ void split_w_kernel(const float* __restrict__ w, int64_t n, float* __restrict__ hi, float* __restrict__ lo) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -332,24 +213,10 @@ extern "C" int64_t tzk_wgrad3x_partial_floats(int32_t K, int32_t slabs) {
 extern "C" int tzk_wgrad3x(const float* x, int64_t ld_x, const float* dz, int64_t ld_dz, int64_t M, int32_t K,
                            int32_t slabs, float* partial, float* dw, int64_t ld_dw, void* stream) {
   if (M <= 0 || K <= 0 || slabs <= 0 || (ld_x % 4) || (ld_dz % 4)) return 1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUtensorMap mx, mz;
-  if (make_map(&mx, x, M, K, ld_x, WG_ROWS) || make_map(&mz, dz, M, 64, ld_dz, WG_ROWS)) return 2;
-  WgParams p;
-  p.partial = partial;
-  p.M = M;
-  p.k_tiles = (K + 127) / 128;
-  p.slab_rows = ((M + slabs - 1) / slabs + WG_ROWS - 1) / WG_ROWS * WG_ROWS;
-  const int used = (int)((M + p.slab_rows - 1) / p.slab_rows);           // slabs that hold rows (<= slabs)
-  const size_t smem = (size_t)WG_STAGES * WG_STAGE + 64;
-#ifndef TZK_CPU_SHIM
-  static bool configured = false;     // once: nothing but the launches happens inside a stream capture
-  if (!configured) {
-    cudaFuncSetAttribute(wgrad3x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    configured = true;
-  }
-#endif
-  TZK_LAUNCH((wgrad3x_kernel), used * p.k_tiles, NUM_THREADS, smem, st, mx, mz, p);
-  TZK_LAUNCH((wgrad_reduce_kernel), (K * 64 + 255) / 256, 256, 0, st, partial, used, p.k_tiles * 128, K, dw, ld_dw);
-  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+  CUtensorMap mx[WG_SRC], mz;
+  if (make_map(&mx[0], x, M, K, ld_x, WG_ROWS) || make_map(&mz, dz, M, 64, ld_dz, WG_ROWS)) return 2;
+  mx[1] = mx[2] = mx[0];
+  const int boxes = (K + 31) / 32, none = 1 << 20;     // one source: every box, K columns
+  const WgSources src = {{0, none, none, boxes}, {0, 0, 0}, {0, 0, 0}, {K, 0, 0}};
+  return wgrad3x_launch(mx, mz, src, M, slabs, partial, dw, ld_dw, reinterpret_cast<cudaStream_t>(stream));
 }

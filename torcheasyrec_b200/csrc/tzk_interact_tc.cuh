@@ -23,9 +23,9 @@
 // Accuracy: x = hi + lo with hi = tf32(x), lo = tf32(x - hi); the dropped lo*lo term is 2^-22 relative — the same class as
 // the fp32 FFMA kernels (tests hold both to 1e-5).  Summation order differs from a sequential dot product.
 //
-// The includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_dense.cu, and tzk_interact_wide.cu for bwd_sample; g++ +
-// tests/native/cuda_cpu_shim.h: tests/test_interact_tc_cpu.py runs this source on the host with an emulated mma),
-// tzk_itc::mma_tf32 and tzk_itc::cvt_tf32.
+// The includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_dense.cu, and tzk_interact_wide.cu for fwd_sample /
+// bwd_sample; g++ + tests/native/cuda_cpu_shim.h: tests/test_interact_tc_cpu.py runs this source on the host with an
+// emulated mma), tzk_itc::mma_tf32 and tzk_itc::cvt_tf32.
 #pragma once
 #include <stdint.h>
 
@@ -47,6 +47,66 @@ __device__ __forceinline__ float4 load_x4(const float* dense_row, const float* s
 }
 
 // ---- forward --------------------------------------------------------------------------------------------------------
+// first pair slot of the four rows lane (g, t)'s accumulators belong to: tri(i, j) = rowbase(i) + j
+__device__ __forceinline__ void pair_rowbase(int g, int (&rowbase)[4]) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int i = g + 8 * q;
+    rowbase[q] = i * kN - (i * (i + 1)) / 2 - i - 1;
+  }
+}
+
+// One sample, one warp: the kP pairs of Z = X X^T from the lane's rows x[j] = X[g + 8 j][4 t .. 4 t + 3] (zero beyond
+// row 26), written as the kInter floats prow[0 .. kInter) in 16-B stores through the warp's staging row O (kInter floats,
+// O[kP] zero).
+__device__ __forceinline__ void fwd_sample(const float4 (&x)[4], const int (&rowbase)[4], float* O, float* prow,
+                                           int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  uint32_t hi[4][4], lo[4][4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    split_tf32(x[j].x, hi[j][0], lo[j][0]);
+    split_tf32(x[j].y, hi[j][1], lo[j][1]);
+    split_tf32(x[j].z, hi[j][2], lo[j][2]);
+    split_tf32(x[j].w, hi[j][3], lo[j][3]);
+  }
+  // tiles (mt, nt) that touch i < j: (0,0) (0,1) (0,2) (0,3) (1,2) (1,3)
+  float acc[6][4];
+#pragma unroll
+  for (int e = 0; e < 6; ++e)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[e][q] = 0.f;
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+    for (int e = 0; e < 6; ++e) {
+      const int mt = e < 4 ? 0 : 1, nt = e < 4 ? e : e - 2;
+      const uint32_t ah[4] = {hi[2 * mt][2 * ks], hi[2 * mt + 1][2 * ks], hi[2 * mt][2 * ks + 1], hi[2 * mt + 1][2 * ks + 1]};
+      const uint32_t al[4] = {lo[2 * mt][2 * ks], lo[2 * mt + 1][2 * ks], lo[2 * mt][2 * ks + 1], lo[2 * mt + 1][2 * ks + 1]};
+      const uint32_t bh[2] = {hi[nt][2 * ks], hi[nt][2 * ks + 1]};
+      const uint32_t bl[2] = {lo[nt][2 * ks], lo[nt][2 * ks + 1]};
+      mma_tf32(acc[e], al, bh);
+      mma_tf32(acc[e], ah, bl);
+      mma_tf32(acc[e], ah, bh);
+    }
+  }
+  // accumulator (q) of tile e: i = g + 16 mt + 8 (q / 2), j = 8 nt + 2 t + (q % 2)
+#pragma unroll
+  for (int e = 0; e < 6; ++e) {
+    const int mt = e < 4 ? 0 : 1, nt = e < 4 ? e : e - 2;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int ri = 2 * mt + (q >> 1);
+      const int i = g + 8 * ri, j = 8 * nt + 2 * t + (q & 1);
+      if (i < j && j < kN) O[rowbase[ri] + j] = acc[e][q];
+    }
+  }
+  __syncwarp();
+  for (int c = lane; c < kInter / 4; c += 32)
+    *reinterpret_cast<float4*>(prow + 4 * c) = *reinterpret_cast<const float4*>(O + 4 * c);
+  __syncwarp();
+}
+
 __global__ void __launch_bounds__(kWarps * 32)
 dot_interact27_fwd_tc_kernel(const float* __restrict__ dense, int64_t ld_dense, const float* __restrict__ sparse,
                              int64_t ld_sparse, int64_t B, float* __restrict__ out, int64_t ld_out) {
@@ -55,13 +115,8 @@ dot_interact27_fwd_tc_kernel(const float* __restrict__ dense, int64_t ld_dense, 
   const int g = lane >> 2, t = lane & 3;
   float* O = smem + warp * kInter;
   if (lane == 0) O[kP] = 0.f;          // the zero between the pairs and the dense block
-  // first pair slot of the four rows this lane's accumulators belong to: tri(i, j) = rowbase(i) + j
   int rowbase[4];
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int i = g + 8 * q;
-    rowbase[q] = i * kN - (i * (i + 1)) / 2 - i - 1;
-  }
+  pair_rowbase(g, rowbase);
   const int64_t stride = (int64_t)gridDim.x * kWarps;
   int64_t b = (int64_t)blockIdx.x * kWarps + warp;
   float4 x[4];
@@ -84,49 +139,7 @@ dot_interact27_fwd_tc_kernel(const float* __restrict__ dense, int64_t ld_dense, 
       const int r = g + 8 * j;
       if (r < kN) *reinterpret_cast<float4*>(orow + kInter + r * kD + 4 * t) = x[j];
     }
-    uint32_t hi[4][4], lo[4][4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      split_tf32(x[j].x, hi[j][0], lo[j][0]);
-      split_tf32(x[j].y, hi[j][1], lo[j][1]);
-      split_tf32(x[j].z, hi[j][2], lo[j][2]);
-      split_tf32(x[j].w, hi[j][3], lo[j][3]);
-    }
-    // tiles (mt, nt) that touch i < j: (0,0) (0,1) (0,2) (0,3) (1,2) (1,3)
-    float acc[6][4];
-#pragma unroll
-    for (int e = 0; e < 6; ++e)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[e][q] = 0.f;
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-#pragma unroll
-      for (int e = 0; e < 6; ++e) {
-        const int mt = e < 4 ? 0 : 1, nt = e < 4 ? e : e - 2;
-        const uint32_t ah[4] = {hi[2 * mt][2 * ks], hi[2 * mt + 1][2 * ks], hi[2 * mt][2 * ks + 1], hi[2 * mt + 1][2 * ks + 1]};
-        const uint32_t al[4] = {lo[2 * mt][2 * ks], lo[2 * mt + 1][2 * ks], lo[2 * mt][2 * ks + 1], lo[2 * mt + 1][2 * ks + 1]};
-        const uint32_t bh[2] = {hi[nt][2 * ks], hi[nt][2 * ks + 1]};
-        const uint32_t bl[2] = {lo[nt][2 * ks], lo[nt][2 * ks + 1]};
-        mma_tf32(acc[e], al, bh);
-        mma_tf32(acc[e], ah, bl);
-        mma_tf32(acc[e], ah, bh);
-      }
-    }
-    // accumulator (q) of tile e: i = g + 16 mt + 8 (q / 2), j = 8 nt + 2 t + (q % 2)
-#pragma unroll
-    for (int e = 0; e < 6; ++e) {
-      const int mt = e < 4 ? 0 : 1, nt = e < 4 ? e : e - 2;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int ri = 2 * mt + (q >> 1);
-        const int i = g + 8 * ri, j = 8 * nt + 2 * t + (q & 1);
-        if (i < j && j < kN) O[rowbase[ri] + j] = acc[e][q];
-      }
-    }
-    __syncwarp();
-    for (int c = lane; c < kInter / 4; c += 32)
-      *reinterpret_cast<float4*>(orow + 4 * c) = *reinterpret_cast<const float4*>(O + 4 * c);
-    __syncwarp();
+    fwd_sample(x, rowbase, O, orow, lane);
     if (bn < B) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) x[j] = xn[j];

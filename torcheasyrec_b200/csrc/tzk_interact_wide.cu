@@ -1,11 +1,13 @@
-// tzk_interact_wide.cu — DLRM-Criteo's dot interaction and the first layer of its final MLP (783 -> 64) share one
-// backward kernel: the layer's input gradient dX [B, 784] is turned into the interaction's input gradients inside the
-// CTA that computes it and never reaches global memory (tzk_interact_wide_bwd, include/tzk.h).
+// tzk_interact_wide.cu — DLRM-Criteo's dot interaction and the first layer of its final MLP (783 -> 64) without the
+// layer's input X [B, 784] or its gradient in global memory (include/tzk.h):
+//   tzk_interact_wide_fwd    the interaction's pairs and the layer's output in one kernel; only the pairs are stored
+//   tzk_interact_wide_bwd    the layer's input gradient turned into the interaction's input gradients in the CTA
+//   tzk_interact_wide_wgrad  the layer's weight gradient with X read from the pairs, dense and sparse (tzk_wgrad3x.cuh)
 //
-// The GEMM part is written like tzk_gemm3x.cu (TMA SWIZZLE_128B boxes through mbarrier-guarded stages, mma.sync m16n8k8
-// TF32 with the 3xTF32 split, every k-step accumulated in fresh registers and added in round-to-nearest); the per-sample
-// interaction backward is tzk_interact_tc.cuh's.  The same source runs on the CPU under tests/native/cuda_cpu_shim.h and
-// sm90_cpu_emu.h (tests/test_interact_wide_fused.py).
+// The GEMM parts are written like tzk_gemm3x.cu (TMA SWIZZLE_128B boxes through mbarrier-guarded stages, mma.sync
+// m16n8k8 TF32 with the 3xTF32 split, every k-step accumulated in fresh registers and added in round-to-nearest); the
+// per-sample interaction is tzk_interact_tc.cuh's.  The same source runs on the CPU under tests/native/cuda_cpu_shim.h
+// and sm90_cpu_emu.h (tests/test_interact_wide_fused.py, tests/test_interact_wide_fwd_fused.py).
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -187,6 +189,189 @@ interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_whi, const __gr
   }
 }
 
+// ======================================================================================================================
+// Forward of the same layer fused with the interaction that produces its input: Y = relu(X W^T + b) with X = [351 pairs
+// | 0 | dense 16 | sparse 416], and the pair columns [M, 352] (column 351 zero) for the weight gradient.  X is never
+// written: 432 of its 784 columns are copies of dense / sparse.  Per CTA of FF_M samples (gemm3x_kernel<64>'s tile):
+//   1. per sample, one warp: the pairs (tzk_itc::fwd_sample) -> `pairs` in global memory (the rows stay in L2).
+//   2. gemm3x_kernel<64>'s k-loop over X's 25 chunks of 32 columns.  A comes by TMA: chunks 0 .. 10 from `pairs` (written
+//      by this CTA in step 1: proxy fence + barrier first), 12 .. 24 from `sparse` at column 32 c - 368.  Chunk 11
+//      straddles dense 0 .. 15 | sparse 0 .. 15: a dense box in the stage and a sparse box (column 0) in the region
+//      that held step 1's staging rows; its k-steps 0, 1 read the first, 2, 3 the second.
+// The pair columns have to exist before the first k-step; the other CTA on the SM (two fit) keeps the tensor cores busy
+// while this one computes them.  Same k-order and per-k-step accumulation as gemm3x_kernel, so Y is bit for bit what
+// dot_interact27_fwd_tc_kernel followed by gemm3x_kernel<64> computes.
+constexpr int FF_M = 128;                     // samples per CTA
+constexpr int FF_THREADS = 256;               // 8 warps x 16 rows, all 64 columns each
+constexpr int FF_WARPS = FF_THREADS / 32;
+constexpr int FF_X_BYTES = FF_M * 128;        // A box: FF_M rows x 32 floats
+constexpr int FF_W_BYTES = 64 * 128;          // W hi or lo box: 64 rows x 32 floats
+constexpr int FF_STAGE = FF_X_BYTES + 2 * FF_W_BYTES;
+constexpr int FF_STAGES = 3;
+constexpr int FF_E_OFF = FF_STAGES * FF_STAGE;          // step 1: the warps' staging rows; chunk 11: the sparse box
+constexpr int FF_BAR_OFF = FF_E_OFF + FF_X_BYTES;
+constexpr int FF_SMEM = FF_BAR_OFF + FF_STAGES * 8;    // 114 712 B: two CTAs per SM
+static_assert(FF_WARPS * tzk_itc::kInter * 4 <= FF_X_BYTES, "staging rows overflow their region");
+constexpr int FF_SPARSE0 = tzk_itc::kInter + tzk_itc::kD;   // X column of sparse column 0
+
+struct FfParams {
+  const float* dense; int64_t ld_dense;
+  const float* sparse; int64_t ld_sparse;
+  float* pairs; int64_t ld_pairs;
+  const float* bias;
+  float* y; int64_t ld_y;
+  int64_t M;
+};
+
+// orders this thread's generic-proxy accesses before later async-proxy (TMA) ones: the pair rows in global memory that
+// TMA reads back, the staging rows in shared memory that TMA overwrites
+__device__ __forceinline__ void fence_proxy_async() {
+#ifndef TZK_CPU_SHIM
+  asm volatile("fence.proxy.async;" ::: "memory");
+#endif
+}
+
+__global__ void __launch_bounds__(FF_THREADS, 2)
+interact_wide_fwd_kernel(const __grid_constant__ CUtensorMap map_pairs, const __grid_constant__ CUtensorMap map_dense,
+                         const __grid_constant__ CUtensorMap map_sparse, const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
+                         FfParams p) {
+  TZK_DYN_SMEM(uint8_t, smem);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + FF_BAR_OFF);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int64_t m0 = (int64_t)blockIdx.x * FF_M;
+  const int64_t m_end = p.M - m0 < FF_M ? p.M : m0 + FF_M;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < FF_STAGES; ++s) mbar_init(full + s, 1);
+    fence_mbarrier_init();
+  }
+  {   // 1. warp w: samples m0 + w, m0 + w + 8, ..; the next sample's rows are requested before this one is worked on
+    float* O = reinterpret_cast<float*>(smem + FF_E_OFF) + warp * tzk_itc::kInter;
+    if (lane == 0) O[tzk_itc::kP] = 0.f;
+    int rowbase[4];
+    tzk_itc::pair_rowbase(g, rowbase);
+    int64_t b = m0 + warp;
+    float4 x[4];
+    if (b < m_end) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) x[j] = tzk_itc::load_x4(p.dense + b * p.ld_dense, p.sparse + b * p.ld_sparse, g + 8 * j, 4 * t);
+    }
+    for (; b < m_end; b += FF_WARPS) {
+      float4 xn[4];
+      const int64_t bn = b + FF_WARPS;
+      if (bn < m_end) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          xn[j] = tzk_itc::load_x4(p.dense + bn * p.ld_dense, p.sparse + bn * p.ld_sparse, g + 8 * j, 4 * t);
+      }
+      tzk_itc::fwd_sample(x, rowbase, O, p.pairs + b * p.ld_pairs, lane);
+      if (bn < m_end) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) x[j] = xn[j];
+      }
+    }
+  }
+  fence_proxy_async();
+  __syncthreads();                                // the pair rows are written; the mbarriers are initialised
+
+  auto load = [&](int c) {                        // thread 0 only
+    uint8_t* sb = smem + (c % FF_STAGES) * FF_STAGE;
+    uint64_t* bar = full + c % FF_STAGES;
+    mbar_expect_tx(bar, c == FB_PAIR_CHUNKS ? FF_STAGE + FF_X_BYTES : FF_STAGE);
+    if (c < FB_PAIR_CHUNKS) {
+      tma_load_2d(sb, &map_pairs, bar, 32 * c, (int)m0);
+    } else if (c == FB_PAIR_CHUNKS) {
+      tma_load_2d(sb, &map_dense, bar, 0, (int)m0);
+      tma_load_2d(smem + FF_E_OFF, &map_sparse, bar, 0, (int)m0);
+    } else {
+      tma_load_2d(sb, &map_sparse, bar, 32 * c - FF_SPARSE0, (int)m0);
+    }
+    tma_load_2d(sb + FF_X_BYTES, &map_whi, bar, 32 * c, 0);
+    tma_load_2d(sb + FF_X_BYTES + FF_W_BYTES, &map_wlo, bar, 32 * c, 0);
+  };
+  if (threadIdx.x == 0)
+    for (int c = 0; c < FF_STAGES; ++c) load(c);
+
+  // 2. gemm3x_kernel<64>: rows r and r + 8 of the tile, all 64 columns
+  const int r = warp * 16 + g;
+  float acc[8][4], part[8][4];
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[nt][q] = 0.f;
+  for (int c = 0; c < FB_CHUNKS; ++c) {
+    const int s = c % FF_STAGES;
+    mbar_wait(full + s, (uint32_t)(c / FF_STAGES) & 1u);
+    const float* xs = reinterpret_cast<const float*>(smem + s * FF_STAGE);
+    const uint32_t* whi = reinterpret_cast<const uint32_t*>(smem + s * FF_STAGE + FF_X_BYTES);
+    const uint32_t* wlo = whi + FF_W_BYTES / 4;
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) part[nt][q] = 0.f;
+      const int k0 = ks * 8 + t, k1 = k0 + 4;
+      // chunk 11, k-steps 2 and 3: X column 368 + j = sparse column j of the second box.  With k = 16 + j the 16-B
+      // chunk index of k is j's with bit 2 set, so swz(., j) = swz(., k) ^ 16.
+      const bool sp = ks >= 2 && c == FB_PAIR_CHUNKS;
+      const float* as = sp ? reinterpret_cast<const float*>(smem + FF_E_OFF) : xs;
+      const int x16 = sp ? 16 : 0;
+      const float a[4] = {as[swz(r, k0) ^ x16], as[swz(r + 8, k0) ^ x16], as[swz(r, k1) ^ x16], as[swz(r + 8, k1) ^ x16]};
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        ah[i] = tf32_bits(a[i]);
+        al[i] = tf32_bits(a[i] - __uint_as_float(ah[i]));
+      }
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const int n = nt * 8 + g;
+        const uint32_t bh[2] = {whi[swz(n, k0)], whi[swz(n, k1)]};
+        const uint32_t bl[2] = {wlo[swz(n, k0)], wlo[swz(n, k1)]};
+        mma_tf32(part[nt], al, bh);               // small terms first
+        mma_tf32(part[nt], ah, bl);
+        mma_tf32(part[nt], ah, bh);
+      }
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[nt][q] += part[nt][q];
+    }
+    __syncthreads();                              // every warp is done with stage s: refill it
+    if (threadIdx.x == 0 && c + FF_STAGES < FB_CHUNKS) load(c + FF_STAGES);
+  }
+  // c0/c1: row r, columns 2t, 2t+1 of the n8 tile; c2/c3: row r + 8
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    const int col = nt * 8 + 2 * t;
+    const float b0 = p.bias ? __ldg(p.bias + col) : 0.f, b1 = p.bias ? __ldg(p.bias + col + 1) : 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = m0 + r + 8 * h;
+      if (row >= p.M) continue;
+      float2 o = make_float2(acc[nt][2 * h] + b0, acc[nt][2 * h + 1] + b1);
+      o.x = fmaxf(o.x, 0.f);
+      o.y = fmaxf(o.y, 0.f);
+      *reinterpret_cast<float2*>(p.y + row * p.ld_y + col) = o;
+    }
+  }
+}
+
+// W hi / lo [64, K] (row stride K) from W [64, ld_w]
+__global__ void split_w_kernel(const float* __restrict__ w, int64_t ld_w, int K, float* __restrict__ hi,
+                               float* __restrict__ lo) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < K * 64) {
+    const float v = w[(int64_t)(i / K) * ld_w + i % K];
+    const float h = tf32_rna(v);
+    hi[i] = h;
+    lo[i] = tf32_rna(v - h);
+  }
+}
+
+#include "tzk_wgrad3x.cuh"   // wgrad3x_kernel, wgrad_reduce_kernel
+
 // W^T hi / lo [K, 64] from W [64, ld_w] (K columns used)
 __global__ void split_wt_kernel(const float* __restrict__ w, int64_t ld_w, int K, float* __restrict__ hi,
                                 float* __restrict__ lo) {
@@ -230,5 +415,64 @@ extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float
 #endif
   TZK_LAUNCH((interact_wide_bwd_kernel), (unsigned)((M + FB_M - 1) / FB_M), FB_THREADS, FB_SMEM, st, mh, ml, p);
   TZK_CHECK_LAUNCH("interact_wide_bwd_kernel");
+  return 0;
+}
+
+extern "C" int tzk_interact_wide_fwd(const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse,
+                                     const float* w, int64_t ld_w, const float* bias, int64_t M, float* y, int64_t ld_y,
+                                     float* pairs, int64_t ld_pairs, float* w_hi, float* w_lo, tzk_stream_t stream) {
+  TZK_REQUIRE(M > 0, "interact_wide_fwd: M must be positive");
+  TZK_REQUIRE(ld_w >= tzk_itc::kRow && ld_y >= 64 && ld_pairs >= tzk_itc::kInter && ld_dense >= tzk_itc::kD &&
+              ld_sparse >= tzk_itc::kRow - FF_SPARSE0, "interact_wide_fwd: row stride shorter than the row");
+  const int64_t lds[] = {ld_dense, ld_sparse, ld_w, ld_y, ld_pairs};
+  for (int64_t ld : lds) TZK_REQUIRE(ld % 4 == 0, "interact_wide_fwd: row strides must be multiples of 4 floats");
+  const void* ptrs[] = {dense, sparse, w, y, pairs, w_hi, w_lo};
+  for (const void* q : ptrs)
+    TZK_REQUIRE(q && reinterpret_cast<uintptr_t>(q) % 16 == 0, "interact_wide_fwd: NULL or not 16-B aligned pointer");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  TZK_LAUNCH((split_w_kernel), (tzk_itc::kRow * 64 + 255) / 256, 256, 0, st, w, ld_w, tzk_itc::kRow, w_hi, w_lo);
+  CUtensorMap mp, md, ms, mh, ml;
+  TZK_REQUIRE(!make_map(&mp, pairs, M, tzk_itc::kInter, ld_pairs, FF_M) &&
+              !make_map(&md, dense, M, tzk_itc::kD, ld_dense, FF_M) &&
+              !make_map(&ms, sparse, M, tzk_itc::kRow - FF_SPARSE0, ld_sparse, FF_M) &&
+              !make_map(&mh, w_hi, 64, tzk_itc::kRow, tzk_itc::kRow, 64) &&
+              !make_map(&ml, w_lo, 64, tzk_itc::kRow, tzk_itc::kRow, 64), "interact_wide_fwd: tensor-map encoding failed");
+  FfParams p;
+  p.dense = dense; p.ld_dense = ld_dense; p.sparse = sparse; p.ld_sparse = ld_sparse; p.pairs = pairs;
+  p.ld_pairs = ld_pairs; p.bias = bias; p.y = y; p.ld_y = ld_y; p.M = M;
+#ifndef TZK_CPU_SHIM
+  static bool configured = false;     // once: nothing but the launches happens inside a stream capture
+  if (!configured) {
+    cudaFuncSetAttribute(interact_wide_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FF_SMEM);
+    configured = true;
+  }
+#endif
+  TZK_LAUNCH((interact_wide_fwd_kernel), (unsigned)((M + FF_M - 1) / FF_M), FF_THREADS, FF_SMEM, st, mp, md, ms, mh, ml, p);
+  TZK_CHECK_LAUNCH("interact_wide_fwd_kernel");
+  return 0;
+}
+
+extern "C" int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const float* pairs, int64_t ld_pairs,
+                                       const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse,
+                                       int64_t M, int32_t slabs, float* partial, float* dw, int64_t ld_dw,
+                                       tzk_stream_t stream) {
+  TZK_REQUIRE(M > 0 && slabs > 0, "interact_wide_wgrad: M and slabs must be positive");
+  TZK_REQUIRE(ld_dw >= tzk_itc::kRow, "interact_wide_wgrad: dw needs %d columns", tzk_itc::kRow);
+  const int64_t lds[] = {ld_dz, ld_pairs, ld_dense, ld_sparse};
+  for (int64_t ld : lds) TZK_REQUIRE(ld % 4 == 0, "interact_wide_wgrad: row strides must be multiples of 4 floats");
+  const void* ptrs[] = {dz, pairs, dense, sparse, partial, dw};
+  for (const void* q : ptrs)
+    TZK_REQUIRE(q && reinterpret_cast<uintptr_t>(q) % 16 == 0, "interact_wide_wgrad: NULL or not 16-B aligned pointer");
+  CUtensorMap mx[WG_SRC], mz;
+  TZK_REQUIRE(!make_map(&mx[0], pairs, M, tzk_itc::kInter, ld_pairs, WG_ROWS) &&
+              !make_map(&mx[1], sparse, M, tzk_itc::kRow - FF_SPARSE0, ld_sparse, WG_ROWS) &&
+              !make_map(&mx[2], dense, M, tzk_itc::kD, ld_dense, WG_ROWS) &&
+              !make_map(&mz, dz, M, 64, ld_dz, WG_ROWS), "interact_wide_wgrad: tensor-map encoding failed");
+  // boxes 0 .. 10: pairs -> X columns 0 .. 351; 11 .. 23: sparse -> 368 ..; 24 (and the tile's padding 25 .. 27,
+  // past the tensor: zeros, never written): dense -> 352 .. 367
+  const WgSources src = {{0, FB_PAIR_CHUNKS, FB_CHUNKS - 1, FB_CHUNKS}, {0, 0, 0}, {0, FF_SPARSE0, tzk_itc::kInter},
+                         {tzk_itc::kInter, tzk_itc::kRow - FF_SPARSE0, tzk_itc::kD}};
+  TZK_REQUIRE(wgrad3x_launch(mx, mz, src, M, slabs, partial, dw, ld_dw, reinterpret_cast<cudaStream_t>(stream)) == 0,
+              "interact_wide_wgrad: launch failed");
   return 0;
 }

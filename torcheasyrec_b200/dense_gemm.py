@@ -280,37 +280,38 @@ class Gemm3xLinearFn(torch.autograd.Function):
 
 class InteractWideFn(torch.autograd.Function):
     """relu(X @ W^T + b) with X = functional.dlrm_interaction(dense, sparse, 26, 16, aligned=True), the first layer of
-    DLRM-Criteo's final MLP.  The forward is the interaction kernel followed by gemm3x; the backward computes the
-    interaction's input gradients in one kernel from dZ and W (tzk_interact_wide_bwd) instead of writing X's gradient
-    [M, 784] to memory and reading it back, and the weight gradient with wgrad3x from the saved X.  fp32 only: under
-    autocast interact_wide_usable() is False and the layer runs as autocast's F.linear."""
+    DLRM-Criteo's final MLP, without X [M, 784] ever reaching memory: the forward computes the interaction and the layer
+    in one kernel (tzk_interact_wide_fwd), which keeps only X's pair columns [M, 352]; the backward computes the
+    interaction's input gradients in one kernel from dZ and W (tzk_interact_wide_bwd) and the weight gradient from the
+    pairs, dense and sparse (tzk_interact_wide_wgrad).  Bit for bit the layer-by-layer path (interaction kernel,
+    gemm3x, wgrad3x).  fp32 only: under autocast interact_wide_usable() is False and the layer runs as autocast's
+    F.linear.  `lib` (libtzk_gemm3x.so) is unused: the signature stays that of Gemm3xLinearFn."""
 
     @staticmethod
     def forward(ctx, lib, dense, sparse, weight, bias, in_map):
-        from .functional import _rows_contig, backend
+        from .functional import _rows_contig
+        from .kernels import default_kernels
 
         dense, sparse = _rows_contig(dense), _rows_contig(sparse)
-        x = backend().dot_interact_fwd(dense, sparse, 26, 16, True, True, 4, 1)
-        w = torch.zeros((weight.shape[0], x.shape[1]), dtype=weight.dtype, device=weight.device)
+        w = torch.zeros((weight.shape[0], 784), dtype=weight.dtype, device=weight.device)
         for (src, dst, n) in in_map:
             w[:, dst:dst + n].copy_(weight[:, src:src + n])
-        y = gemm3x(lib, x, w, bias, True)
-        ctx.lib, ctx.in_map, ctx.has_bias = lib, in_map, bias is not None
-        ctx.save_for_backward(dense, sparse, x, w, y)
+        y, pairs = default_kernels().interact_wide_fwd(dense, sparse, w, bias)
+        ctx.in_map, ctx.has_bias = in_map, bias is not None
+        ctx.save_for_backward(dense, sparse, pairs, w, y)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         from .kernels import default_kernels
 
-        dense, sparse, x, w, y = ctx.saved_tensors
-        lib = ctx.lib
+        dense, sparse, pairs, w, y = ctx.saved_tensors
         dz, colsum = default_kernels().act_bwd_colsum(dy.contiguous(), y, True, want_dz=True)
         d_dense = d_sparse = dw = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             d_dense, d_sparse = default_kernels().interact_wide_bwd(dz, w, dense, sparse)
         if ctx.needs_input_grad[3]:
-            full = wgrad3x(lib, x, dz)
+            full = default_kernels().interact_wide_wgrad(dz, pairs, dense, sparse, SLABS)
             dw = torch.cat([full[:, dst:dst + n] for (_, dst, n) in ctx.in_map], dim=1)
         db = colsum if (ctx.has_bias and ctx.needs_input_grad[4]) else None
         return (None, d_dense if ctx.needs_input_grad[1] else None, d_sparse if ctx.needs_input_grad[2] else None, dw, db,

@@ -870,6 +870,37 @@ class CudaKernels:
         self.launches += 1
         return d_dense, d_sparse
 
+    def interact_wide_fwd(self, dense: torch.Tensor, sparse: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]):
+        """(y [B, 64], pairs [B, 352]): relu(X w^T + bias) of DLRM-Criteo's interaction output X [B, 784] (never written)
+        and X's pair columns, with w [64, 784] in the interaction's column layout."""
+        dense, ld_d = _rows2d(dense, "dense")
+        sparse, ld_s = _rows2d(sparse, "sparse")
+        w, ld_w = _rows2d(w, "w")
+        B = dense.shape[0]
+        y = torch.empty((B, 64), dtype=torch.float32, device=dense.device)
+        pairs = torch.empty((B, 352), dtype=torch.float32, device=dense.device)
+        ws = torch.empty((2, 64, 784), dtype=torch.float32, device=dense.device)
+        check(self._lib.tzk_interact_wide_fwd(_ptr(dense), ld_d, _ptr(sparse), ld_s, _ptr(w), ld_w, _ptr(bias), B,
+                                              _ptr(y), 64, _ptr(pairs), 352, _ptr(ws[0]), _ptr(ws[1]), _stream()),
+              "tzk_interact_wide_fwd")
+        self.launches += 2
+        return y, pairs
+
+    def interact_wide_wgrad(self, dz: torch.Tensor, pairs: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor,
+                            slabs: int) -> torch.Tensor:
+        """dW [64, 784] = dz^T X in the interaction's column layout, X = [pairs | dense | sparse] read in place."""
+        dz, ld_z = _rows2d(dz, "dz")
+        pairs, ld_p = _rows2d(pairs, "pairs")
+        dense, ld_d = _rows2d(dense, "dense")
+        sparse, ld_s = _rows2d(sparse, "sparse")
+        B = dz.shape[0]
+        dw = torch.empty((64, 784), dtype=torch.float32, device=dz.device)
+        part = torch.empty(slabs * 896 * 64, dtype=torch.float32, device=dz.device)
+        check(self._lib.tzk_interact_wide_wgrad(_ptr(dz), ld_z, _ptr(pairs), ld_p, _ptr(dense), ld_d, _ptr(sparse), ld_s,
+                                                B, slabs, _ptr(part), _ptr(dw), 784, _stream()), "tzk_interact_wide_wgrad")
+        self.launches += 2
+        return dw
+
     def interact_wide_bwd(self, dz: torch.Tensor, w: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor):
         """(d_dense [B, 16], d_sparse [B, 416]) of DLRM-Criteo's interaction followed by a 784 -> 64 layer with weight
         w [64, 784] (the interaction's column layout), from dz [B, 64], the gradient of the layer's pre-activation."""
