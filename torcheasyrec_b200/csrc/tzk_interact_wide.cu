@@ -2,12 +2,16 @@
 // layer's input X [B, 784] or its gradient in global memory (include/tzk.h):
 //   tzk_interact_wide_fwd    the interaction's pairs and the layer's output in one kernel; only the pairs are stored
 //   tzk_interact_wide_bwd    the layer's input gradient turned into the interaction's input gradients in the CTA
-//   tzk_interact_wide_wgrad  the layer's weight gradient with X read from the pairs, dense and sparse (tzk_wgrad3x.cuh)
+//   tzk_interact_wide_wgrad  the layer's weight gradient with X read from the pairs, dense and sparse (tzk_wgrad3x.cuh's
+//                            work items)
 //
-// The GEMM parts are written like tzk_gemm3x.cu (TMA SWIZZLE_128B boxes through mbarrier-guarded stages, mma.sync
-// m16n8k8 TF32 with the 3xTF32 split, every k-step accumulated in fresh registers and added in round-to-nearest); the
-// per-sample interaction is tzk_interact_tc.cuh's.  The same source runs on the CPU under tests/native/cuda_cpu_shim.h
-// and sm90_cpu_emu.h (tests/test_interact_wide_fused.py, tests/test_interact_wide_fwd_fused.py).
+// The GEMM parts compute what tzk_gemm3x.cu computes (TMA SWIZZLE_128B boxes through mbarrier-guarded stages, the 3xTF32
+// split, every k-step's three products in a fresh accumulator, added in round-to-nearest in k order).  The forward and
+// the weight gradient issue each k-step as m64n64k8 warpgroup MMAs (tzk_wgmma.cuh) with B straight from shared memory:
+// one wgmma k8 gives the bits of the mma.sync m16n8k8 it replaces (tests/test_wgmma_bits_gpu.py).  The input gradient
+// stays on mma.sync.  The per-sample interaction is tzk_interact_tc.cuh's.  The same source runs on the CPU under
+// tests/native/cuda_cpu_shim.h, sm90_cpu_emu.h and sm90_wgmma_emu.h (tests/test_interact_wide_fused.py,
+// tests/test_interact_wide_fwd_fused.py).
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -15,6 +19,7 @@
 #ifdef TZK_CPU_SHIM
 #include "cuda_cpu_shim.h"
 #include "sm90_cpu_emu.h"
+#include "sm90_wgmma_emu.h"
 typedef void* tzk_stream_t;
 #define TZK_REQUIRE(cond, ...) do { if (!(cond)) return 1; } while (0)
 #define TZK_CHECK_LAUNCH(name) do {} while (0)
@@ -31,6 +36,7 @@ namespace {
 #include "tzk_sm90_ptx.h"
 #endif
 #include "tzk_tma.h"
+#include "tzk_wgmma.cuh"
 namespace tzk_itc {      // what tzk_interact_tc.cuh expects from its includer
 __device__ __forceinline__ uint32_t cvt_tf32(float x) { return tf32_bits(x); }
 __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) { ::mma_tf32(c, a, b); }
@@ -51,9 +57,9 @@ __device__ __forceinline__ float4 load_l2(const float* p) {
 // Input gradient of the wide layer fused with the backward of the DLRM interaction that produced its input (DLRM-Criteo:
 // X = [351 pairs | 0 | dense 16 | sparse 416], 784 columns).  Per CTA of FB_M samples:
 //   1. dX[FB_M x 784] = dZ W, in chunks of 32 columns: dZ's fragments are split once and stay in registers (K = 64), W^T
-//      hi / lo chunks arrive by TMA through the stage ring.  The pass-through columns (352 ..) are stored straight into
-//      d_dense / d_sparse; the pair columns (0 .. 351) go to a shared-memory tile.  They run second so that the
-//      tile is complete when the ring drains.
+//      hi / lo chunks arrive by TMA through the stage ring; mma.sync m16n8k8 (m64n8k8 wgmma per warpgroup was slower,
+//      DESIGN §8).  The pass-through columns (352 ..) are stored straight into d_dense / d_sparse; the pair columns
+//      (0 .. 351) go to a shared-memory tile.  They run second so that the tile is complete when the ring drains.
 //   2. per sample, one warp: S from the pair columns, dE = S E + pass-through (tzk_itc::bwd_sample), the pass-through
 //      read back from d_dense / d_sparse (written by this CTA in step 1, so an L2 hit).
 // dX never reaches global memory.  The MMA order and the per-k-step accumulation are gemm3x_kernel's, so dX and with it
@@ -194,8 +200,9 @@ interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_whi, const __gr
 // | 0 | dense 16 | sparse 416], and the pair columns [M, 352] (column 351 zero) for the weight gradient.  X is never
 // written: 432 of its 784 columns are copies of dense / sparse.  Per CTA of FF_M samples (gemm3x_kernel<64>'s tile):
 //   1. per sample, one warp: the pairs (tzk_itc::fwd_sample) -> `pairs` in global memory (the rows stay in L2).
-//   2. gemm3x_kernel<64>'s k-loop over X's 25 chunks of 32 columns.  A comes by TMA: chunks 0 .. 10 from `pairs` (written
-//      by this CTA in step 1: proxy fence + barrier first), 12 .. 24 from `sparse` at column 32 c - 368.  Chunk 11
+//   2. gemm3x_kernel<64>'s k-loop over X's 25 chunks of 32 columns, on m64n64k8 wgmma.  A comes by TMA: chunks 0 .. 10
+//      from `pairs` (written by this CTA in step 1: proxy fence + barrier first), 12 .. 24 from `sparse` at column
+//      32 c - 368.  Chunk 11
 //      straddles dense 0 .. 15 | sparse 0 .. 15: a dense box in the stage and a sparse box (column 0) in the region
 //      that held step 1's staging rows; its k-steps 0, 1 read the first, 2, 3 the second.
 // The pair columns have to exist before the first k-step; the other CTA on the SM (two fit) keeps the tensor cores busy
@@ -292,25 +299,20 @@ interact_wide_fwd_kernel(const __grid_constant__ CUtensorMap map_pairs, const __
   if (threadIdx.x == 0)
     for (int c = 0; c < FF_STAGES; ++c) load(c);
 
-  // 2. gemm3x_kernel<64>: rows r and r + 8 of the tile, all 64 columns
+  // 2. gemm3x_kernel<64>'s k-steps on wgmma: warpgroup w / 4 takes rows 64 (w / 4) .., m64n64k8 with A = X hi / lo from
+  // registers (rows r and r + 8 of the tile) and B = the W hi / lo boxes
   const int r = warp * 16 + g;
-  float acc[8][4], part[8][4];
+  float acc[32], part[32];
 #pragma unroll
-  for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) acc[nt][q] = 0.f;
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
   for (int c = 0; c < FB_CHUNKS; ++c) {
     const int s = c % FF_STAGES;
     mbar_wait(full + s, (uint32_t)(c / FF_STAGES) & 1u);
     const float* xs = reinterpret_cast<const float*>(smem + s * FF_STAGE);
-    const uint32_t* whi = reinterpret_cast<const uint32_t*>(smem + s * FF_STAGE + FF_X_BYTES);
-    const uint32_t* wlo = whi + FF_W_BYTES / 4;
+    const uint8_t* whi = smem + s * FF_STAGE + FF_X_BYTES;
+    const uint8_t* wlo = whi + FF_W_BYTES;
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) part[nt][q] = 0.f;
       const int k0 = ks * 8 + t, k1 = k0 + 4;
       // chunk 11, k-steps 2 and 3: X column 368 + j = sparse column j of the second box.  With k = 16 + j the 16-B
       // chunk index of k is j's with bit 2 set, so swz(., j) = swz(., k) ^ 16.
@@ -324,24 +326,20 @@ interact_wide_fwd_kernel(const __grid_constant__ CUtensorMap map_pairs, const __
         ah[i] = tf32_bits(a[i]);
         al[i] = tf32_bits(a[i] - __uint_as_float(ah[i]));
       }
+      wgmma_fence();
+      wgmma_3xtf32<64>(part, ah, al, wgmma_desc(whi, ks), wgmma_desc(wlo, ks));
+      wgmma_commit();
+      wgmma_wait<0>();
 #pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        const int n = nt * 8 + g;
-        const uint32_t bh[2] = {whi[swz(n, k0)], whi[swz(n, k1)]};
-        const uint32_t bl[2] = {wlo[swz(n, k0)], wlo[swz(n, k1)]};
-        mma_tf32(part[nt], al, bh);               // small terms first
-        mma_tf32(part[nt], ah, bl);
-        mma_tf32(part[nt], ah, bh);
+      for (int i = 0; i < 32; ++i) {
+        wgmma_reg_fence(part[i]);
+        acc[i] += part[i];
       }
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[nt][q] += part[nt][q];
     }
-    __syncthreads();                              // every warp is done with stage s: refill it
+    __syncthreads();                              // every warpgroup is done with stage s: refill it
     if (threadIdx.x == 0 && c + FF_STAGES < FB_CHUNKS) load(c + FF_STAGES);
   }
-  // c0/c1: row r, columns 2t, 2t+1 of the n8 tile; c2/c3: row r + 8
+  // acc[4 nt + q], q = 0/1: row r, columns 2t, 2t+1 of the n8 tile nt; q = 2/3: row r + 8
 #pragma unroll
   for (int nt = 0; nt < 8; ++nt) {
     const int col = nt * 8 + 2 * t;
@@ -350,7 +348,7 @@ interact_wide_fwd_kernel(const __grid_constant__ CUtensorMap map_pairs, const __
     for (int h = 0; h < 2; ++h) {
       const int64_t row = m0 + r + 8 * h;
       if (row >= p.M) continue;
-      float2 o = make_float2(acc[nt][2 * h] + b0, acc[nt][2 * h + 1] + b1);
+      float2 o = make_float2(acc[4 * nt + 2 * h] + b0, acc[4 * nt + 2 * h + 1] + b1);
       o.x = fmaxf(o.x, 0.f);
       o.y = fmaxf(o.y, 0.f);
       *reinterpret_cast<float2*>(p.y + row * p.ld_y + col) = o;
@@ -370,7 +368,122 @@ __global__ void split_w_kernel(const float* __restrict__ w, int64_t ld_w, int K,
   }
 }
 
-#include "tzk_wgrad3x.cuh"   // wgrad3x_kernel, wgrad_reduce_kernel
+#include "tzk_wgrad3x.cuh"   // the work items, partial layout, wgrad_reduce_kernel and launch of the weight gradient
+
+// ======================================================================================================================
+// The weight gradient of the fused layer: wgrad3x_kernel's work items, stages and partial layout, its k-steps on wgmma.
+// TF32 wgmma takes B only K-major from shared memory and both operands arrive batch-major, so the roles swap: the
+// warpgroups compute dW^T = X^T dZ, warpgroup w / 4 on X columns 64 (w / 4) .. of the tile (m64n64k8), A = X^T read from
+// the boxes and split in registers, B = dZ^T hi / lo that the warps write per chunk, transposed, into two K-major
+// SWIZZLE_128B boxes [64 n x 32 batch rows].  The products of a k-step are gemm3x's in its order, dZ lo X hi, dZ hi X lo,
+// dZ hi X hi, and the partial block is stored as wgrad3x_kernel stores it, so dW keeps its bits.
+constexpr int WW_ZT = 64 * 128;                     // one dZ^T box: 64 n rows x 32 batch rows = 8 KB
+
+__global__ void __launch_bounds__(WG_THREADS, 2)
+interact_wide_wgrad_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant__ CUtensorMap map_x1,
+                           const __grid_constant__ CUtensorMap map_x2, const __grid_constant__ CUtensorMap map_dz,
+                           WgParams p) {
+  TZK_DYN_SMEM(uint8_t, smem);
+  uint8_t* zt = smem + WG_STAGES * WG_STAGE;              // dZ^T hi | lo (1024-B aligned)
+  uint64_t* full = reinterpret_cast<uint64_t*>(zt + 2 * WW_ZT);
+  int* boxes = reinterpret_cast<int*>(full + WG_STAGES);  // as in wgrad3x_kernel
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int jt = blockIdx.x % p.k_tiles;
+  const int64_t slab = blockIdx.x / p.k_tiles;
+  const int64_t row0 = slab * p.slab_rows;
+  const int64_t rows = (p.M - row0 < p.slab_rows) ? p.M - row0 : p.slab_rows;
+  const int num_c = (int)((rows + WG_ROWS - 1) / WG_ROWS);  // rows past M are zero-filled by the TMA
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < WG_STAGES; ++s) mbar_init(full + s, 1);
+    fence_mbarrier_init();
+    for (int b = 0; b < 4; ++b) {
+      const int box = jt * 4 + b, s = wg_source(p.src, box);
+      boxes[b] = s;
+      boxes[4 + b] = wg_pick(p.src.col0, s) + 32 * (box - wg_pick(p.src.first, s));
+    }
+  }
+  __syncthreads();
+  auto load = [&](int c) {                                // thread 0 only
+    uint8_t* sb = smem + (c % WG_STAGES) * WG_STAGE;
+    uint64_t* bar = full + c % WG_STAGES;
+    const int r = (int)(row0 + (int64_t)c * WG_ROWS);
+    mbar_expect_tx(bar, WG_A + WG_B);
+#pragma unroll 1
+    for (int b = 0; b < 4; ++b) {
+      const int s = *reinterpret_cast<volatile int*>(boxes + b), col = *reinterpret_cast<volatile int*>(boxes + 4 + b);
+      tma_load_2d(sb + b * WG_BOX, s == 0 ? &map_x0 : s == 1 ? &map_x1 : &map_x2, bar, col, r);
+    }
+#pragma unroll
+    for (int b = 0; b < 2; ++b) tma_load_2d(sb + WG_A + b * WG_BOX, &map_dz, bar, b * 32, r);
+  };
+  if (threadIdx.x == 0)
+    for (int c = 0; c < WG_STAGES && c < num_c; ++c) load(c);
+
+  const int xc = (warp >> 2) * 64 + (warp & 3) * 16 + g; // this lane's A rows: X columns xc and xc + 8 of the tile
+  const int tn = threadIdx.x & 63, tq = threadIdx.x >> 6; // transpose: n row tn, batch rows 4 tq .. and 16 + 4 tq ..
+  uint32_t* zhi = reinterpret_cast<uint32_t*>(zt);
+  uint32_t* zlo = zhi + WW_ZT / 4;
+  float acc[32], part[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  for (int c = 0; c < num_c; ++c) {
+    const int s = c % WG_STAGES;
+    mbar_wait(full + s, (uint32_t)(c / WG_STAGES) & 1u);
+    const float* xs = reinterpret_cast<const float*>(smem + s * WG_STAGE);
+    const float* zs = reinterpret_cast<const float*>(smem + s * WG_STAGE + WG_A);
+    auto at = [](const float* base, int m, int col) { return base[(col >> 5) * (WG_BOX / 4) + swz(m, col & 31)]; };
+    // dZ^T (n, m) at swz(n, m): 16-B stores, the 8 lanes of a quarter-warp on the 8 chunks of a swizzle row group
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = 4 * tq + 16 * h;
+      float hi[4], lo[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float v = at(zs, m + j, tn);
+        hi[j] = tf32_rna(v);
+        lo[j] = tf32_rna(v - hi[j]);
+      }
+      *reinterpret_cast<float4*>(zhi + swz(tn, m)) = make_float4(hi[0], hi[1], hi[2], hi[3]);
+      *reinterpret_cast<float4*>(zlo + swz(tn, m)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+    }
+    fence_proxy_async();                                  // the generic stores before wgmma's reads
+    __syncthreads();
+#pragma unroll
+    for (int ks = 0; ks < WG_ROWS / 8; ++ks) {
+      const int m = ks * 8 + t;                           // batch rows m (a0, a1) and m + 4 (a2, a3)
+      const float a[4] = {at(xs, m, xc), at(xs, m, xc + 8), at(xs, m + 4, xc), at(xs, m + 4, xc + 8)};
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        ah[i] = tf32_bits(a[i]);
+        al[i] = tf32_bits(a[i] - __uint_as_float(ah[i]));
+      }
+      wgmma_fence();
+      wgmma_tf32<64>(part, ah, wgmma_desc(zlo, ks), false);
+      wgmma_tf32<64>(part, al, wgmma_desc(zhi, ks), true);
+      wgmma_tf32<64>(part, ah, wgmma_desc(zhi, ks), true);
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        wgmma_reg_fence(part[i]);
+        acc[i] += part[i];
+      }
+    }
+    __syncthreads();                                      // stage s and the dZ^T boxes are free
+    if (threadIdx.x == 0 && c + WG_STAGES < num_c) load(c + WG_STAGES);
+  }
+  // acc[4 i + q]: X column xc + 8 (q / 2), n = 8 i + 2 t + q % 2
+  float* out = p.partial + ((int64_t)slab * p.k_tiles + jt) * 128 * 64;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(out + (int64_t)(xc + 8 * h) * 64 + 8 * i + 2 * t) =
+          make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+}
 
 // W^T hi / lo [K, 64] from W [64, ld_w] (K columns used)
 __global__ void split_wt_kernel(const float* __restrict__ w, int64_t ld_w, int K, float* __restrict__ hi,
@@ -472,7 +585,8 @@ extern "C" int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const flo
   // past the tensor: zeros, never written): dense -> 352 .. 367
   const WgSources src = {{0, FB_PAIR_CHUNKS, FB_CHUNKS - 1, FB_CHUNKS}, {0, 0, 0}, {0, FF_SPARSE0, tzk_itc::kInter},
                          {tzk_itc::kInter, tzk_itc::kRow - FF_SPARSE0, tzk_itc::kD}};
-  TZK_REQUIRE(wgrad3x_launch(mx, mz, src, M, slabs, partial, dw, ld_dw, reinterpret_cast<cudaStream_t>(stream)) == 0,
+  TZK_REQUIRE(wgrad3x_launch<interact_wide_wgrad_kernel>(mx, mz, src, M, slabs, partial, dw, ld_dw,
+                                                         reinterpret_cast<cudaStream_t>(stream), 2 * WW_ZT) == 0,
               "interact_wide_wgrad: launch failed");
   return 0;
 }

@@ -1,8 +1,9 @@
 // tzk_wgrad3x.cuh — the weight gradient of the wide tower layer,  dW[n, k] = sum_m dZ[m, n] * X[m, k]  (n < 64, m < M =
 // batch), on mma.sync m16n8k8 with the 3xTF32 split.  Shared by tzk_gemm3x.cu (tzk_wgrad3x: X is one tensor) and
 // tzk_interact_wide.cu (tzk_interact_wide_wgrad: X = [pairs | dense | sparse] of DLRM-Criteo's interaction, never
-// materialised).  Included inside the includer's anonymous namespace after tzk_sm90_ptx.h (or sm90_cpu_emu.h) and
-// tzk_tma.h; the includer provides TZK_DYN_SMEM / TZK_LAUNCH.
+// materialised; its own wgmma kernel on these work items, partials and reduction).  Included inside the includer's
+// anonymous namespace after tzk_sm90_ptx.h (or sm90_cpu_emu.h) and tzk_tma.h; the includer provides TZK_DYN_SMEM /
+// TZK_LAUNCH.
 //
 // X is read as 32-column TMA boxes.  Box b belongs to source s (first[s] <= b < first[s + 1]) and covers its columns
 // col0[s] + 32 (b - first[s]) ..; its dW columns are dst[s] + 32 (b - first[s]) .., those below width[s] are written.
@@ -162,9 +163,12 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int slabs
 }
 
 // dw (columns as `src` maps them) = dz[M, 64]^T @ X, X given by up to WG_SRC tensor maps of [rows x 32] boxes
-// (WG_ROWS rows); partial: slabs * k_tiles * 128 * 64 floats, k_tiles = ceil(src.first[WG_SRC] / 4).
+// (WG_ROWS rows); partial: slabs * k_tiles * 128 * 64 floats, k_tiles = ceil(src.first[WG_SRC] / 4).  Kernel: one with
+// wgrad3x_kernel's parameters, work items and partial layout, using `extra_smem` bytes past the stages.
+template <auto Kernel = wgrad3x_kernel>
 inline int wgrad3x_launch(const CUtensorMap (&mx)[WG_SRC], const CUtensorMap& mz, const WgSources& src, int64_t M,
-                          int32_t slabs, float* partial, float* dw, int64_t ld_dw, cudaStream_t st) {
+                          int32_t slabs, float* partial, float* dw, int64_t ld_dw, cudaStream_t st,
+                          size_t extra_smem = 0) {
   WgParams p;
   p.partial = partial;
   p.M = M;
@@ -172,15 +176,15 @@ inline int wgrad3x_launch(const CUtensorMap (&mx)[WG_SRC], const CUtensorMap& mz
   p.slab_rows = ((M + slabs - 1) / slabs + WG_ROWS - 1) / WG_ROWS * WG_ROWS;
   p.src = src;
   const int used = (int)((M + p.slab_rows - 1) / p.slab_rows);           // slabs that hold rows (<= slabs)
-  const size_t smem = (size_t)WG_STAGES * WG_STAGE + WG_STAGES * 8 + 8 * 4;
+  const size_t smem = (size_t)WG_STAGES * WG_STAGE + extra_smem + WG_STAGES * 8 + 8 * 4;
 #ifndef TZK_CPU_SHIM
   static bool configured = false;     // once: nothing but the launches happens inside a stream capture
   if (!configured) {
-    cudaFuncSetAttribute(wgrad3x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     configured = true;
   }
 #endif
-  TZK_LAUNCH((wgrad3x_kernel), used * p.k_tiles, WG_THREADS, smem, st, mx[0], mx[1], mx[2], mz, p);
+  TZK_LAUNCH((Kernel), used * p.k_tiles, WG_THREADS, smem, st, mx[0], mx[1], mx[2], mz, p);
   TZK_LAUNCH((wgrad_reduce_kernel), (p.k_tiles * 128 * 64 + 255) / 256, 256, 0, st, partial, used, p.k_tiles * 128, src,
              dw, ld_dw);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
