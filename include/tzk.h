@@ -523,6 +523,16 @@ int tzk_dot_interact27_bwd_bf16(const uint16_t* d_out, int64_t ld_dout, const ui
                                 const float* sparse, int64_t ld_sparse, int64_t B, uint16_t* d_dense, int64_t ld_ddense,
                                 float* d_sparse, int64_t ld_dsparse, tzk_stream_t stream);
 
+/* ---- evaluation metrics (csrc/tzk_metrics.cuh) --------------------------------------------------------------------
+ * binned_auc_update: the update of torchmetrics.AUROC(task="binary", thresholds=T) (tzrec/models/rank_model.py:392-398,
+ * `_binary_precision_recall_curve_update_vectorized`) as a histogram.  For i < n with label y in {0, 1} and p in [0, 1]:
+ *     counts[bin(p) * 2 + y] += 1,  bin(p) = #{k < T : p >= thresholds[k]}  (0..T; thresholds nondecreasing);
+ * any other sample (label outside {0, 1}, p NaN or outside [0, 1]) adds 1 to *invalid instead.  counts is int64
+ * [(T + 1) * 2] and is accumulated into, never cleared.  preds: pred_dtype 0 = fp32, 1 = bf16 (16-bit patterns);
+ * labels: label_dtype 0 = fp32, 1 = int64.  Deterministic (integer atomics).  n = 0 launches nothing. */
+int tzk_binned_auc_update(const void* preds, int32_t pred_dtype, const void* labels, int32_t label_dtype, int64_t n,
+                          const float* thresholds, int32_t T, int64_t* counts, int64_t* invalid, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

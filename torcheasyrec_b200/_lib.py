@@ -150,6 +150,7 @@ SIGNATURES = {
     "tzk_dot_interact27_fwd_bf16": (c_int32, [P, c_int64, P, c_int64, c_int64, P, c_int64, P]),
     "tzk_dot_interact27_bwd_bf16": (
         c_int32, [P, c_int64, P, c_int64, P, c_int64, c_int64, P, c_int64, P, c_int64, P]),
+    "tzk_binned_auc_update": (c_int32, [P, c_int32, P, c_int32, c_int64, P, c_int32, P, P, P]),
 }
 
 _lib = None

@@ -1,4 +1,4 @@
-"""Step driver: builds a model from a tzrec pipeline config and runs train steps on one H100.
+"""Step driver: builds a model from a tzrec pipeline config and runs train steps (and forward-only eval steps) on one H100.
 
 Replaces the part of tzrec/main.py that surrounds the hot path (model construction :763-781, optimizers
 :814-876, the step loop :519-547) and torchrec's TrainPipelineSparseDist (tzrec/utils/dist_util.py:221-303)
@@ -8,8 +8,9 @@ replayed; a side stream stages the next host batch (pinned H2D) while the curren
 Variable-shape workloads (sequence features) run the same code eagerly.
 """
 
+import contextlib
 import os
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, Iterable, List, Optional, Sequence
 
 import torch
 
@@ -58,6 +59,9 @@ class Pipeline:
         if max_rows:
             override_num_buckets(self.cfg, max_rows)
         self.device = torch.device(device)
+        self.capturable = capturable
+        # process group whose ranks' metric states compute_metric sums (sharded pipelines; None = the default group)
+        self.metric_group = group
         self.features: List[BaseFeature] = create_features(list(self.cfg.feature_configs),
                                                            fg_mode=self.cfg.data_config.fg_mode)
         self.labels = list(self.cfg.data_config.label_fields)
@@ -169,6 +173,90 @@ class Pipeline:
         for m in self.sharded:
             m.check_overflow()
 
+    # ---- evaluation (tzrec/main.py:169-233 `_evaluate`) -------------------------------------------------------------
+    def _ensure_metrics(self) -> None:
+        if getattr(self.model, "_metric_modules", None) is None:
+            self.model.init_metric(process_group=self.metric_group, distributed=bool(self.sharded))
+
+    @contextlib.contextmanager
+    def _eval_mode(self):
+        """model.eval() and no_grad for the block; the model's previous mode comes back even if the block raises."""
+        was_training = self.model.training
+        self.model.eval()
+        try:
+            with torch.no_grad():
+                yield
+        finally:
+            self.model.train(was_training)
+
+    def _check_eval_batch(self, batch: Batch) -> None:
+        """The peer exchange is sized for the local batch of its first step: an eval batch larger than that is refused
+        here, before anything is launched (a smaller one, e.g. the last of an eval set, is gathered at its own size)."""
+        B = next(iter(batch.labels.values())).shape[0]
+        for sm in self.sharded:
+            for st in getattr(sm, "_peer_states", None) or []:
+                if B > st.B:
+                    raise ValueError(f"eval batch of {B} samples: the peer exchange is sized for local batches of at "
+                                     f"most {st.B} (the training batch); split the eval set into batches of that size")
+
+    def _eval_body(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        """Forward through train_wrapper (autocast as in training) + update_metric; the caller holds _eval_mode."""
+        _, (losses, predictions, _) = self.train_wrapper(batch)
+        self.model.update_metric(predictions, batch, {k: v.detach() for k, v in losses.items()})
+        return predictions
+
+    def eval_step(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        """One eager forward-only step under model.eval() and no_grad: adds `batch` to the metric states and returns the
+        predictions."""
+        self._ensure_metrics()
+        self._check_eval_batch(batch)
+        with self._eval_mode():
+            return self._eval_body(batch)
+
+    def evaluate(self, batches: Iterable[Batch], num_steps: Optional[int] = None) -> Dict[str, float]:
+        """Runs `num_steps` eval steps (default eval_config.num_steps; every batch when it is unset or <= 0), then returns
+        {metric name: value} and resets the metric states.  On CUDA with `capturable`, batches shaped like the first one
+        replay a GraphedEvalStep (one per batch shape, kept for later evaluations); any other batch, e.g. a shorter last
+        one, takes the eager eval_step, and so does every batch of a model with sequence features.  The model's train /
+        eval mode is restored afterwards."""
+        if num_steps is None:
+            num_steps = int(self.cfg.eval_config.num_steps)
+        if num_steps <= 0:                 # as main.py:187: unset or 0 evaluates every batch
+            num_steps = None
+        self._ensure_metrics()
+        # captured graphs update the metric state tensors they were captured with: a new init_metric drops them
+        mods = self.model._metric_modules
+        cache = self.__dict__.get("_eval_graphs")
+        if cache is None or cache[0] is not mods:
+            cache = self._eval_graphs = (mods, {})
+        graphs = cache[1]
+        graph = None
+        # sequence features vary in shape from batch to batch: those models step eagerly, as in training
+        graphable = self.device.type == "cuda" and self.capturable and not any(f.is_sequence for f in self.features)
+        try:
+            for i, batch in enumerate(batches):
+                if num_steps is not None and i >= num_steps:
+                    break
+                self._check_eval_batch(batch)
+                # (a capture needs the per-key id counts on the host: a device batch without them steps eagerly)
+                if graphable and all(k._length_per_key is not None or not k.lengths().is_cuda
+                                     for k in batch.sparse_features.values()):
+                    if graph is None:
+                        key = tuple(t.shape for t in _tensors_of(batch))
+                        graph = graphs.get(key)
+                        if graph is None or not graph.fits(batch):
+                            graph = graphs[key] = GraphedEvalStep(self, batch)
+                    if graph.fits(batch):
+                        graph.load(batch)
+                        graph.replay()
+                        continue
+                self.eval_step(batch.to(self.device))
+        except BaseException:
+            for m in self.model._metric_modules.values():
+                m.reset()
+            raise
+        return {k: float(v) for k, v in self.model.compute_metric().items()}
+
 
 def _tensors_of(batch: Batch) -> List[torch.Tensor]:
     out = []
@@ -184,33 +272,30 @@ def _tensors_of(batch: Batch) -> List[torch.Tensor]:
     return out
 
 
-class GraphedTrainStep:
-    """One CUDA graph per (model, batch shape).  `load()` refreshes the static inputs, `replay()` runs a step."""
+class _StaticFeed:
+    """Static device copies of one example batch (the inputs a captured step reads) and the feed that refreshes them."""
 
-    def __init__(self, pipe: Pipeline, example: Batch, warmup: int = 3) -> None:
+    def __init__(self, pipe: Pipeline, example: Batch) -> None:
         assert pipe.device.type == "cuda"
-        self.pipe = pipe
         self.static = example.to(pipe.device)
         for k, kjt in example.sparse_features.items():
             self.static.sparse_features[k]._length_per_key = kjt._length_per_key
         self._static_tensors = _tensors_of(self.static)
         self.copy_stream = torch.cuda.Stream()
         self._staging = None
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(warmup):
-                self._fresh_kjt_caches()
-                pipe.eager_step(self.static)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        if pipe.grad_sync is None:
-            pipe.dense_optimizer.zero_grad(set_to_none=True)
-        self._fresh_kjt_caches()
-        with torch.cuda.graph(self.graph):
-            self.loss = pipe.step_body(self.static)
-        torch.cuda.synchronize()
+
+    def fits(self, batch: Batch) -> bool:
+        """True when `batch` has the static inputs' shapes and per-key id counts, which a replay takes as given."""
+        if [t.shape for t in _tensors_of(batch)] != [t.shape for t in self._static_tensors]:
+            return False
+        for k, kjt in self.static.sparse_features.items():
+            other = batch.sparse_features[k]
+            lpk = other._length_per_key
+            if lpk is None and not other.lengths().is_cuda:
+                lpk = other.length_per_key()
+            if lpk is None or list(lpk) != list(kjt._length_per_key or []):
+                return False
+        return True
 
     def _fresh_kjt_caches(self) -> None:
         # offsets are derived data: recompute them from the (possibly refreshed) lengths inside every step
@@ -244,6 +329,64 @@ class GraphedTrainStep:
             dst.copy_(src, non_blocking=True)
         self._consumed.record(cur)
 
+
+class GraphedTrainStep(_StaticFeed):
+    """One CUDA graph per (model, batch shape).  `load()` refreshes the static inputs, `replay()` runs a step."""
+
+    def __init__(self, pipe: Pipeline, example: Batch, warmup: int = 3) -> None:
+        super().__init__(pipe, example)
+        self.pipe = pipe
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(warmup):
+                self._fresh_kjt_caches()
+                pipe.eager_step(self.static)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        if pipe.grad_sync is None:
+            pipe.dense_optimizer.zero_grad(set_to_none=True)
+        self._fresh_kjt_caches()
+        with torch.cuda.graph(self.graph):
+            self.loss = pipe.step_body(self.static)
+        torch.cuda.synchronize()
+
     def replay(self) -> torch.Tensor:
         self.graph.replay()
         return self.loss
+
+
+class GraphedEvalStep(_StaticFeed):
+    """Pipeline.eval_step captured in one CUDA graph: the forward and the metric update.  `load()` / `prefetch()` +
+    `commit()` refresh the static inputs as for GraphedTrainStep; `replay()` adds the loaded batch to the metric states
+    and returns the step's (static) predictions.  The warm-up steps' metric updates are undone.  The graph updates the
+    metric states that existed at capture: after another `model.init_metric()`, capture a new step.  It keeps no reference
+    to the pipeline, which caches it (Pipeline.evaluate): no cycle holds the graph's memory after the pipeline is gone."""
+
+    def __init__(self, pipe: Pipeline, example: Batch, warmup: int = 2) -> None:
+        from . import metrics
+
+        super().__init__(pipe, example)
+        pipe._ensure_metrics()
+        mods = pipe.model._metric_modules
+        saved = metrics.snapshot(mods)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(warmup):
+                self._fresh_kjt_caches()
+                pipe.eval_step(self.static)
+        torch.cuda.current_stream().wait_stream(side)
+        metrics.restore(mods, saved)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        self._fresh_kjt_caches()
+        with pipe._eval_mode():
+            with torch.cuda.graph(self.graph):
+                self.predictions = pipe._eval_body(self.static)
+        torch.cuda.synchronize()
+
+    def replay(self) -> Dict[str, torch.Tensor]:
+        self.graph.replay()
+        return self.predictions

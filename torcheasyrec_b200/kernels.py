@@ -1021,6 +1021,30 @@ class CudaKernels:
         return (out[o + 2 * N + 1], logits, dy1, out[:o].view(N, K), out[o:o + N], out[o + N:o + 2 * N].view(1, N),
                 out[o + 2 * N:o + 2 * N + 1])
 
+    def binned_auc_update(self, preds: torch.Tensor, labels: torch.Tensor, thresholds: torch.Tensor,
+                          counts: torch.Tensor, invalid: torch.Tensor) -> None:
+        """counts [T + 1, 2] int64 += the histogram of bin(p) = #{k : p >= thresholds[k]} by label; invalid [1] int64 +=
+        the samples with a label outside {0, 1} or a prediction NaN / outside [0, 1] (csrc/tzk_metrics.cuh).
+        preds fp32 or bf16, labels fp32 or int64, n of each; thresholds fp32 [T], nondecreasing (not checked here)."""
+        if preds.dtype not in (torch.float32, torch.bfloat16):
+            raise TzkError(f"binned_auc_update: predictions must be float32 or bfloat16, got {preds.dtype}")
+        if labels.dtype not in (torch.float32, torch.int64):
+            raise TzkError(f"binned_auc_update: labels must be float32 or int64, got {labels.dtype}")
+        _need(preds, preds.dtype, "preds")
+        _need(labels, labels.dtype, "labels")
+        _need(thresholds, torch.float32, "thresholds")
+        _need(counts, torch.int64, "counts")
+        _need(invalid, torch.int64, "invalid")
+        n, T = preds.numel(), thresholds.numel()
+        if labels.numel() != n:
+            raise TzkError(f"binned_auc_update: {n} predictions but {labels.numel()} labels")
+        if T < 1 or counts.numel() != 2 * (T + 1) or invalid.numel() != 1:
+            raise TzkError("binned_auc_update: counts must be [T + 1, 2] and invalid [1] for T >= 1 thresholds")
+        check(self._lib.tzk_binned_auc_update(_ptr(preds), int(preds.dtype == torch.bfloat16), _ptr(labels),
+                                              int(labels.dtype == torch.int64), n, _ptr(thresholds), T, _ptr(counts),
+                                              _ptr(invalid), _stream()), "tzk_binned_auc_update")
+        self.launches += int(n > 0)
+
 
 @dataclass
 class ColPlan:

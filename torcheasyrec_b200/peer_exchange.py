@@ -323,9 +323,15 @@ class PeerState(PeerBase):
         return psw
 
     # ---- forward ---------------------------------------------------------------------------------------------------
-    def gather(self, ids: torch.Tensor, offsets: torch.Tensor, psw: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """psw: the local batch's per-sample weights (weighted bags) or None."""
+    def gather(self, ids: torch.Tensor, offsets: torch.Tensor, psw: Optional[torch.Tensor] = None,
+               B: Optional[int] = None) -> torch.Tensor:
+        """psw: the local batch's per-sample weights (weighted bags) or None.  B: the local batch when it is smaller
+        than the one the exchange was sized for — only forward-only steps do that (the gather reads peer tables and
+        needs no other rank's counts; the wire buffers of the backward are sized for self.B)."""
         g, k = self.g, Fn.backend()
+        B = self.B if B is None else int(B)
+        if B > self.B:
+            raise RuntimeError(f"peer exchange is sized for local batches of {self.B} samples, got {B}")
         if ids.numel() > self.max_nnz:
             raise RuntimeError(f"peer exchange is sized for {self.max_nnz} ids per step, got {ids.numel()}")
         psw = self._weights(psw)
@@ -334,13 +340,13 @@ class PeerState(PeerBase):
         if sel is not None:
             # two launches over complementary feature lists: the one whose rows cross NVLink starts first, on its own
             # stream; the mirror refresh and the mirrored features' lookup run next to it
-            out = torch.empty((self.B, g.local.layout.total_dim), dtype=torch.float32, device=ids.device)
+            out = torch.empty((B, g.local.layout.total_dim), dtype=torch.float32, device=ids.device)
             gs = self._gather_stream()
             cur = torch.cuda.current_stream() if gs is not None else None
 
             def remote():
                 k.peer_pooled_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
-                                         g.local.layout, ids, offsets, self.B, self.W, out, self.mirror,
+                                         g.local.layout, ids, offsets, B, self.W, out, self.mirror,
                                          self.feat_mirror_off, feat_sel=sel[1], **wkw)
 
             if gs is not None:
@@ -351,7 +357,7 @@ class PeerState(PeerBase):
                 remote()
             k.peer_mirror_refresh(self.tables, self.W, *self._seg, self.mirror)
             k.peer_pooled_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
-                                     g.local.layout, ids, offsets, self.B, self.W, out, self.mirror, self.feat_mirror_off,
+                                     g.local.layout, ids, offsets, B, self.W, out, self.mirror, self.feat_mirror_off,
                                      feat_sel=sel[0], **wkw)
             if gs is not None:
                 cur.wait_stream(gs)
@@ -360,10 +366,10 @@ class PeerState(PeerBase):
             k.peer_mirror_refresh(self.tables, self.W, *self._seg, self.mirror)
         if self.pooled:
             return k.peer_pooled_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
-                                            g.local.layout, ids, offsets, self.B, self.W, None, self.mirror,
+                                            g.local.layout, ids, offsets, B, self.W, None, self.mirror,
                                             self.feat_mirror_off, **wkw)
         return k.peer_seq_gather_fwd(self.tables, self.rf_w_off, self.feat_rows, g.feat_block, g.feat_owner,
-                                     g.local.layout, ids, offsets, self.B, self.W, self.mirror, self.feat_mirror_off)
+                                     g.local.layout, ids, offsets, B, self.W, self.mirror, self.feat_mirror_off)
 
     def _split_lists(self):
         """(mirrored features, features whose rows live in the owners' arenas) as device int32 lists, or None when the
@@ -546,8 +552,8 @@ class _PeerLookup(torch.autograd.Function):
     """psw: the KJT's per-sample weights (weighted bags) or None; data, no gradient flows to them."""
 
     @staticmethod
-    def forward(ctx, hook, st: PeerState, ids, offsets, psw=None):
-        out = st.gather(ids, offsets, psw)
+    def forward(ctx, hook, st: PeerState, ids, offsets, psw=None, B=None):
+        out = st.gather(ids, offsets, psw, B)
         ctx.st = None
         if hook is not None:                  # (also with zero local ids: the barriers are collective)
             st.prep(ids, offsets, psw)
@@ -560,7 +566,7 @@ class _PeerLookup(torch.autograd.Function):
         if ctx.st is not None:
             (offsets,) = ctx.saved_tensors
             ctx.st.backward(Fn._rows_contig(grad_out) if ctx.st.pooled else grad_out.contiguous(), offsets)
-        return None, None, None, None, None
+        return None, None, None, None, None, None
 
 
 def enable_peer_exchange(sm, batch_size: int, ids_per_feature: Optional[Dict[str, int]] = None) -> List[PeerState]:
@@ -586,10 +592,13 @@ def enable_peer_exchange(sm, batch_size: int, ids_per_feature: Optional[Dict[str
         out = {}
         for g, st in zip(sm.groups, states):
             kjt = g.local._select(features)
-            if kjt.stride() != st.B:
+            hook = sm._hook_tensor(kjt.values().device)
+            # a training step must have the sized batch (the backward's wire layout); a forward-only step (evaluation)
+            # may be shorter, e.g. the last batch of an eval set
+            if kjt.stride() > st.B or (kjt.stride() != st.B and hook is not None):
                 raise RuntimeError(f"peer exchange was sized for batch {st.B}, got {kjt.stride()}")
-            res = _PeerLookup.apply(sm._hook_tensor(kjt.values().device), st, kjt.values(), kjt.offsets(),
-                                    kjt.weights_or_none() if pooled else None)
+            res = _PeerLookup.apply(hook, st, kjt.values(), kjt.offsets(), kjt.weights_or_none() if pooled else None,
+                                    kjt.stride())
             if pooled:
                 vals.append(res)
                 keys += g.embedding_names

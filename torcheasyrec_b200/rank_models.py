@@ -267,6 +267,52 @@ class RankModel(nn.Module):
 
         return {"binary_cross_entropy": bce_with_logits(predictions["logits"], label)}
 
+    # ---- evaluation metrics (rank_model.py:289-398, model.py:207-223): `auc` and the loss means --------------------
+    def _metric_heads(self):
+        """[(metric configs, loss configs, label name, name suffix)]: the model's own for single-task models."""
+        return [(list(self._base_model_config.metrics), list(self._base_model_config.losses), self._label_name, "")]
+
+    def init_metric(self, device=None, process_group=None, distributed: bool = False) -> None:
+        """One metric state per configured metric and loss, named as the reference names them.  `distributed`:
+        compute_metric first sums the states over `process_group` (None: the default group).  Only `auc` is
+        implemented; any other metric kind raises here, i.e. when evaluation is requested."""
+        from .metrics import BinnedAUC, MeanLoss
+
+        if device is None:
+            device = next(p.device for p in self.parameters() if p.device.type != "meta")
+        mods = {}
+        for metrics, losses, _, suffix in self._metric_heads():
+            for mc in metrics:
+                kind = mc.WhichOneof("metric")
+                if kind != "auc":
+                    raise NotImplementedError(f"metric {kind}{suffix}: only auc and the loss metrics are implemented")
+                mods[kind + suffix] = BinnedAUC(mc.auc.thresholds, device)
+            for lc in losses:
+                mods[lc.WhichOneof("loss") + suffix] = MeanLoss(device)
+        self._metric_modules = mods
+        self._metric_sync = (process_group, bool(distributed))
+
+    def update_metric(self, predictions: Dict[str, torch.Tensor], batch: Batch,
+                      losses: Optional[Dict[str, torch.Tensor]] = None) -> None:
+        """Adds one batch to every metric state (device work only, capturable)."""
+        mods = self._metric_modules
+        for metrics, loss_cfgs, label_name, suffix in self._metric_heads():
+            label = batch.labels[label_name]
+            for mc in metrics:
+                mods[mc.WhichOneof("metric") + suffix].update(predictions["probs" + suffix], label)
+            if losses is not None:
+                for lc in loss_cfgs:
+                    name = lc.WhichOneof("loss") + suffix
+                    mods[name].update(losses[name], label.size(0))
+
+    def compute_metric(self) -> Dict[str, torch.Tensor]:
+        """{name: value} of every metric (summed over the ranks first when distributed), then every state reset.
+        Raises ValueError when an auc saw labels outside {0, 1} or predictions outside [0, 1]."""
+        from .metrics import compute_all
+
+        group, distributed = self._metric_sync
+        return compute_all(self._metric_modules, group, distributed)
+
     def sparse_collections(self):
         return list(self.embedding_group.sparse_collections())
 
@@ -540,6 +586,10 @@ class MMoE(RankModel):
         for i, cfg in enumerate(self._task_tower_cfgs):
             preds.update(self._output_to_prediction(self._task_tower[i](task_inputs[i]), suffix=f"_{cfg.tower_name}"))
         return preds
+
+    def _metric_heads(self):
+        """multi_task_rank.py:144-196: per task tower, its metrics and losses on its label, suffixed `_<tower_name>`."""
+        return [(list(c.metrics), list(c.losses), c.label_name, f"_{c.tower_name}") for c in self._task_tower_cfgs]
 
     def loss(self, predictions, batch):
         from .dense_gemm import bce_with_logits
