@@ -140,7 +140,8 @@ int tzk_seq_gather_fwd_strided(const float* weights, const int64_t* feat_w_off, 
 
 /* ---- FP16 tables (tzrec/protos/feature.proto `data_type = "FP16"` -> EmbeddingBagConfig.data_type, features/feature.py:
  * 626,652): the same lookups over an arena of IEEE halfs; pooling and outputs stay fp32.  The fused backward takes such
- * an arena through tzk_opt_args.weights_f16 (the _ex entry points); optimizer state stays fp32. */
+ * an arena through tzk_opt_args.weights_f16 (the _ex entry points); optimizer state stays fp32.  Sharded collections
+ * keep their shards as halfs too: the peer step's _f16 entry points at the end of this header. */
 int tzk_pooled_gather_fwd_f16(const void* weights, const int64_t* feat_w_off, const int64_t* feat_rows,
                               const int32_t* feat_dim, const int32_t* feat_col, const int32_t* feat_pool,
                               const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B, int32_t max_dim,
@@ -532,6 +533,44 @@ int tzk_dot_interact27_bwd_bf16(const uint16_t* d_out, int64_t ld_dout, const ui
  * labels: label_dtype 0 = fp32, 1 = int64.  Deterministic (integer atomics).  n = 0 launches nothing. */
 int tzk_binned_auc_update(const void* preds, int32_t pred_dtype, const void* labels, int32_t label_dtype, int64_t n,
                           const float* thresholds, int32_t T, int64_t* counts, int64_t* invalid, tzk_stream_t stream);
+
+/* ---- FP16 tables on the peer step: every rank's arena (table_ptrs) and the local mirror hold IEEE halfs; everything
+ * else — outputs, gradients on the wire, receive buffers, published gradients, partial sums, optimizer state — stays
+ * fp32.  Arguments as in the fp32 entry points above; dims must be multiples of 4 (rows 8-B aligned).
+ *   peer_pooled_gather_fwd_f16 / _sel_f16 / _weighted_f16, peer_seq_gather_fwd_f16: every row (owner arena or mirror)
+ *                            is read with a coherent 8-B load and widened exactly; pooling as tzk_pooled_gather_fwd_f16,
+ *                            tzk_pooled_gather_fwd_weighted (weights_f16 = 1) and tzk_seq_gather_fwd_f16 — the same bits.
+ *   peer_mirror_refresh_f16: segments counted in halfs (multiples of 4), copied bit for bit in 8-B vectors.
+ * The owner-side updates take a half arena through tzk_opt_args.weights_f16: tzk_fused_bwd_apply_peer (pull transport),
+ * tzk_fused_bwd_apply_ex over the receive buffer (push) and tzk_peer_small_update widen the row, update in fp32 and
+ * round back to nearest even. */
+int tzk_peer_pooled_gather_fwd_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
+                                   const int64_t* feat_block, const int32_t* feat_owner, const int32_t* feat_dim,
+                                   const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
+                                   const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t max_dim, float* out,
+                                   int64_t ld_out, const void* mirror, const int64_t* feat_mirror_off,
+                                   tzk_stream_t stream);
+int tzk_peer_pooled_gather_fwd_sel_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
+                                       const int64_t* feat_block, const int32_t* feat_owner, const int32_t* feat_dim,
+                                       const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
+                                       const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t max_dim,
+                                       float* out, int64_t ld_out, const void* mirror, const int64_t* feat_mirror_off,
+                                       const int32_t* feat_sel, int32_t n_sel, tzk_stream_t stream);
+int tzk_peer_pooled_gather_fwd_weighted_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off,
+                                            const int64_t* feat_rows, const int64_t* feat_block,
+                                            const int32_t* feat_owner, const int32_t* feat_dim, const int32_t* feat_col,
+                                            const int32_t* feat_pool, const int64_t* ids, const int64_t* offsets,
+                                            int32_t F, int32_t B, int32_t W, int32_t max_dim, float* out, int64_t ld_out,
+                                            const void* mirror, const int64_t* feat_mirror_off,
+                                            const float* per_sample_weights, const int32_t* feat_sel, int32_t n_sel,
+                                            tzk_stream_t stream);
+int tzk_peer_seq_gather_fwd_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
+                                const int64_t* feat_block, const int32_t* feat_owner, const int64_t* ids,
+                                const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t D, int64_t nnz,
+                                float* out, const void* mirror, const int64_t* feat_mirror_off, tzk_stream_t stream);
+int tzk_peer_mirror_refresh_f16(const uint64_t* table_ptrs, int32_t W, const int32_t* seg_rank, const int64_t* seg_src,
+                                const int64_t* seg_dst, const int64_t* seg_n, int32_t n_seg, void* mirror,
+                                tzk_stream_t stream);
 
 #ifdef __cplusplus
 }

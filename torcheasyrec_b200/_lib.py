@@ -151,6 +151,16 @@ SIGNATURES = {
     "tzk_dot_interact27_bwd_bf16": (
         c_int32, [P, c_int64, P, c_int64, P, c_int64, c_int64, P, c_int64, P, c_int64, P]),
     "tzk_binned_auc_update": (c_int32, [P, c_int32, P, c_int32, c_int64, P, c_int32, P, P, P]),
+    # FP16 tables on the peer step: the fp32 entry points' arguments, arenas and mirror of halfs
+    "tzk_peer_pooled_gather_fwd_f16": (
+        c_int32, [P, P, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, P, c_int64, P, P, P]),
+    "tzk_peer_pooled_gather_fwd_sel_f16": (
+        c_int32, [P, P, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, P, c_int64, P, P, P, c_int32, P]),
+    "tzk_peer_pooled_gather_fwd_weighted_f16": (
+        c_int32, [P, P, P, P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, P, c_int64, P, P, P, P, c_int32, P]),
+    "tzk_peer_seq_gather_fwd_f16": (
+        c_int32, [P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, c_int64, P, P, P, P]),
+    "tzk_peer_mirror_refresh_f16": (c_int32, [P, c_int32, P, P, P, P, c_int32, P, P]),
 }
 
 _lib = None

@@ -157,12 +157,29 @@ def save_model(checkpoint_dir: str, model, dense_optimizer: Optional[torch.optim
             json.dump(plan_json(model), f)
 
 
+def _check_dtypes(sd: Dict[str, object], path: str) -> None:
+    """Tables are saved in their data_type (FP16 tables as fp16 tensors).  Loading a checkpoint into a model whose table
+    has the other data_type would convert every row silently: raise instead, before anything is read."""
+    import torch.distributed.checkpoint as dcp
+
+    meta = dcp.FileSystemReader(path).read_metadata().state_dict_metadata
+    bad = []
+    for k, v in sd.items():
+        props = getattr(meta.get(k), "properties", None)
+        if isinstance(v, torch.Tensor) and props is not None and props.dtype != v.dtype:
+            bad.append(f"{k} (checkpoint {props.dtype}, model {v.dtype})")
+    if bad:
+        raise ValueError("checkpoint and model disagree on the tables' data_type (FP32 / FP16); loading across "
+                         "data_type is not supported: " + ", ".join(bad))
+
+
 def restore_model(checkpoint_dir: str, model, dense_optimizer: Optional[torch.optim.Optimizer] = None, group=None) -> None:
     """checkpoint_util.restore_model: loads `<dir>/model` (+ `<dir>/optimizer`) into the CURRENT sharding — DCP
     re-shards by chunk metadata, so world size and plan may differ from the run that saved."""
     import torch.distributed.checkpoint as dcp
 
     sd = dict(model.state_dict())            # table entries view the arenas: DCP writes straight into the shards
+    _check_dtypes(sd, os.path.join(checkpoint_dir, "model"))
     dcp.load(sd, checkpoint_id=os.path.join(checkpoint_dir, "model"), process_group=group)
     model.load_state_dict(sd)
     opt_dir = os.path.join(checkpoint_dir, "optimizer")

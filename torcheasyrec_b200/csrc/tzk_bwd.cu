@@ -1890,8 +1890,8 @@ extern "C" int tzk_peer_small_update(const tzk_opt_args* opt, const uint64_t* ps
   if (n_tabs == 0 || total_rows == 0) return 0;
   TZK_REQUIRE(tabs && weights && max_dim >= 4 && max_dim <= 128 && max_dim % 4 == 0 && n_tabs <= 1024,
               "peer_small_update: dims must be multiples of 4 and <= 128");
-  TZK_REQUIRE(opt->optimizer >= 0 && opt->optimizer <= TZK_OPT_LARS_SGD && !opt->weights_f16,
-              "peer_small_update: unsupported optimizer");
+  TZK_REQUIRE(opt->optimizer >= 0 && opt->optimizer <= TZK_OPT_LARS_SGD, "peer_small_update: unsupported optimizer");
+  TZK_REQUIRE(!opt->weights_f16 || !opt->interleaved, "peer_small_update: interleaved rows are fp32");
   TZK_REQUIRE(opt->optimizer == TZK_OPT_SGD || opt->state, "peer_small_update: optimizer state is NULL");
   TZK_REQUIRE(opt->per_sample_weights == nullptr, "peer_small_update: weighted bags are not supported on the peer step");
   TZK_REQUIRE(!norm_family(*opt) || !opt->interleaved, "peer_small_update: interleaved rows are Adagrad only");
@@ -1904,7 +1904,9 @@ extern "C" int tzk_peer_small_update(const tzk_opt_args* opt, const uint64_t* ps
   a.lr = opt->lr; a.eps = opt->eps; a.grad_scale = 1.f; a.F = 0; a.B = 1; a.optimizer = opt->optimizer; a.pooled = 0;
   a.n = total_rows; a.sentinel = 0; a.state2 = opt->state2; a.step = opt->step; a.beta1 = opt->beta1; a.beta2 = opt->beta2;
   a.weight_decay = opt->weight_decay; a.max_gradient = opt->max_gradient; a.bc1 = a.bc2 = 1.f;
-  a.peer_w = 0; a.idx_span = 1; a.w_f16 = 0; a.interleaved = opt->interleaved ? 1 : 0;
+  // weights_f16: the owner widens its half row, adds the W fp32 partial sums in rank order, updates in fp32 and rounds
+  // the row back to nearest even (finish_run's FP16 path)
+  a.peer_w = 0; a.idx_span = 1; a.w_f16 = opt->weights_f16 ? 1 : 0; a.interleaved = opt->interleaved ? 1 : 0;
   a.div_b = make_fast_div(1); a.div_span = make_fast_div(1); a.ld32 = 0; a.wd_mode = opt->weight_decay_mode;
   if (opt->optimizer == TZK_OPT_LARS_SGD) { a.beta1 = opt->momentum; a.beta2 = opt->eta; }
   const bool norm = norm_family(*opt);

@@ -25,12 +25,18 @@
 //   weighted  (per-sample weights of weighted id features; pooled, push transport) the weights never leave the sample's
 //             rank: the gather pools w * row, the scatter records each wire slot's weight in a local buffer, the push
 //             sends w * g (/ L).  Each weighted kernel is the unweighted one's body with a compile-time switch.
+//   FP16      (data_type = FP16 tables) the arenas and the mirror hold halfs; the gathers widen every row to fp32 and pool
+//             exactly as the unsharded f16 lookups do, the mirror refresh copies the halfs' bits.  Gradients on the wire,
+//             the partial sums and the optimizer state stay fp32 (the owner's update rounds the row back, tzk_bwd.cu).
+//             Each _f16 kernel is the fp32 one's body instantiated for the table type TT = __half.
 //
 // This file compiles for the host too (TZK_CPU_SHIM, tests/test_peer_exchange_model.py runs the kernels' source on
 // std::threads), so it uses plain CUDA + warp shuffles only; the barrier (PTX) is excluded from that build.
 #ifdef TZK_CPU_SHIM
 #include "cuda_cpu_shim.h"
+#include "half_cpu_shim.h"
 #else
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
 #define TZK_UNPAREN(...) __VA_ARGS__
@@ -38,6 +44,8 @@
 #endif
 #include <stdint.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 namespace {
 
@@ -67,6 +75,42 @@ __device__ __forceinline__ float4 ld_peer_f4(const float* p) {
 #endif
 }
 
+// FP16 tables: ld_peer_f4's half-width twin — 4 halfs (8 B) with the same coherent no-L1-allocate load, widened to fp32
+__device__ __forceinline__ float4 ld_peer_h4(const __half* p) {
+#ifdef TZK_CPU_SHIM
+  return make_float4(__half2float(p[0]), __half2float(p[1]), __half2float(p[2]), __half2float(p[3]));
+#else
+  unsigned int a, b;
+  asm("ld.global.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(a), "=r"(b) : "l"(p));
+  const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&a));
+  const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&b));
+  return make_float4(lo.x, lo.y, hi.x, hi.y);
+#endif
+}
+template <typename TT> __device__ __forceinline__ float4 ld_peer_row4(const TT* p);
+template <> __device__ __forceinline__ float4 ld_peer_row4<float>(const float* p) { return ld_peer_f4(p); }
+template <> __device__ __forceinline__ float4 ld_peer_row4<__half>(const __half* p) { return ld_peer_h4(p); }
+
+// 4 table elements moved as one vector, bits unchanged (mirror refresh): 16 B of floats, 8 B of halfs
+struct __align__(8) H4 { uint32_t a, b; };
+template <typename TT> struct Unit4;
+template <> struct Unit4<float> {
+  using V = float4;
+  __device__ __forceinline__ static V ld(const float* p) { return ld_peer_f4(p); }
+};
+template <> struct Unit4<__half> {
+  using V = H4;
+  __device__ __forceinline__ static V ld(const __half* p) {
+#ifdef TZK_CPU_SHIM
+    return *reinterpret_cast<const H4*>(p);
+#else
+    H4 r;
+    asm("ld.global.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.a), "=r"(r.b) : "l"(p));
+    return r;
+#endif
+  }
+};
+
 // owner rank and owner-local row of a (clamped, non-negative) id — tzk_dist.cu's dest_of.  The quotient is below W <= 16:
 // a float estimate plus one exact fix-up replaces the 64-bit integer division (~100 instructions on the SM, per row,
 // which made the requester-side gather instruction-bound).
@@ -90,14 +134,16 @@ __device__ __forceinline__ int owner_of(int64_t id, int64_t block, int owner, in
 // WTD: weighted bags (per-sample weights psw[l], the sample's own rank holds them): out = sum_l psw[l] * row(ids[l]) in
 // list order as acc = fmaf(psw[l], row, acc), the first term psw[l0] * row, MEAN then * 1/L — the arithmetic of
 // tzk_gather.cu's pooled_gather_fwd_weighted_kernel, so the bits equal the unsharded weighted lookup's.
-template <int G, bool WTD>
+// TT: the table element (float, or __half for FP16 tables: arena and mirror rows are halfs, widened exactly on load, so
+// the sums are the unsharded f16 lookup's).
+template <int G, bool WTD, typename TT = float>
 __device__ __forceinline__ void
 peer_pooled_gather_body(const Peers& tables, const int64_t* __restrict__ rf_w_off, const int64_t* __restrict__ feat_rows,
                         const int64_t* __restrict__ feat_block, const int32_t* __restrict__ feat_owner,
                         const int32_t* __restrict__ feat_dim, const int32_t* __restrict__ feat_col,
                         const int32_t* __restrict__ feat_pool, const int64_t* __restrict__ ids,
                         const int64_t* __restrict__ offsets, int F, int B, int W, float* __restrict__ out,
-                        int64_t ld_out, const float* __restrict__ mirror, const int64_t* __restrict__ feat_mirror_off,
+                        int64_t ld_out, const TT* __restrict__ mirror, const int64_t* __restrict__ feat_mirror_off,
                         const int32_t* __restrict__ feat_sel, int n_sel, const float* __restrict__ psw) {
   // feat_sel (nullable): this launch serves only the listed features (e.g. the mirrored ones, or the ones whose rows
   // cross NVLink — two launches on two streams overlap the local and the remote half of the lookup)
@@ -123,12 +169,12 @@ peer_pooled_gather_body(const Peers& tables, const int64_t* __restrict__ rf_w_of
   if (threadIdx.x < W) base[threadIdx.x] = tables.p[threadIdx.x];
   __syncthreads();
 
-  auto row_ptr = [&](int f, const FeatDesc& d, int64_t id) -> const float* {
+  auto row_ptr = [&](int f, const FeatDesc& d, int64_t id) -> const TT* {
     if ((uint64_t)id >= (uint64_t)d.rows) id = 0;
     if (m_off[f] >= 0) return mirror + m_off[f] + id * d.dim;     // small table: this step's local copy of all its rows
     int64_t loc;
     const int r = owner_of(id, d.block, d.owner, W, &loc);
-    return reinterpret_cast<const float*>(base[r]) + w_off[r * F + f] + loc * d.dim;
+    return reinterpret_cast<const TT*>(base[r]) + w_off[r * F + f] + loc * d.dim;
   };
 
   const int g = threadIdx.x / G, lane = threadIdx.x % G;
@@ -165,7 +211,7 @@ peer_pooled_gather_body(const Peers& tables, const int64_t* __restrict__ rf_w_of
         if (len[u] > 0) {
           const int f = sel[(i0 + u * NG) / TB];
           const FeatDesc& d = fd[f];
-          if (lane * 4 < d.dim) acc[u] = ld_peer_f4(row_ptr(f, d, id0[u]) + lane * 4);
+          if (lane * 4 < d.dim) acc[u] = ld_peer_row4<TT>(row_ptr(f, d, id0[u]) + lane * 4);
         }
       }
 #pragma unroll
@@ -177,17 +223,17 @@ peer_pooled_gather_body(const Peers& tables, const int64_t* __restrict__ rf_w_of
         for (int c = lane * 4; c < d.dim; c += G * 4) {
           float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
           if (len[u] > 0) {
-            a = (c == lane * 4) ? acc[u] : ld_peer_f4(row_ptr(f, d, id0[u]) + c);
+            a = (c == lane * 4) ? acc[u] : ld_peer_row4<TT>(row_ptr(f, d, id0[u]) + c);
             if constexpr (WTD) {
               a = make_float4(a.x * w0[u], a.y * w0[u], a.z * w0[u], a.w * w0[u]);
               for (int l = 1; l < len[u]; ++l) {
                 const float wl = __ldg(psw + s[u] + l);
-                const float4 r = ld_peer_f4(row_ptr(f, d, __ldg(ids + s[u] + l)) + c);
+                const float4 r = ld_peer_row4<TT>(row_ptr(f, d, __ldg(ids + s[u] + l)) + c);
                 a = make_float4(fmaf(wl, r.x, a.x), fmaf(wl, r.y, a.y), fmaf(wl, r.z, a.z), fmaf(wl, r.w, a.w));
               }
             } else {
               for (int l = 1; l < len[u]; ++l)
-                a = f4_add(a, ld_peer_f4(row_ptr(f, d, __ldg(ids + s[u] + l)) + c));
+                a = f4_add(a, ld_peer_row4<TT>(row_ptr(f, d, __ldg(ids + s[u] + l)) + c));
             }
             if (d.pool == 1) {
               const float inv = 1.0f / (float)len[u];
@@ -230,15 +276,30 @@ peer_pooled_gather_fwd_weighted_kernel(const __grid_constant__ Peers tables, con
                                    ids, offsets, F, B, W, out, ld_out, mirror, feat_mirror_off, feat_sel, n_sel, psw);
 }
 
-// un-pooled (sequence) lookup: one lane group per id position, feature by binary search over the segment starts
-template <int G>
+// FP16 tables (arenas and mirror of halfs), plain (WTD = false, psw unused) and weighted bags
+template <int G, bool WTD>
 __global__ void __launch_bounds__(kThreads)
-peer_seq_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off,
-                           const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
-                           const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ ids,
-                           const int64_t* __restrict__ offsets, int F, int B, int W, int D, int64_t nnz,
-                           float* __restrict__ out, const float* __restrict__ mirror,
-                           const int64_t* __restrict__ feat_mirror_off) {
+peer_pooled_gather_fwd_f16_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off,
+                                  const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                                  const int32_t* __restrict__ feat_owner, const int32_t* __restrict__ feat_dim,
+                                  const int32_t* __restrict__ feat_col, const int32_t* __restrict__ feat_pool,
+                                  const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F, int B,
+                                  int W, float* __restrict__ out, int64_t ld_out, const __half* __restrict__ mirror,
+                                  const int64_t* __restrict__ feat_mirror_off, const int32_t* __restrict__ feat_sel,
+                                  int n_sel, const float* __restrict__ psw) {
+  peer_pooled_gather_body<G, WTD, __half>(tables, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col,
+                                          feat_pool, ids, offsets, F, B, W, out, ld_out, mirror, feat_mirror_off,
+                                          feat_sel, n_sel, psw);
+}
+
+// un-pooled (sequence) lookup: one lane group per id position, feature by binary search over the segment starts
+template <int G, typename TT>
+__device__ __forceinline__ void
+peer_seq_gather_body(const Peers& tables, const int64_t* __restrict__ rf_w_off, const int64_t* __restrict__ feat_rows,
+                     const int64_t* __restrict__ feat_block, const int32_t* __restrict__ feat_owner,
+                     const int64_t* __restrict__ ids, const int64_t* __restrict__ offsets, int F, int B, int W, int D,
+                     int64_t nnz, float* __restrict__ out, const TT* __restrict__ mirror,
+                     const int64_t* __restrict__ feat_mirror_off) {
   constexpr int NG = kThreads / G, U = 4;
   TZK_DYN_SMEM(unsigned char, smem_raw);
   int64_t* seg = reinterpret_cast<int64_t*>(smem_raw);   // [F + 1] first id position of every feature
@@ -259,7 +320,7 @@ peer_seq_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* 
   const int lane = threadIdx.x % G;
   const int64_t stride = (int64_t)gridDim.x * NG * U;
   for (int64_t l0 = ((int64_t)blockIdx.x * NG + threadIdx.x / G) * U; l0 < nnz; l0 += stride) {
-    const float* src[U];
+    const TT* src[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int64_t l = l0 + u;
@@ -278,14 +339,14 @@ peer_seq_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* 
         } else {
           int64_t loc;
           const int r = owner_of(id, block[lo], owner[lo], W, &loc);
-          src[u] = reinterpret_cast<const float*>(base[r]) + w_off[r * F + lo] + loc * D;
+          src[u] = reinterpret_cast<const TT*>(base[r]) + w_off[r * F + lo] + loc * D;
         }
       }
     }
     for (int c = lane * 4; c < D; c += G * 4) {
       float4 v[U];
 #pragma unroll
-      for (int u = 0; u < U; ++u) v[u] = src[u] ? ld_peer_f4(src[u] + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int u = 0; u < U; ++u) v[u] = src[u] ? ld_peer_row4<TT>(src[u] + c) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
       for (int u = 0; u < U; ++u)
         if (src[u]) *reinterpret_cast<float4*>(out + (l0 + u) * D + c) = v[u];
@@ -293,22 +354,64 @@ peer_seq_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* 
   }
 }
 
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+peer_seq_gather_fwd_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off,
+                           const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                           const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ ids,
+                           const int64_t* __restrict__ offsets, int F, int B, int W, int D, int64_t nnz,
+                           float* __restrict__ out, const float* __restrict__ mirror,
+                           const int64_t* __restrict__ feat_mirror_off) {
+  peer_seq_gather_body<G, float>(tables, rf_w_off, feat_rows, feat_block, feat_owner, ids, offsets, F, B, W, D, nnz, out,
+                                 mirror, feat_mirror_off);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kThreads)
+peer_seq_gather_fwd_f16_kernel(const __grid_constant__ Peers tables, const int64_t* __restrict__ rf_w_off,
+                               const int64_t* __restrict__ feat_rows, const int64_t* __restrict__ feat_block,
+                               const int32_t* __restrict__ feat_owner, const int64_t* __restrict__ ids,
+                               const int64_t* __restrict__ offsets, int F, int B, int W, int D, int64_t nnz,
+                               float* __restrict__ out, const __half* __restrict__ mirror,
+                               const int64_t* __restrict__ feat_mirror_off) {
+  peer_seq_gather_body<G, __half>(tables, rf_w_off, feat_rows, feat_block, feat_owner, ids, offsets, F, B, W, D, nnz,
+                                  out, mirror, feat_mirror_off);
+}
+
 // ---- per-step local copy of the small tables ------------------------------------------------------------------------------
 // Most lookups of a Criteo-like workload hit tables of a few thousand rows (18 of 26 features, 69 % of the ids): their
 // shards are a few MB in total, so every rank copies them from the owners once per step — long sequential NVLink reads
 // — and its gather reads those features from local memory; only the big tables' rows cross NVLink as
-// random 64-B reads.  Segment s: n[s] floats from rank r[s]'s arena at src[s] to mirror + dst[s].
+// random 64-B reads.  Segment s: n[s] elements from rank r[s]'s arena at src[s] to mirror + dst[s].
+// TT: the table element; the copy moves 4 elements per vector (16 B of floats, 8 B of halfs — table starts and row
+// sizes are multiples of 4 elements, which for halfs is 8-B but not always 16-B alignment) and keeps their bits.
+template <typename TT>
+__device__ __forceinline__ void
+peer_mirror_refresh_simple_body(const Peers& tables, const int32_t* __restrict__ seg_rank,
+                                const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
+                                const int64_t* __restrict__ seg_n, int n_seg, TT* __restrict__ mirror) {
+  using V = typename Unit4<TT>::V;
+  for (int s = blockIdx.y; s < n_seg; s += gridDim.y) {
+    const TT* src = reinterpret_cast<const TT*>(tables.p[__ldg(seg_rank + s)]) + __ldg(seg_src + s);
+    TT* dst = mirror + __ldg(seg_dst + s);
+    const int64_t n4 = __ldg(seg_n + s) >> 2;       // table starts and row sizes are multiples of 4 elements
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
+      reinterpret_cast<V*>(dst)[i] = Unit4<TT>::ld(src + i * 4);
+  }
+}
+
 __global__ void __launch_bounds__(kThreads)
 peer_mirror_refresh_simple_kernel(const __grid_constant__ Peers tables, const int32_t* __restrict__ seg_rank,
                                   const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
                                   const int64_t* __restrict__ seg_n, int n_seg, float* __restrict__ mirror) {
-  for (int s = blockIdx.y; s < n_seg; s += gridDim.y) {
-    const float* src = reinterpret_cast<const float*>(tables.p[__ldg(seg_rank + s)]) + __ldg(seg_src + s);
-    float* dst = mirror + __ldg(seg_dst + s);
-    const int64_t n4 = __ldg(seg_n + s) >> 2;       // table starts and row sizes are multiples of 4 floats
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
-      reinterpret_cast<float4*>(dst)[i] = ld_peer_f4(src + i * 4);
-  }
+  peer_mirror_refresh_simple_body<float>(tables, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
+}
+
+__global__ void __launch_bounds__(kThreads)
+peer_mirror_refresh_simple_f16_kernel(const __grid_constant__ Peers tables, const int32_t* __restrict__ seg_rank,
+                                      const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
+                                      const int64_t* __restrict__ seg_n, int n_seg, __half* __restrict__ mirror) {
+  peer_mirror_refresh_simple_body<__half>(tables, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
 }
 
 // The segments cut into chunks of kMirrorChunk floats, chunks dealt round-robin to the CTAs: every thread has
@@ -316,10 +419,12 @@ peer_mirror_refresh_simple_kernel(const __grid_constant__ Peers tables, const in
 // pays the NVLink round trip once per 16 B and thread).  n_seg <= kMirrorMaxSeg.
 constexpr int kMirrorChunk = 4096;
 constexpr int kMirrorMaxSeg = 4 * kThreads;
-__global__ void __launch_bounds__(kThreads)
-peer_mirror_refresh_kernel(const __grid_constant__ Peers tables, const int32_t* __restrict__ seg_rank,
-                           const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
-                           const int64_t* __restrict__ seg_n, int n_seg, float* __restrict__ mirror) {
+template <typename TT>
+__device__ __forceinline__ void
+peer_mirror_refresh_body(const Peers& tables, const int32_t* __restrict__ seg_rank, const int64_t* __restrict__ seg_src,
+                         const int64_t* __restrict__ seg_dst, const int64_t* __restrict__ seg_n, int n_seg,
+                         TT* __restrict__ mirror) {
+  using V = typename Unit4<TT>::V;
   TZK_DYN_SMEM(int32_t, pre);                     // [kMirrorMaxSeg + 1] chunks before segment s
   int32_t* part = pre + kMirrorMaxSeg + 1;        // [kThreads]
   {   // exclusive scan of the segments' chunk counts: 4 segments per thread + a Hillis-Steele scan of the 256 partial sums
@@ -357,22 +462,37 @@ peer_mirror_refresh_kernel(const __grid_constant__ Peers tables, const int32_t* 
       if (pre[mid] <= chunk) lo = mid; else hi = mid;
     }
     const int sg = lo;
-    const float* src = reinterpret_cast<const float*>(tables.p[__ldg(seg_rank + sg)]) + __ldg(seg_src + sg);
-    float* dst = mirror + __ldg(seg_dst + sg);
+    const TT* src = reinterpret_cast<const TT*>(tables.p[__ldg(seg_rank + sg)]) + __ldg(seg_src + sg);
+    TT* dst = mirror + __ldg(seg_dst + sg);
     const int64_t n4 = __ldg(seg_n + sg) >> 2;
     const int64_t base4 = (int64_t)(chunk - pre[sg]) * (kMirrorChunk / 4);
-    float4 v[Q];
+    V v[Q];
 #pragma unroll
     for (int q = 0; q < Q; ++q) {
       const int64_t i = base4 + threadIdx.x + q * kThreads;
-      if (i < n4) v[q] = ld_peer_f4(src + i * 4);
+      if (i < n4) v[q] = Unit4<TT>::ld(src + i * 4);
     }
 #pragma unroll
     for (int q = 0; q < Q; ++q) {
       const int64_t i = base4 + threadIdx.x + q * kThreads;
-      if (i < n4) reinterpret_cast<float4*>(dst)[i] = v[q];
+      if (i < n4) reinterpret_cast<V*>(dst)[i] = v[q];
     }
   }
+}
+
+__global__ void __launch_bounds__(kThreads)
+peer_mirror_refresh_kernel(const __grid_constant__ Peers tables, const int32_t* __restrict__ seg_rank,
+                           const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
+                           const int64_t* __restrict__ seg_n, int n_seg, float* __restrict__ mirror) {
+  peer_mirror_refresh_body<float>(tables, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
+}
+
+// FP16 tables: the same chunks (kMirrorChunk elements = 8 KB of halfs), 8-B vectors
+__global__ void __launch_bounds__(kThreads)
+peer_mirror_refresh_f16_kernel(const __grid_constant__ Peers tables, const int32_t* __restrict__ seg_rank,
+                               const int64_t* __restrict__ seg_src, const int64_t* __restrict__ seg_dst,
+                               const int64_t* __restrict__ seg_n, int n_seg, __half* __restrict__ mirror) {
+  peer_mirror_refresh_body<__half>(tables, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
 }
 
 // ---- source side of the backward: stable multi-split of the ids by destination ---------------------------------------
@@ -710,11 +830,12 @@ inline int64_t bkt_tiles(int64_t n_bags) { return (n_bags + kBktTile - 1) / kBkt
 
 // table_ptrs: HOST array [W] of device addresses (rank r's arena as mapped in THIS process); rf_w_off: device
 // [W * F] int64 arena element offset of feature f's table on rank r; the other feature arrays as in tzk.h.
+template <typename TT>
 static int peer_pooled_gather_fwd_impl(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
                                        const int64_t* feat_block, const int32_t* feat_owner, const int32_t* feat_dim,
                                        const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
                                        const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t max_dim,
-                                       float* out, int64_t ld_out, const float* mirror,
+                                       float* out, int64_t ld_out, const TT* mirror,
                                        const int64_t* feat_mirror_off, const int32_t* feat_sel, int32_t n_sel,
                                        void* stream, const float* psw = nullptr) {
   Peers t;
@@ -724,6 +845,23 @@ static int peer_pooled_gather_fwd_impl(const uint64_t* table_ptrs, const int64_t
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const size_t smem = (size_t)F * sizeof(FeatDesc) + (size_t)W * F * 8 + (size_t)W * 8 + (size_t)F * 8 + (size_t)F * 4;
   const int grid = grid_for((B + 31) / 32);
+  if constexpr (!std::is_same<TT, float>::value) {     // FP16 tables
+#define TZK_PEER_LAUNCH_H(G, WTD_)                                                                                     \
+  TZK_LAUNCH((peer_pooled_gather_fwd_f16_kernel<G, WTD_>), grid, kThreads, smem, st, t, rf_w_off, feat_rows,          \
+             feat_block, feat_owner, feat_dim, feat_col, feat_pool, ids, offsets, F, B, W, out, ld_out, mirror,        \
+             feat_mirror_off, feat_sel, n_sel, psw)
+    if (psw) {
+      if (max_dim <= 16) TZK_PEER_LAUNCH_H(4, true);
+      else if (max_dim <= 32) TZK_PEER_LAUNCH_H(8, true);
+      else if (max_dim <= 64) TZK_PEER_LAUNCH_H(16, true);
+      else TZK_PEER_LAUNCH_H(32, true);
+    } else if (max_dim <= 16) TZK_PEER_LAUNCH_H(4, false);
+    else if (max_dim <= 32) TZK_PEER_LAUNCH_H(8, false);
+    else if (max_dim <= 64) TZK_PEER_LAUNCH_H(16, false);
+    else TZK_PEER_LAUNCH_H(32, false);
+#undef TZK_PEER_LAUNCH_H
+    return cudaGetLastError() == cudaSuccess ? 0 : 3;
+  } else {
 #define TZK_PEER_LAUNCH(G)                                                                                             \
   TZK_LAUNCH((peer_pooled_gather_fwd_kernel<G>), grid, kThreads, smem, st, t, rf_w_off, feat_rows, feat_block,         \
              feat_owner, feat_dim, feat_col, feat_pool, ids, offsets, F, B, W, out, ld_out, mirror, feat_mirror_off,   \
@@ -744,6 +882,7 @@ static int peer_pooled_gather_fwd_impl(const uint64_t* table_ptrs, const int64_t
 #undef TZK_PEER_LAUNCH_W
 #undef TZK_PEER_LAUNCH
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
+  }
 }
 
 extern "C" int tzk_peer_pooled_gather_fwd(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
@@ -789,6 +928,49 @@ extern "C" int tzk_peer_pooled_gather_fwd_weighted(const uint64_t* table_ptrs, c
                                      stream, per_sample_weights);
 }
 
+// FP16 tables: the same lookups over arenas and a mirror of halfs (pooling and outputs fp32, the bits of
+// tzk_pooled_gather_fwd_f16 / tzk_pooled_gather_fwd_weighted with weights_f16).  Rows are 8-B aligned (dims multiples of 4).
+extern "C" int tzk_peer_pooled_gather_fwd_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off,
+                                              const int64_t* feat_rows, const int64_t* feat_block,
+                                              const int32_t* feat_owner, const int32_t* feat_dim, const int32_t* feat_col,
+                                              const int32_t* feat_pool, const int64_t* ids, const int64_t* offsets,
+                                              int32_t F, int32_t B, int32_t W, int32_t max_dim, float* out,
+                                              int64_t ld_out, const void* mirror, const int64_t* feat_mirror_off,
+                                              void* stream) {
+  return peer_pooled_gather_fwd_impl(table_ptrs, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
+                                     ids, offsets, F, B, W, max_dim, out, ld_out, static_cast<const __half*>(mirror),
+                                     feat_mirror_off, nullptr, 0, stream);
+}
+
+extern "C" int tzk_peer_pooled_gather_fwd_sel_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off,
+                                                  const int64_t* feat_rows, const int64_t* feat_block,
+                                                  const int32_t* feat_owner, const int32_t* feat_dim,
+                                                  const int32_t* feat_col, const int32_t* feat_pool, const int64_t* ids,
+                                                  const int64_t* offsets, int32_t F, int32_t B, int32_t W,
+                                                  int32_t max_dim, float* out, int64_t ld_out, const void* mirror,
+                                                  const int64_t* feat_mirror_off, const int32_t* feat_sel, int32_t n_sel,
+                                                  void* stream) {
+  if (!feat_sel) return 1;
+  return peer_pooled_gather_fwd_impl(table_ptrs, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
+                                     ids, offsets, F, B, W, max_dim, out, ld_out, static_cast<const __half*>(mirror),
+                                     feat_mirror_off, feat_sel, n_sel, stream);
+}
+
+extern "C" int tzk_peer_pooled_gather_fwd_weighted_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off,
+                                                       const int64_t* feat_rows, const int64_t* feat_block,
+                                                       const int32_t* feat_owner, const int32_t* feat_dim,
+                                                       const int32_t* feat_col, const int32_t* feat_pool,
+                                                       const int64_t* ids, const int64_t* offsets, int32_t F, int32_t B,
+                                                       int32_t W, int32_t max_dim, float* out, int64_t ld_out,
+                                                       const void* mirror, const int64_t* feat_mirror_off,
+                                                       const float* per_sample_weights, const int32_t* feat_sel,
+                                                       int32_t n_sel, void* stream) {
+  if (!per_sample_weights) return 1;
+  return peer_pooled_gather_fwd_impl(table_ptrs, rf_w_off, feat_rows, feat_block, feat_owner, feat_dim, feat_col, feat_pool,
+                                     ids, offsets, F, B, W, max_dim, out, ld_out, static_cast<const __half*>(mirror),
+                                     feat_mirror_off, feat_sel, n_sel, stream, per_sample_weights);
+}
+
 extern "C" int tzk_peer_seq_gather_fwd(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
                                        const int64_t* feat_block, const int32_t* feat_owner, const int64_t* ids,
                                        const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t D, int64_t nnz,
@@ -810,11 +992,36 @@ extern "C" int tzk_peer_seq_gather_fwd(const uint64_t* table_ptrs, const int64_t
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
 
+extern "C" int tzk_peer_seq_gather_fwd_f16(const uint64_t* table_ptrs, const int64_t* rf_w_off, const int64_t* feat_rows,
+                                           const int64_t* feat_block, const int32_t* feat_owner, const int64_t* ids,
+                                           const int64_t* offsets, int32_t F, int32_t B, int32_t W, int32_t D,
+                                           int64_t nnz, float* out, const void* mirror, const int64_t* feat_mirror_off,
+                                           void* stream) {
+  Peers t;
+  if (fill(&t, table_ptrs, W) || F <= 0 || B <= 0 || D <= 0 || (D % 4) || nnz < 0) return 1;
+  if (nnz == 0) return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const __half* mh = static_cast<const __half*>(mirror);
+  const size_t smem = (size_t)(F + 1) * 8 + (size_t)F * 16 + (size_t)W * F * 8 + (size_t)W * 8 + (size_t)F * 4 + 16;
+#define TZK_PEER_LAUNCH(G)                                                                                            \
+  TZK_LAUNCH((peer_seq_gather_fwd_f16_kernel<G>), grid_for((nnz + (kThreads / G) * 4 - 1) / ((kThreads / G) * 4)),    \
+             kThreads, smem, st, t, rf_w_off, feat_rows, feat_block, feat_owner, ids, offsets, F, B, W, D, nnz, out,   \
+             mh, feat_mirror_off)
+  if (D <= 16) TZK_PEER_LAUNCH(4);
+  else if (D <= 32) TZK_PEER_LAUNCH(8);
+  else if (D <= 64) TZK_PEER_LAUNCH(16);
+  else TZK_PEER_LAUNCH(32);
+#undef TZK_PEER_LAUNCH
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
 // Copies n_seg contiguous pieces of the ranks' arenas into the local mirror (see peer_mirror_refresh_kernel); the
 // segment arrays are device arrays built once from the sharding plan.
-extern "C" int tzk_peer_mirror_refresh(const uint64_t* table_ptrs, int32_t W, const int32_t* seg_rank,
-                                       const int64_t* seg_src, const int64_t* seg_dst, const int64_t* seg_n,
-                                       int32_t n_seg, float* mirror, void* stream) {
+template <typename TT>
+static int peer_mirror_refresh_impl(const uint64_t* table_ptrs, int32_t W, const int32_t* seg_rank,
+                                    const int64_t* seg_src, const int64_t* seg_dst, const int64_t* seg_n,
+                                    int32_t n_seg, TT* mirror, void* stream) {
+  constexpr bool f16 = !std::is_same<TT, float>::value;
   Peers t;
   if (fill(&t, table_ptrs, W) || n_seg < 0) return 1;
   if (n_seg == 0) return 0;
@@ -835,8 +1042,12 @@ extern "C" int tzk_peer_mirror_refresh(const uint64_t* table_ptrs, int32_t W, co
 #else
     dim3 grid(8, n_seg < 4096 ? n_seg : 4096);
 #endif
-    TZK_LAUNCH((peer_mirror_refresh_simple_kernel), grid, kThreads, 0, reinterpret_cast<cudaStream_t>(stream), t, seg_rank,
-               seg_src, seg_dst, seg_n, n_seg, mirror);
+    if constexpr (f16)
+      TZK_LAUNCH((peer_mirror_refresh_simple_f16_kernel), grid, kThreads, 0, reinterpret_cast<cudaStream_t>(stream), t,
+                 seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
+    else
+      TZK_LAUNCH((peer_mirror_refresh_simple_kernel), grid, kThreads, 0, reinterpret_cast<cudaStream_t>(stream), t,
+                 seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
     return cudaGetLastError() == cudaSuccess ? 0 : 3;
   }
 #ifdef TZK_CPU_SHIM
@@ -844,9 +1055,27 @@ extern "C" int tzk_peer_mirror_refresh(const uint64_t* table_ptrs, int32_t W, co
 #else
   const int grid = 132 * 4;
 #endif
-  TZK_LAUNCH((peer_mirror_refresh_kernel), grid, kThreads, (kMirrorMaxSeg + 1 + kThreads) * sizeof(int32_t),
-             reinterpret_cast<cudaStream_t>(stream), t, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
+  if constexpr (f16)
+    TZK_LAUNCH((peer_mirror_refresh_f16_kernel), grid, kThreads, (kMirrorMaxSeg + 1 + kThreads) * sizeof(int32_t),
+               reinterpret_cast<cudaStream_t>(stream), t, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
+  else
+    TZK_LAUNCH((peer_mirror_refresh_kernel), grid, kThreads, (kMirrorMaxSeg + 1 + kThreads) * sizeof(int32_t),
+               reinterpret_cast<cudaStream_t>(stream), t, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+extern "C" int tzk_peer_mirror_refresh(const uint64_t* table_ptrs, int32_t W, const int32_t* seg_rank,
+                                       const int64_t* seg_src, const int64_t* seg_dst, const int64_t* seg_n,
+                                       int32_t n_seg, float* mirror, void* stream) {
+  return peer_mirror_refresh_impl(table_ptrs, W, seg_rank, seg_src, seg_dst, seg_n, n_seg, mirror, stream);
+}
+
+// FP16 tables: segments counted in halfs (multiples of 4: 8-B vectors), mirror of halfs, bits copied unchanged
+extern "C" int tzk_peer_mirror_refresh_f16(const uint64_t* table_ptrs, int32_t W, const int32_t* seg_rank,
+                                           const int64_t* seg_src, const int64_t* seg_dst, const int64_t* seg_n,
+                                           int32_t n_seg, void* mirror, void* stream) {
+  return peer_mirror_refresh_impl(table_ptrs, W, seg_rank, seg_src, seg_dst, seg_n, n_seg, static_cast<__half*>(mirror),
+                                  stream);
 }
 
 #ifndef TZK_CPU_SHIM

@@ -93,14 +93,12 @@ class _DimGroup:
     def __init__(self, configs: List, plan: Dict[str, TableShard], rank: int, world: int, device, pooled: bool,
                  names: List[List[str]]):
         self.configs, self.rank, self.world, self.pooled = configs, rank, world, pooled
-        from .embedding_modules import DataType
-
-        if any(getattr(c, "data_type", DataType.FP32) != DataType.FP32 for c in configs):
-            raise NotImplementedError("FP16 tables are supported on unsharded collections only")
         self.dim = configs[0].embedding_dim
         rows_local = [local_rows(c, plan[c.name], rank) for c in configs]
         cls = EmbeddingBagCollection if pooled else EmbeddingCollection
-        # local shard arena + slot bookkeeping; output keys follow the WHOLE collection's naming
+        # local shard arena + slot bookkeeping; output keys follow the WHOLE collection's naming.  FP16 tables
+        # (data_type) give a shard arena of halfs; a group that mixes FP32 and FP16 tables raises there, as the
+        # unsharded collection does
         self.local = cls(configs, device=device, local_rows=rows_local, names_by_table=names)
         self.local.allow_interleave = False      # peers read this arena (dense rows): csrc/tzk_peer.cu
         self.feature_names = self.local.feature_names()
@@ -447,7 +445,8 @@ class _ShardedBase(nn.Module):
                 if c.name == name:
                     sh = self.plan[name]
                     block = c.num_embeddings if sh.kind == TABLE_WISE else sh.block
-                    pad = torch.zeros((block, c.embedding_dim), dtype=torch.float32, device=g.local.weights.device)
+                    pad = torch.zeros((block, c.embedding_dim), dtype=g.local.weights.dtype,
+                                      device=g.local.weights.device)
                     n = g.local._table_rows[t]
                     if n:
                         pad[:n] = g.local.table_weight(t)

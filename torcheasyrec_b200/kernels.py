@@ -551,7 +551,18 @@ class CudaKernels:
 
     # ------------------------------------------------------------------ sharded step over peer memory (tzk_peer.cu)
     # `symm` arguments: objects with `.ptrs` = ctypes array [W] of device addresses (rank r's symmetric buffer as
-    # mapped in this process) — peer_exchange._Symm.
+    # mapped in this process) — peer_exchange._Symm.  The table arenas' `.t` says their element type: float32, or float16
+    # for FP16 tables (the _f16 entry points; the mirror then holds halfs too).
+    @staticmethod
+    def _peer_f16(tables, mirror: Optional[torch.Tensor]) -> bool:
+        t = getattr(tables, "t", None)
+        dt = torch.float32 if t is None else t.dtype
+        if dt not in (torch.float32, torch.float16):
+            raise TzkError(f"peer tables: expected float32 or float16 arenas, got {dt}")
+        if mirror is not None:
+            _need(mirror, dt, "mirror")
+        return dt == torch.float16
+
     def peer_pooled_gather_fwd(self, tables, rf_w_off: torch.Tensor, feat_rows: torch.Tensor, feat_block: torch.Tensor,
                                feat_owner: torch.Tensor, lay: FeatureLayout, ids: torch.Tensor, offsets: torch.Tensor,
                                B: int, W: int, out: Optional[torch.Tensor] = None, mirror: Optional[torch.Tensor] = None,
@@ -562,6 +573,7 @@ class CudaKernels:
         `per_sample_weights` (fp32 [nnz], nullable): weighted bags, pooled as pooled_gather_fwd pools them."""
         _need(ids, torch.int64, "ids")
         _need(offsets, torch.int64, "offsets")
+        f16 = self._peer_f16(tables, mirror)
         F = lay.num_features
         if offsets.numel() != F * B + 1:
             raise TzkError(f"offsets has {offsets.numel()} entries, expected F*B+1 = {F * B + 1}")
@@ -577,7 +589,9 @@ class CudaKernels:
                 raise TzkError(f"per_sample_weights has {psw.numel()} entries, ids {ids.numel()}")
             if feat_sel is not None:
                 _need(feat_sel, torch.int32, "feat_sel")
-            check(self._lib.tzk_peer_pooled_gather_fwd_weighted(
+            fn = (self._lib.tzk_peer_pooled_gather_fwd_weighted_f16 if f16
+                  else self._lib.tzk_peer_pooled_gather_fwd_weighted)
+            check(fn(
                 tables.ptrs, _ptr(rf_w_off), _ptr(feat_rows), _ptr(feat_block), _ptr(feat_owner), _ptr(lay.d_dim),
                 _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(ids), _ptr(offsets), F, B, W, (lay.max_dim + 3) // 4 * 4,
                 _ptr(out), ld, _ptr(mirror), _ptr(feat_mirror_off), _ptr(psw), _ptr(feat_sel),
@@ -586,14 +600,16 @@ class CudaKernels:
             return out
         if feat_sel is not None:
             _need(feat_sel, torch.int32, "feat_sel")
-            check(self._lib.tzk_peer_pooled_gather_fwd_sel(
+            fn = self._lib.tzk_peer_pooled_gather_fwd_sel_f16 if f16 else self._lib.tzk_peer_pooled_gather_fwd_sel
+            check(fn(
                 tables.ptrs, _ptr(rf_w_off), _ptr(feat_rows), _ptr(feat_block), _ptr(feat_owner), _ptr(lay.d_dim),
                 _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(ids), _ptr(offsets), F, B, W, (lay.max_dim + 3) // 4 * 4,
                 _ptr(out), ld, _ptr(mirror), _ptr(feat_mirror_off), _ptr(feat_sel), feat_sel.numel(), _stream()),
                 "tzk_peer_pooled_gather_fwd_sel")
             self.launches += 1
             return out
-        check(self._lib.tzk_peer_pooled_gather_fwd(
+        fn = self._lib.tzk_peer_pooled_gather_fwd_f16 if f16 else self._lib.tzk_peer_pooled_gather_fwd
+        check(fn(
             tables.ptrs, _ptr(rf_w_off), _ptr(feat_rows), _ptr(feat_block), _ptr(feat_owner), _ptr(lay.d_dim),
             _ptr(lay.d_col), _ptr(lay.d_pool), _ptr(ids), _ptr(offsets), F, B, W, (lay.max_dim + 3) // 4 * 4, _ptr(out),
             ld, _ptr(mirror), _ptr(feat_mirror_off), _stream()), "tzk_peer_pooled_gather_fwd")
@@ -606,21 +622,23 @@ class CudaKernels:
                             feat_mirror_off: Optional[torch.Tensor] = None) -> torch.Tensor:
         _need(ids, torch.int64, "ids")
         _need(offsets, torch.int64, "offsets")
+        f16 = self._peer_f16(tables, mirror)
         F, D, nnz = lay.num_features, lay.dim[0], ids.numel()
         out = torch.empty((nnz, D), dtype=torch.float32, device=ids.device)
-        check(self._lib.tzk_peer_seq_gather_fwd(tables.ptrs, _ptr(rf_w_off), _ptr(feat_rows), _ptr(feat_block),
-                                                _ptr(feat_owner), _ptr(ids), _ptr(offsets), F, B, W, D, nnz, _ptr(out),
-                                                _ptr(mirror), _ptr(feat_mirror_off), _stream()),
+        fn = self._lib.tzk_peer_seq_gather_fwd_f16 if f16 else self._lib.tzk_peer_seq_gather_fwd
+        check(fn(tables.ptrs, _ptr(rf_w_off), _ptr(feat_rows), _ptr(feat_block), _ptr(feat_owner), _ptr(ids),
+                 _ptr(offsets), F, B, W, D, nnz, _ptr(out), _ptr(mirror), _ptr(feat_mirror_off), _stream()),
               "tzk_peer_seq_gather_fwd")
         self.launches += 1 if nnz else 0
         return out
 
     def peer_mirror_refresh(self, tables, W: int, seg_rank: torch.Tensor, seg_src: torch.Tensor, seg_dst: torch.Tensor,
                             seg_n: torch.Tensor, mirror: torch.Tensor) -> None:
-        """This step's local copy of the small tables (see tzk_peer_mirror_refresh)."""
-        _need(mirror, torch.float32, "mirror")
-        check(self._lib.tzk_peer_mirror_refresh(tables.ptrs, W, _ptr(seg_rank), _ptr(seg_src), _ptr(seg_dst), _ptr(seg_n),
-                                                seg_rank.numel(), _ptr(mirror), _stream()), "tzk_peer_mirror_refresh")
+        """This step's local copy of the small tables (see tzk_peer_mirror_refresh); FP16 tables: a mirror of halfs."""
+        f16 = self._peer_f16(tables, mirror)
+        fn = self._lib.tzk_peer_mirror_refresh_f16 if f16 else self._lib.tzk_peer_mirror_refresh
+        check(fn(tables.ptrs, W, _ptr(seg_rank), _ptr(seg_src), _ptr(seg_dst), _ptr(seg_n), seg_rank.numel(), _ptr(mirror),
+                 _stream()), "tzk_peer_mirror_refresh")
         self.launches += 1
 
     def peer_barrier(self, pads, me: int, W: int, epoch: torch.Tensor) -> None:
@@ -707,7 +725,8 @@ class CudaKernels:
                           max_dim: int, weights: torch.Tensor, state: Optional[torch.Tensor], lr: float, eps: float,
                           **ex) -> None:
         """Owner side of the small-table exchange (see tzk_peer_small_update): psum / flags are symmetric buffers."""
-        _need(weights, torch.float32, "weights")
+        if _table_dtype(weights):             # FP16 tables: fp32 partial sums, the half row rounded back
+            ex = dict(ex, weights_f16=True)
         oa = _opt_args(optimizer, state, lr, eps, ex)
         check(self._lib.tzk_peer_small_update(ctypes.byref(oa), psum.ptrs, flags.ptrs, W, _ptr(tabs), n_tabs, total_rows,
                                               max_dim, _ptr(weights), _stream()), "tzk_peer_small_update")
@@ -727,7 +746,8 @@ class CudaKernels:
     def fused_bwd_apply_peer(self, optimizer: int, pooled: bool, grads, ld_grad: int, weights: torch.Tensor,
                              state: Optional[torch.Tensor], lay: FeatureLayout, B: int, me: int, W: int, cap: int,
                              idx_span: int, lr: float, eps: float, grad_scale: float, ws: torch.Tensor, **ex) -> None:
-        _need(weights, torch.float32, "weights")
+        if _table_dtype(weights):             # FP16 tables: the gradients stay fp32, the update rounds the half row
+            ex = dict(ex, weights_f16=True)
         if state is not None:
             _need(state, torch.float32, "state")
         oa = _opt_args(optimizer, state, lr, eps, ex)

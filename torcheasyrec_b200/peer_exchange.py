@@ -167,8 +167,9 @@ class PeerState(PeerBase):
         self.rf_key_base = torch.tensor([k for lr in per_rank for k in lr.key_base], dtype=torch.int64, device=dev)
         self.feat_rows = torch.tensor([g.configs[t].num_embeddings for t in g.local._feat_table], dtype=torch.int64,
                                       device=dev)
-        # the arena moves into symmetric memory (same size on every rank: the largest shard)
-        self.tables = self._alloc(max(lr.arena_elems for lr in per_rank), torch.float32)
+        # the arena moves into symmetric memory (same size on every rank: the largest shard), in the collection's table
+        # dtype (FP16 tables: halfs; everything else of the exchange stays fp32)
+        self.tables = self._alloc(max(lr.arena_elems for lr in per_rank), g.local.weights.dtype)
         n = g.local.weights.numel()
         self.tables.t[:n].copy_(g.local.weights.data)
         g.local.weights.data = self.tables.t[:n]
@@ -238,7 +239,7 @@ class PeerState(PeerBase):
                     seg_dst.append(base + start * c.embedding_dim)
                     seg_n.append(n * c.embedding_dim)
         self._m_off = m_off
-        self.mirror = torch.zeros(max(o, 4), dtype=torch.float32, device=dev)
+        self.mirror = torch.zeros(max(o, 4), dtype=g.local.weights.dtype, device=dev)     # (FP16 tables: halfs)
         self.feat_mirror_off = torch.tensor([m_off.get(t, -1) for t in g.local._feat_table], dtype=torch.int64, device=dev)
         self._seg = (torch.tensor(seg_rank, dtype=torch.int32, device=dev), torch.tensor(seg_src, dtype=torch.int64, device=dev),
                      torch.tensor(seg_dst, dtype=torch.int64, device=dev), torch.tensor(seg_n, dtype=torch.int64, device=dev))
