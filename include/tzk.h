@@ -572,6 +572,32 @@ int tzk_peer_mirror_refresh_f16(const uint64_t* table_ptrs, int32_t W, const int
                                 const int64_t* seg_dst, const int64_t* seg_n, int32_t n_seg, void* mirror,
                                 tzk_stream_t stream);
 
+/* ---- WuKong layer (tzrec/modules/interaction.py:236-378) around its dense FMB MLP, X [B, n, d] fp32 row-major, m = f + l.
+ * Shapes: n <= 64, d in {4, 8, 16, 32}, k <= 32, f, l >= 1, f + l <= 64.  All weights row-major as the reference
+ * stores them: w_fmb [n, k], w_lcb [n, l], w_res [n, m] (NULL: identity residual, needs n == m); gamma / beta of the FMB
+ * norm [n * k], of the output norm [d].  LayerNorm eps 1e-5.  Everything is fp32 FFMA.  `grid` CTAs walk the samples
+ * (rows) grid-stride; weight / gamma / beta gradients are per-CTA partial sums (`partials`, grid x P floats) reduced in
+ * CTA order into `dparams`: deterministic for a given grid, no float atomics.
+ *   mix_fwd: ln_f [B, n * k] = LayerNorm(X (X^T w_fmb)) with affine, stats [B, 2] = (mean, rstd);
+ *            base [B, m, d] = residual (w_res^T X or X) with w_lcb^T X added to rows >= f.
+ *   mix_bwd: d_ln_f [B, n * k], d_base [B, m, d] -> dx [B, n, d] and dparams (P floats) =
+ *            dw_fmb [n k] | dw_lcb [n l] | dw_res [n m] (w_res only) | dgamma [n k] | dbeta [n k].  F is recomputed.
+ *   out_fwd: y [B, m, d] = LayerNorm_d(z) with affine, z = fmb_out [B, f * d] + base on rows < f, base on the rest;
+ *            stats [B, m, 2].
+ *   out_bwd: dy -> d_fmb_out [B, f * d], d_base [B, m, d], dparams (2 d floats) = dgamma | dbeta. */
+int tzk_wukong_mix_fwd(const float* x, const float* w_fmb, const float* gamma, const float* beta, const float* w_lcb,
+                       const float* w_res, int64_t B, int32_t n, int32_t d, int32_t k, int32_t f, int32_t l,
+                       int32_t grid, float* ln_f, float* stats, float* base, tzk_stream_t stream);
+int tzk_wukong_mix_bwd(const float* x, const float* w_fmb, const float* gamma, const float* w_lcb, const float* w_res,
+                       const float* stats, const float* d_ln_f, const float* d_base, int64_t B, int32_t n, int32_t d,
+                       int32_t k, int32_t f, int32_t l, int32_t grid, float* dx, float* partials, float* dparams,
+                       tzk_stream_t stream);
+int tzk_wukong_out_fwd(const float* fmb_out, const float* base, const float* gamma, const float* beta, int64_t B,
+                       int32_t d, int32_t f, int32_t l, int32_t grid, float* y, float* stats, tzk_stream_t stream);
+int tzk_wukong_out_bwd(const float* fmb_out, const float* base, const float* gamma, const float* stats,
+                       const float* dy, int64_t B, int32_t d, int32_t f, int32_t l, int32_t grid, float* d_fmb_out,
+                       float* d_base, float* partials, float* dparams, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

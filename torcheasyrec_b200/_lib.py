@@ -161,6 +161,15 @@ SIGNATURES = {
     "tzk_peer_seq_gather_fwd_f16": (
         c_int32, [P, P, P, P, P, P, P, c_int32, c_int32, c_int32, c_int32, c_int64, P, P, P, P]),
     "tzk_peer_mirror_refresh_f16": (c_int32, [P, c_int32, P, P, P, P, c_int32, P, P]),
+    # WuKong layer: the FM / linear-compress mix and the output norm, forward and backward
+    "tzk_wukong_mix_fwd": (
+        c_int32, [P, P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, P, P, P, P]),
+    "tzk_wukong_mix_bwd": (
+        c_int32,
+        [P, P, P, P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, P, P, P, P]),
+    "tzk_wukong_out_fwd": (c_int32, [P, P, P, P, c_int64, c_int32, c_int32, c_int32, c_int32, P, P, P]),
+    "tzk_wukong_out_bwd": (
+        c_int32, [P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, c_int32, P, P, P, P, P]),
 }
 
 _lib = None

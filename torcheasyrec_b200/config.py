@@ -130,7 +130,7 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "train_metrics": _f("TrainMetricConfig", rep=True), "kernel": _f(E, "PYTORCH"),
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
-                  "multi_tower": "MultiTower"}.get(k, "Generic")) for k in _MODEL_KINDS}),
+                  "multi_tower": "MultiTower", "wukong": "WuKong"}.get(k, "Generic")) for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
                            "sequence_encoders": _f("SeqEncoderConfig", rep=True),
@@ -139,6 +139,9 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     "MLP": {"hidden_units": _f(I, rep=True), "dropout_ratio": _f(F, rep=True), "activation": _f(S, "nn.ReLU"),
             "use_bn": _f(B, False), "bias": _f(B, True), "use_ln": _f(B, False)},
     "DLRM": {"dense_mlp": _f("MLP"), "arch_with_sparse": _f(B, True), "final": _f("MLP")},
+    "WuKong": {"dense_mlp": _f("MLP"), "wukong_layers": _f("WuKongLayer", rep=True), "final": _f("MLP")},
+    "WuKongLayer": {"lcb_feature_num": _f(I), "fmb_feature_num": _f(I), "compressed_feature_num": _f(I, 16),
+                    "feature_num_mlp": _f("MLP")},
     "DeepFM": {"deep": _f("MLP"), "final": _f("MLP"), "wide_embedding_dim": _f(I, 4), "wide_init_fn": _f(S)},
     "MultiTower": {"towers": _f("Tower", rep=True), "final": _f("MLP")},
     "MultiTowerDIN": {"towers": _f("Tower", rep=True), "din_towers": _f("DINTower", rep=True), "final": _f("MLP")},

@@ -46,12 +46,12 @@ class Pipeline:
                  sharding: Optional[str] = None, group=None, rw_min_rows: int = 0,
                  static_capacity: Optional[float] = None, exchange: str = "nccl") -> None:
         """`config`: path of a pipeline .config/.json, or the name of a built-in example
-        (example_configs.GENERATORS: dlrm_criteo, deepfm_criteo, mmoe_taobao, multi_tower_din_taobao)."""
+        (example_configs.BUILTINS: dlrm_criteo, deepfm_criteo, mmoe_taobao, multi_tower_din_taobao, wukong_criteo)."""
         from . import example_configs
         from .config import parse_text
 
-        if config in example_configs.GENERATORS:
-            self.cfg = parse_text(example_configs.GENERATORS[config]())
+        if config in example_configs.BUILTINS:
+            self.cfg = parse_text(example_configs.BUILTINS[config]())
         else:
             self.cfg = load_pipeline_config(config)
         if edits:

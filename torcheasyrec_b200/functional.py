@@ -387,3 +387,83 @@ def jagged_softmax_weighted_sum(scores: torch.Tensor, seq: torch.Tensor, offsets
     if dt is not None:
         return _torch_jagged_softmax_wsum(scores, seq, offsets, int(max_len), dt)
     return _JaggedSoftmaxWsum.apply(scores, seq, offsets, int(max_len))
+
+
+# ------------------------------------------------------------------------------------------------ WuKong layer
+def wukong_usable(x: torch.Tensor, n: int, d: int, k: int, f: int, l: int) -> bool:
+    """True when the fused WuKong kernels (csrc/tzk_wukong.cuh) cover this layer call: fp32 [B, n, d] input with
+    n <= 64, d in {4, 8, 16, 32}, k <= 32, f, l >= 1 and f + l <= 64, autocast off, on a device the compute backend
+    runs (CUDA; on the CPU only a test backend that implements the WuKong kernels)."""
+    if autocast_dtype(x) is not None or x.dtype != torch.float32 or x.dim() != 3 or tuple(x.shape[1:]) != (n, d):
+        return False
+    if not (1 <= n <= 64 and d in (4, 8, 16, 32) and 1 <= k <= 32 and f >= 1 and l >= 1 and f + l <= 64):
+        return False
+    return x.is_cuda or (_backend is not None and hasattr(_backend, "wukong_mix_fwd"))
+
+
+class _WuKongMix(torch.autograd.Function):
+    """x -> (LayerNorm(n k)(X (X^T W_fmb)), base): the FMB's interaction and norm, and the LCB + residual."""
+
+    @staticmethod
+    def forward(ctx, x, w_fmb, gamma, beta, w_lcb, w_res, f):
+        x = x.contiguous()
+        ln_f, stats, base = backend().wukong_mix_fwd(x, w_fmb, gamma, beta, w_lcb, w_res, f)
+        ctx.save_for_backward(x, w_fmb, gamma, w_lcb, w_res, stats)
+        ctx.f = f
+        return ln_f, base
+
+    @staticmethod
+    def backward(ctx, d_ln_f, d_base):
+        x, w_fmb, gamma, w_lcb, w_res, stats = ctx.saved_tensors
+        B, n, d = x.shape
+        if d_ln_f is None:
+            d_ln_f = x.new_zeros((B, n * w_fmb.shape[1]))
+        if d_base is None:
+            d_base = x.new_zeros((B, ctx.f + w_lcb.shape[1], d))
+        dx, dwf, dg, db, dwl, dwr = backend().wukong_mix_bwd(x, w_fmb, gamma, w_lcb, w_res, ctx.f, stats,
+                                                             d_ln_f.contiguous(), d_base.contiguous())
+        return dx, dwf, dg, db, dwl, dwr, None
+
+
+class _WuKongOut(torch.autograd.Function):
+    """(fmb_out, base) -> LayerNorm(d)(concat(fmb, lcb) + residual)."""
+
+    @staticmethod
+    def forward(ctx, fmb_out, base, gamma, beta, f):
+        fmb_out = fmb_out.contiguous()
+        y, stats = backend().wukong_out_fwd(fmb_out, base, gamma, beta, f)
+        ctx.save_for_backward(fmb_out, base, gamma, stats)
+        ctx.f = f
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        fmb_out, base, gamma, stats = ctx.saved_tensors
+        d_fmb, d_base, dg, db = backend().wukong_out_bwd(fmb_out, base, gamma, ctx.f, stats, dy.contiguous())
+        return d_fmb, d_base, dg, db, None
+
+
+def wukong_mix(x: torch.Tensor, w_fmb: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, w_lcb: torch.Tensor,
+               w_res: Optional[torch.Tensor], f: int):
+    """Fused first half of a WuKong layer (csrc/tzk_wukong.cuh mix_fwd / mix_bwd): x [B, n, d] ->
+    (LayerNorm(X (X^T w_fmb)) [B, n k], base [B, f + l, d]) where base holds the residual (w_res^T X, or X when w_res is
+    None) and, on rows >= f, lcb + residual.  The caller checks wukong_usable first."""
+    return _WuKongMix.apply(x, w_fmb, gamma, beta, w_lcb, w_res, f)
+
+
+def wukong_out(fmb_out: torch.Tensor, base: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, f: int):
+    """Fused end of a WuKong layer (csrc/tzk_wukong.cuh out_fwd / out_bwd): LayerNorm(d) with affine of base with
+    fmb_out [B, f d] added to its first f rows -> [B, f + l, d]."""
+    return _WuKongOut.apply(fmb_out, base, gamma, beta, f)
+
+
+def torch_wukong_interaction(x: torch.Tensor, w_fmb: torch.Tensor) -> torch.Tensor:
+    """FactorizationMachineBlock's interaction as the reference states it (tzrec/modules/interaction.py:314-317):
+    X (X^T W) flattened to [B, n k]."""
+    t = torch.matmul(x.permute(0, 2, 1), w_fmb)
+    return torch.matmul(x, t).reshape(x.shape[0], -1)
+
+
+def torch_linear_compress(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
+    """LinearCompressBlock.forward (tzrec/modules/interaction.py:255-264): W^T X as [B, l, d]."""
+    return (x.permute(0, 2, 1) @ w).permute(0, 2, 1)

@@ -1065,6 +1065,87 @@ class CudaKernels:
                                               _ptr(invalid), _stream()), "tzk_binned_auc_update")
         self.launches += int(n > 0)
 
+    # ------------------------------------------------------------------ WuKong layer (csrc/tzk_wukong.cuh)
+    def _wukong_grid(self, work: int, per_sm: int) -> int:
+        """CTAs of a WuKong launch: min(work, per_sm x SMs).  The weight-gradient partials are per CTA, so the grid
+        fixes the reduction order; it depends only on the batch size and the device."""
+        sms = getattr(self, "_sms", None)
+        if sms is None:
+            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
+        return max(1, min(int(work), per_sm * sms))
+
+    def wukong_mix_fwd(self, x, w_fmb, gamma, beta, w_lcb, w_res, f: int):
+        """x [B, n, d] -> (ln_f [B, n k], stats [B, 2], base [B, f + l, d]); w_res None: identity residual."""
+        for t, nm in ((x, "x"), (w_fmb, "w_fmb"), (gamma, "gamma"), (beta, "beta"), (w_lcb, "w_lcb")):
+            _need(t, torch.float32, nm)
+        if w_res is not None:
+            _need(w_res, torch.float32, "w_res")
+        B, n, d = x.shape
+        k, l = w_fmb.shape[1], w_lcb.shape[1]
+        m = f + l
+        ln_f = torch.empty((B, n * k), dtype=torch.float32, device=x.device)
+        stats = torch.empty((B, 2), dtype=torch.float32, device=x.device)
+        base = torch.empty((B, m, d), dtype=torch.float32, device=x.device)
+        check(self._lib.tzk_wukong_mix_fwd(_ptr(x), _ptr(w_fmb), _ptr(gamma), _ptr(beta), _ptr(w_lcb), _ptr(w_res), B,
+                                           n, d, k, f, l, self._wukong_grid(B, 8), _ptr(ln_f), _ptr(stats), _ptr(base),
+                                           _stream()), "tzk_wukong_mix_fwd")
+        self.launches += int(B > 0)
+        return ln_f, stats, base
+
+    def wukong_mix_bwd(self, x, w_fmb, gamma, w_lcb, w_res, f: int, stats, d_ln_f, d_base):
+        """-> (dx, dw_fmb, dgamma, dbeta, dw_lcb, dw_res or None)."""
+        for t, nm in ((x, "x"), (w_fmb, "w_fmb"), (gamma, "gamma"), (w_lcb, "w_lcb"), (stats, "stats"),
+                      (d_ln_f, "d_ln_f"), (d_base, "d_base")):
+            _need(t, torch.float32, nm)
+        if w_res is not None:
+            _need(w_res, torch.float32, "w_res")
+        B, n, d = x.shape
+        k, l = w_fmb.shape[1], w_lcb.shape[1]
+        m = f + l
+        nk, nr = n * k, (n * m if w_res is not None else 0)
+        P = 3 * nk + n * l + nr
+        grid = self._wukong_grid(B, 4)       # mix_bwd_kernel: 4 resident CTAs per SM (launch bounds)
+        dx = torch.empty_like(x)
+        partials = self._workspace("wukong_mix_bwd", grid * P * 4, x.device)
+        dparams = torch.empty(P, dtype=torch.float32, device=x.device)
+        check(self._lib.tzk_wukong_mix_bwd(_ptr(x), _ptr(w_fmb), _ptr(gamma), _ptr(w_lcb), _ptr(w_res), _ptr(stats),
+                                           _ptr(d_ln_f), _ptr(d_base), B, n, d, k, f, l, grid, _ptr(dx),
+                                           _ptr(partials), _ptr(dparams), _stream()), "tzk_wukong_mix_bwd")
+        self.launches += 1 + int(B > 0)
+        o = [0, nk, nk + n * l, nk + n * l + nr, 2 * nk + n * l + nr, P]
+        dw_res = dparams[o[2]:o[3]].view(n, m) if w_res is not None else None
+        return (dx, dparams[o[0]:o[1]].view(n, k), dparams[o[3]:o[4]], dparams[o[4]:o[5]],
+                dparams[o[1]:o[2]].view(n, l), dw_res)
+
+    def wukong_out_fwd(self, fmb_out, base, gamma, beta, f: int):
+        """fmb_out [B, f d], base [B, m, d] -> (y [B, m, d], stats [B, m, 2])."""
+        for t, nm in ((fmb_out, "fmb_out"), (base, "base"), (gamma, "gamma"), (beta, "beta")):
+            _need(t, torch.float32, nm)
+        B, m, d = base.shape
+        y = torch.empty_like(base)
+        stats = torch.empty((B, m, 2), dtype=torch.float32, device=base.device)
+        check(self._lib.tzk_wukong_out_fwd(_ptr(fmb_out), _ptr(base), _ptr(gamma), _ptr(beta), B, d, f, m - f,
+                                           self._wukong_grid(-(-B * m // 128), 8), _ptr(y), _ptr(stats), _stream()),
+              "tzk_wukong_out_fwd")
+        self.launches += int(B > 0)
+        return y, stats
+
+    def wukong_out_bwd(self, fmb_out, base, gamma, f: int, stats, dy):
+        """-> (d_fmb_out [B, f d], d_base [B, m, d], dgamma [d], dbeta [d])."""
+        for t, nm in ((fmb_out, "fmb_out"), (base, "base"), (gamma, "gamma"), (stats, "stats"), (dy, "dy")):
+            _need(t, torch.float32, nm)
+        B, m, d = base.shape
+        grid = self._wukong_grid(-(-B * m // 128), 4)
+        d_fmb = torch.empty_like(fmb_out)
+        d_base = torch.empty_like(base)
+        partials = self._workspace("wukong_out_bwd", grid * 2 * d * 4, base.device)
+        dparams = torch.empty(2 * d, dtype=torch.float32, device=base.device)
+        check(self._lib.tzk_wukong_out_bwd(_ptr(fmb_out), _ptr(base), _ptr(gamma), _ptr(stats), _ptr(dy), B, d, f,
+                                           m - f, grid, _ptr(d_fmb), _ptr(d_base), _ptr(partials), _ptr(dparams),
+                                           _stream()), "tzk_wukong_out_bwd")
+        self.launches += 1 + int(B > 0)
+        return d_fmb, d_base, dparams[:d], dparams[d:]
+
 
 @dataclass
 class ColPlan:

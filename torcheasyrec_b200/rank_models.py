@@ -606,8 +606,128 @@ class MultiTower(MultiTowerDIN):
     """tzrec/models/multi_tower.py:27-85: the same towers + final MLP without attention towers."""
 
 
+class LinearCompressBlock(nn.Module):
+    """tzrec/modules/interaction.py:236-264: W^T X with W [feature_num_in, feature_num_out]."""
+
+    def __init__(self, feature_num_in: int, feature_num_out: int) -> None:
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty((feature_num_in, feature_num_out)))
+        nn.init.kaiming_uniform_(self.weight)
+
+    def forward(self, inputs: torch.Tensor) -> torch.Tensor:
+        return Fn.torch_linear_compress(inputs, self.weight)
+
+
+class FactorizationMachineBlock(nn.Module):
+    """tzrec/modules/interaction.py:267-321: LayerNorm(X (X^T W)) -> MLP -> Linear to feature_num_out x input_dim."""
+
+    def __init__(self, input_dim: int, feature_num_in: int, feature_num_out: int, compressed_feature_num: int,
+                 feature_num_mlp: Optional[Dict[str, Any]] = None) -> None:
+        super().__init__()
+        self.feature_num_out, self.input_dim = feature_num_out, input_dim
+        self.weight = nn.Parameter(torch.empty((feature_num_in, compressed_feature_num)))
+        self.norm = nn.LayerNorm(feature_num_in * compressed_feature_num)
+        self.mlp = MLP(in_features=feature_num_in * compressed_feature_num, **(feature_num_mlp or {}))
+        self.feature_out_liner = _Linear(self.mlp.output_dim(), feature_num_out * input_dim)
+        nn.init.kaiming_uniform_(self.weight)
+
+    def forward(self, inputs: torch.Tensor) -> torch.Tensor:
+        out = self.mlp(self.norm(Fn.torch_wukong_interaction(inputs, self.weight)))
+        return self.feature_out_liner(out).view(-1, self.feature_num_out, self.input_dim)
+
+
+class WuKongLayer(nn.Module):
+    """tzrec/modules/interaction.py:324-378.  When Fn.wukong_usable holds, the FMB's interaction + norm, the LCB and the
+    residual run as one kernel (Fn.wukong_mix), the FMB's MLP and output Linear on the dense path, and the residual
+    add + LayerNorm(d) as a second kernel (Fn.wukong_out); otherwise the reference's torch formulation."""
+
+    def __init__(self, input_dim: int, feature_num: int, lcb_feature_num: int, fmb_feature_num: int,
+                 compressed_feature_num: int = 16, feature_num_mlp: Optional[Dict[str, Any]] = None) -> None:
+        super().__init__()
+        self.input_dim, self.feature_num = input_dim, feature_num
+        self.lcb_feature_num, self.fmb_feature_num = lcb_feature_num, fmb_feature_num
+        self.compressed_feature_num = compressed_feature_num
+        self.lcb = LinearCompressBlock(feature_num, lcb_feature_num)
+        self.fmb = FactorizationMachineBlock(input_dim, feature_num, fmb_feature_num, compressed_feature_num,
+                                             feature_num_mlp)
+        self.norm = nn.LayerNorm(input_dim)
+        if feature_num != lcb_feature_num + fmb_feature_num:
+            self.residual_projection = LinearCompressBlock(feature_num, lcb_feature_num + fmb_feature_num)
+        else:
+            self.residual_projection = nn.Identity()
+
+    def output_feature_num(self) -> int:
+        return self.lcb_feature_num + self.fmb_feature_num
+
+    def fused_usable(self, inputs: torch.Tensor) -> bool:
+        return Fn.wukong_usable(inputs, self.feature_num, self.input_dim, self.compressed_feature_num,
+                                self.fmb_feature_num, self.lcb_feature_num)
+
+    def forward(self, inputs: torch.Tensor) -> torch.Tensor:
+        if self.fused_usable(inputs):
+            f = self.fmb_feature_num
+            w_res = None if isinstance(self.residual_projection, nn.Identity) else self.residual_projection.weight
+            ln_f, base = Fn.wukong_mix(inputs, self.fmb.weight, self.fmb.norm.weight, self.fmb.norm.bias,
+                                       self.lcb.weight, w_res, f)
+            fmb_out = self.fmb.feature_out_liner(self.fmb.mlp(ln_f))
+            return Fn.wukong_out(fmb_out, base, self.norm.weight, self.norm.bias, f)
+        lcb = self.lcb(inputs)
+        fmb = self.fmb(inputs)
+        outputs = torch.concat((fmb, lcb), dim=1)
+        return self.norm(outputs + self.residual_projection(inputs))
+
+
+class WuKong(RankModel):
+    """tzrec/models/wukong.py:26-130: the DLRM-style inputs (a `dense` group through a bottom MLP and a `sparse` group of
+    equal-dim ids) through a stack of WuKong layers, then the final MLP and the output Linear."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self.init_input()
+        eg = self.embedding_group
+        self._sparse_group_name = eg.group_names()[0] if len(eg.group_names()) == 1 else "sparse"
+        self.dense_mlp = None
+        self._dense_group_name = "dense"
+        if len(eg.group_names()) > 1 and eg.has_group(self._dense_group_name):
+            for name in eg.group_feature_dims(self._dense_group_name):
+                if "seq_encoder" in name:
+                    raise Exception("dense group not have sequence features.")
+            self.dense_mlp = MLP(eg.group_total_dim(self._dense_group_name),
+                                 **config_to_kwargs(self._model_config.dense_mlp))
+        sparse_dims = eg.group_feature_dims(self._sparse_group_name)
+        self._per_sparse_dim = 0
+        for name, dim in sparse_dims.items():
+            self._per_sparse_dim = dim
+            if "seq_encoder" in name:
+                raise Exception("sparse group not have sequence features.")
+        self._sparse_num = len(sparse_dims)
+        if len(set(sparse_dims.values())) > 1:
+            raise Exception(f"sparse group feature dims must be the same, but we find {set(sparse_dims.values())}")
+        if self.dense_mlp and self._per_sparse_dim != self.dense_mlp.output_dim():
+            raise Exception("dense mlp last hidden_unit must be the same sparse feature dim")
+        self._wukong_layers = nn.ModuleList()
+        feature_num = self._sparse_num + (1 if self.dense_mlp else 0)
+        for layer_cfg in self._model_config.wukong_layers:
+            layer = WuKongLayer(self._per_sparse_dim, feature_num, **config_to_kwargs(layer_cfg))
+            self._wukong_layers.append(layer)
+            feature_num = layer.output_feature_num()
+        self.final_mlp = MLP(feature_num * self._per_sparse_dim, **config_to_kwargs(self._model_config.final))
+        self.output_mlp = _Linear(self.final_mlp.output_dim(), self._num_class)
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        grouped = self.build_input(batch)
+        feat = grouped[self._sparse_group_name].reshape(-1, self._sparse_num, self._per_sparse_dim)
+        if self.dense_mlp:
+            dense_feat = self.dense_mlp(grouped[self._dense_group_name])
+            feat = torch.cat([dense_feat.unsqueeze(1), feat], dim=1)
+        for layer in self._wukong_layers:
+            feat = layer(feat)
+        y = self.output_mlp(self.final_mlp(feat.reshape(feat.size(0), -1)))
+        return self._output_to_prediction(y)
+
+
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
-                 "mmoe": MMoE}
+                 "mmoe": MMoE, "wukong": WuKong}
 
 
 def create_model(model_config: Message, features: List[BaseFeature], labels: List[str], device=None) -> RankModel:
