@@ -598,6 +598,35 @@ int tzk_wukong_out_bwd(const float* fmb_out, const float* base, const float* gam
                        const float* dy, int64_t B, int32_t d, int32_t f, int32_t l, int32_t grid, float* d_fmb_out,
                        float* d_base, float* partials, float* dparams, tzk_stream_t stream);
 
+/* ---- MaskNet's parallel mask blocks (tzrec/modules/masknet.py:77-85, 142-155) around their GEMMs.  nb blocks, input
+ * width E, FFN width H; Ep = E rounded up to a multiple of 4 is the row pitch of every [B, nb Ep] operand, so the GEMMs
+ * between these stages run on 16-B aligned rows.  Shapes: pad4(E) <= 1024, 4 <= H <= 1024 with H % 4 == 0,
+ * 1 <= nb <= 8.  fp32 row-major; LayerNorm eps 1e-5; fp32 FFMA.  `grid` CTAs walk the samples grid-stride; batch sums
+ * (bias / gamma / beta gradients) are per-CTA partials (`partials`) reduced in CTA order into `dparams`: deterministic
+ * for a given grid, no float atomics.
+ *   mask_fwd: e [B, lde] (first E columns), m [B, nb Ep] (the mask generators' second GEMM, no bias), b2 [nb E],
+ *             gamma / beta [E] of ln_emb -> v [B, nb Ep] = LN(e) * (m_i + b2_i) per block (pad columns 0),
+ *             stats [B, 2] = (mean, rstd).  Replaces ln_emb, the bias add and `feature_input * weights` (:80, :144).
+ *   mask_bwd: dv [B, nb Ep] -> dm [B, nb Ep] = dv_i * LN(e), de [B, Ep] = LayerNorm backward of
+ *             sum_i dv_i * (m_i + b2_i) (pad columns 0), dparams ((nb + 2) E floats) = db2 [nb E] | dgamma | dbeta.
+ *             partials: grid x (nb + 2) E floats.
+ *   ffn_fwd:  z [B, nb H] (each block's ffn.0 GEMM, no bias), b3 / gamma / beta [nb H] -> y [B, nb H] =
+ *             ReLU(LN_H(z_i + b3_i)) in block i's column slot (the concat at :145-151), stats [B, nb, 2].
+ *             Replaces ffn's bias add, LayerNorm and ReLU (:68-72, :82).
+ *   ffn_bwd:  dy [B, nb H] -> dz [B, nb H], dparams (nb x 3 H floats) = per block dgamma | dbeta | db3.
+ *             partials: nb x grid x 3 H floats. */
+int tzk_masknet_mask_fwd(const float* e, int32_t lde, const float* m, const float* b2, const float* gamma,
+                         const float* beta, int64_t B, int32_t E, int32_t nb, int32_t grid, float* v, float* stats,
+                         tzk_stream_t stream);
+int tzk_masknet_mask_bwd(const float* e, int32_t lde, const float* m, const float* b2, const float* gamma,
+                         const float* beta, const float* stats, const float* dv, int64_t B, int32_t E, int32_t nb,
+                         int32_t grid, float* dm, float* de, float* partials, float* dparams, tzk_stream_t stream);
+int tzk_masknet_ffn_fwd(const float* z, const float* b3, const float* gamma, const float* beta, int64_t B, int32_t H,
+                        int32_t nb, int32_t grid, float* y, float* stats, tzk_stream_t stream);
+int tzk_masknet_ffn_bwd(const float* z, const float* b3, const float* gamma, const float* beta, const float* stats,
+                        const float* dy, int64_t B, int32_t H, int32_t nb, int32_t grid, float* dz, float* partials,
+                        float* dparams, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -170,6 +170,12 @@ SIGNATURES = {
     "tzk_wukong_out_fwd": (c_int32, [P, P, P, P, c_int64, c_int32, c_int32, c_int32, c_int32, P, P, P]),
     "tzk_wukong_out_bwd": (
         c_int32, [P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, c_int32, P, P, P, P, P]),
+    # MaskNet: the instance-guided mask and the FFN's bias + LayerNorm + ReLU, forward and backward
+    "tzk_masknet_mask_fwd": (c_int32, [P, c_int32, P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P]),
+    "tzk_masknet_mask_bwd": (
+        c_int32, [P, c_int32, P, P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P, P, P]),
+    "tzk_masknet_ffn_fwd": (c_int32, [P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P]),
+    "tzk_masknet_ffn_bwd": (c_int32, [P, P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P, P]),
 }
 
 _lib = None

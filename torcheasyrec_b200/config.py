@@ -130,7 +130,8 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "train_metrics": _f("TrainMetricConfig", rep=True), "kernel": _f(E, "PYTORCH"),
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
-                  "multi_tower": "MultiTower", "wukong": "WuKong"}.get(k, "Generic")) for k in _MODEL_KINDS}),
+                  "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet"}.get(k, "Generic"))
+           for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
                            "sequence_encoders": _f("SeqEncoderConfig", rep=True),
@@ -142,6 +143,10 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     "WuKong": {"dense_mlp": _f("MLP"), "wukong_layers": _f("WuKongLayer", rep=True), "final": _f("MLP")},
     "WuKongLayer": {"lcb_feature_num": _f(I), "fmb_feature_num": _f(I), "compressed_feature_num": _f(I, 16),
                     "feature_num_mlp": _f("MLP")},
+    "MaskNet": {"mask_net_module": _f("MaskNetModule")},
+    "MaskNetModule": {"n_mask_blocks": _f(I), "mask_block": _f("MaskBlock"), "top_mlp": _f("MLP"),
+                      "use_parallel": _f(B, True)},
+    "MaskBlock": {"reduction_ratio": _f(F, 1.0), "aggregation_dim": _f(I), "hidden_dim": _f(I)},
     "DeepFM": {"deep": _f("MLP"), "final": _f("MLP"), "wide_embedding_dim": _f(I, 4), "wide_init_fn": _f(S)},
     "MultiTower": {"towers": _f("Tower", rep=True), "final": _f("MLP")},
     "MultiTowerDIN": {"towers": _f("Tower", rep=True), "din_towers": _f("DINTower", rep=True), "final": _f("MLP")},

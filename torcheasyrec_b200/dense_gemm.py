@@ -85,6 +85,33 @@ def _mm(a: torch.Tensor, ta: bool, b: torch.Tensor, tb: bool, M: int, N: int, K:
     return out
 
 
+def gemm(a: torch.Tensor, ta: bool, b: torch.Tensor, tb: bool, out: Optional[torch.Tensor] = None,
+         beta: float = 0.0) -> torch.Tensor:
+    """out = op(a) @ op(b) + beta * out for row-major 2-D views whose rows may be strided (column slices of a wider
+    buffer: each operand's row pitch is its stride(0)).  cuBLASLt BF16x9 on CUDA; `out` None allocates [M, N].  On the
+    CPU (test backends only) the same product in torch."""
+    M = a.shape[1] if ta else a.shape[0]
+    K = a.shape[0] if ta else a.shape[1]
+    N = b.shape[0] if tb else b.shape[1]
+    if out is None:
+        out = torch.empty((M, N), dtype=torch.float32, device=a.device)
+    if not a.is_cuda:
+        r = (a.t() if ta else a) @ (b.t() if tb else b)
+        return out.copy_(r) if beta == 0.0 else out.mul_(beta).add_(r)
+    lib = _load()
+    if lib is None:
+        raise RuntimeError("dense_gemm.gemm: the cuBLASLt library (csrc/libtzk_gemm.so, cuBLAS >= 12.9) is not loaded")
+    ws = _workspace(a.device)
+    used = ctypes.c_int(0)
+    rc = lib.tzg_matmul(int(ta), int(tb), M, N, K, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0),
+                        out.data_ptr(), out.stride(0), 1.0, float(beta), 1, ws.data_ptr(), ws.numel(),
+                        torch.cuda.current_stream().cuda_stream, ctypes.byref(used))
+    if rc != 0:
+        raise RuntimeError(lib.tzg_last_error().decode())
+    _state["emulated_calls" if used.value else "plain_calls"] += 1
+    return out
+
+
 class _LinearFn(torch.autograd.Function):
     """y = act(x @ W^T + b), act = ReLU or identity (tzrec/modules/mlp.py Perceptron).  GEMMs: cuBLASLt BF16x9;
     bias+ReLU and ReLU-backward+bias-gradient are one tzk kernel each instead of four ATen passes.

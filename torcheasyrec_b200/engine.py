@@ -46,7 +46,8 @@ class Pipeline:
                  sharding: Optional[str] = None, group=None, rw_min_rows: int = 0,
                  static_capacity: Optional[float] = None, exchange: str = "nccl") -> None:
         """`config`: path of a pipeline .config/.json, or the name of a built-in example
-        (example_configs.BUILTINS: dlrm_criteo, deepfm_criteo, mmoe_taobao, multi_tower_din_taobao, wukong_criteo)."""
+        (example_configs.BUILTINS: dlrm_criteo, deepfm_criteo, mmoe_taobao, multi_tower_din_taobao, masknet_criteo,
+        wukong_criteo)."""
         from . import example_configs
         from .config import parse_text
 

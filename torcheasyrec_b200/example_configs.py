@@ -1,5 +1,5 @@
 """Generators for the pipeline configs BASELINE.json names (text format, same message tree as the reference's
-examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao}.config).
+examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo}.config).
 
 The package does not depend on the reference's files, so the configs are re-derived here from their defining facts
 (SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table list and price boundaries, and the model
@@ -123,6 +123,33 @@ def wukong_criteo() -> str:
             "    metrics {\n        auc {}\n    }\n    losses {\n        binary_cross_entropy {}\n    }\n}\n")
 
 
+def masknet_criteo() -> str:
+    """examples/masknet_criteo.config: 13 raw features (embedding_dim 16, but no dense_emb, so 1 wide each) + 26 hashed
+    id(D=16) in one DEEP group all_features of width 26 * 16 + 13 = 429; mask_net{3 parallel blocks, reduction_ratio 3,
+    hidden_dim 512, top_mlp 256-128-64}.  Unlike the other Criteo examples: empty paths, lr 1e-4 for both optimizers,
+    save_checkpoints_epochs 1, no eval num_steps and no odps_data_quota_name."""
+    ints = [f"int_{i}" for i in range(13)]
+    cats = [f"cat_{i}" for i in range(26)]
+    hdr = _header("", "", "", "FG_DAG", ["label"], None, quota=False)
+    hdr = (hdr.replace('"odps://{PROJECT}/tables/"', '""').replace('"experiments/"', '""')
+           .replace("lr: 0.001\n", "lr: 0.0001\n")
+           .replace("    num_epochs: 1\n", "    num_epochs: 1\n    save_checkpoints_epochs: 1\n"))
+    feats = []
+    for i in range(13):
+        feats.append("feature_configs {\n    raw_feature {\n" f'        feature_name: "int_{i}"\n'
+                     f'        embedding_dim: 16\n        expression: "user:int_{i}"\n'
+                     '        normalizer: "method=expression,expr=log(x+3)"\n    }\n}\n')
+    for i, h in enumerate(CRITEO_HASH_SIZES):
+        feats.append(_id_feature(f"cat_{i}", "item", h, field="hash_bucket_size"))
+    return (hdr + "".join(feats)
+            + "model_config {\n" + _group("all_features", cats + ints, "DEEP")
+            + "    mask_net {\n        mask_net_module {\n            n_mask_blocks: 3\n"
+            "            mask_block {\n                reduction_ratio: 3\n                hidden_dim: 512\n"
+            "            }\n            use_parallel: true\n" + _mlp("top_mlp", [256, 128, 64], "            ")
+            + "        }\n    }\n"
+            "    metrics {\n        auc {}\n    }\n    losses {\n        binary_cross_entropy {}\n    }\n}\n")
+
+
 def _taobao_features() -> str:
     out = [_id_feature(n, "user", r) for n, r in TAOBAO_USER] + [_id_feature(n, "item", r) for n, r in TAOBAO_ITEM]
     bounds = ", ".join(repr(float(b)) for b in TAOBAO_PRICE_BOUNDARIES)
@@ -178,7 +205,7 @@ def multi_tower_din_taobao() -> str:
 
 
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
-              "multi_tower_din_taobao": multi_tower_din_taobao}
+              "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
 EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}

@@ -467,3 +467,124 @@ def torch_wukong_interaction(x: torch.Tensor, w_fmb: torch.Tensor) -> torch.Tens
 def torch_linear_compress(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
     """LinearCompressBlock.forward (tzrec/modules/interaction.py:255-264): W^T X as [B, l, d]."""
     return (x.permute(0, 2, 1) @ w).permute(0, 2, 1)
+
+
+# ------------------------------------------------------------------------------------------------ MaskNet
+MASKNET_MAX_WIDTH = 1024     # csrc/tzk_masknet.cuh kMaxWidth: pad4(E) and H
+MASKNET_MAX_BLOCKS = 8
+
+
+def _pad4(n: int) -> int:
+    return (n + 3) // 4 * 4
+
+
+def masknet_usable(e: torch.Tensor, E: int, H: int, n_blocks: int, use_parallel: bool) -> bool:
+    """True when the fused MaskNet path (csrc/tzk_masknet.cuh around cuBLASLt GEMMs) covers this module call: parallel
+    blocks, fp32 [B, E] input with pad4(E) <= 1024, 4 <= H <= 1024 and H % 4 == 0, 1 <= n_blocks <= 8, autocast off, on
+    CUDA with the dense GEMM library loaded and TF32 off (on the CPU only a test backend that implements the MaskNet
+    kernels)."""
+    if not use_parallel or autocast_dtype(e) is not None or e.dtype != torch.float32 or e.dim() != 2:
+        return False
+    if e.shape[1] != E or not (1 <= E and _pad4(E) <= MASKNET_MAX_WIDTH and 4 <= H <= MASKNET_MAX_WIDTH and H % 4 == 0
+                               and 1 <= n_blocks <= MASKNET_MAX_BLOCKS):
+        return False
+    if e.is_cuda:
+        from . import dense_gemm
+
+        return _backend is None and dense_gemm.available() and not torch.backends.cuda.matmul.allow_tf32
+    return _backend is not None and hasattr(_backend, "masknet_mask_fwd")
+
+
+class _MaskNetParallel(torch.autograd.Function):
+    """e [B, E] -> hidden [B, nb H] of MaskNetModule's parallel blocks (tzrec/modules/masknet.py:77-85, 142-151).
+
+    Every GEMM operand and result has a row pitch that is a multiple of 4 floats: E travels as Ep = pad4(E) and the
+    aggregation width A as Ap = pad4(A), with zero columns and zero weight rows / columns (their gradients dropped).
+      h  = ReLU(e W1cat^T + b1cat)        one GEMM over all blocks, N = nb Ap, then bias_act
+      m_i = h_i W2_i^T                    into m [B, nb Ep], block i at columns i Ep
+      v, stats = mask_fwd(e, m, b2)       LN(e) * (m_i + b2_i)
+      z_i = v_i W3_i^T                    into z [B, nb H]
+      hidden, stats2 = ffn_fwd(z, b3)     ReLU(LN_H(z_i + b3_i)) in block i's slot of hidden
+    The backward mirrors it; the input gradient is de_ln (mask_bwd) + dh W1cat as one GEMM with beta = 1."""
+
+    @staticmethod
+    def forward(ctx, e, ln_w, ln_b, *params):
+        from . import dense_gemm
+
+        K = backend()
+        nb = len(params) // 8
+        w1s, b1s, w2s, b2s, w3s, b3s, gs, bs = (params[j::8] for j in range(8))
+        B, E = e.shape
+        A, H = w1s[0].shape[0], w3s[0].shape[0]
+        Ep, Ap = _pad4(E), _pad4(A)
+        e_p = e.new_zeros((B, Ep))
+        e_p[:, :E] = e
+        w1cat = e.new_zeros((nb * Ap, Ep))
+        b1cat = e.new_zeros((nb * Ap,))
+        w2p = e.new_zeros((nb, Ep, Ap))
+        w3p = e.new_zeros((nb, H, Ep))
+        for i in range(nb):
+            w1cat[i * Ap:i * Ap + A, :E] = w1s[i]
+            b1cat[i * Ap:i * Ap + A] = b1s[i]
+            w2p[i, :E, :A] = w2s[i]
+            w3p[i, :, :E] = w3s[i]
+        b2cat, b3cat = torch.cat(b2s).contiguous(), torch.cat(b3s).contiguous()
+        gcat, bcat = torch.cat(gs).contiguous(), torch.cat(bs).contiguous()
+        ln_w, ln_b = ln_w.contiguous(), ln_b.contiguous()
+
+        h = dense_gemm.gemm(e_p, False, w1cat, True)
+        if h.is_cuda:
+            K.bias_act(h, b1cat, True)
+        else:
+            h.add_(b1cat).relu_()
+        m = e.new_empty((B, nb * Ep))
+        for i in range(nb):
+            dense_gemm.gemm(h[:, i * Ap:(i + 1) * Ap], False, w2p[i], True, out=m[:, i * Ep:(i + 1) * Ep])
+        v, stats = K.masknet_mask_fwd(e_p, m, b2cat, ln_w, ln_b, E, nb)
+        z = e.new_empty((B, nb * H))
+        for i in range(nb):
+            dense_gemm.gemm(v[:, i * Ep:(i + 1) * Ep], False, w3p[i], True, out=z[:, i * H:(i + 1) * H])
+        hidden, stats2 = K.masknet_ffn_fwd(z, b3cat, gcat, bcat, nb)
+        ctx.save_for_backward(e_p, h, m, v, z, stats, stats2, w1cat, w2p, w3p, b2cat, b3cat, gcat, bcat, ln_w, ln_b)
+        ctx.dims = (nb, E, A, H)
+        return hidden
+
+    @staticmethod
+    def backward(ctx, d_hidden):
+        from . import dense_gemm
+
+        K = backend()
+        e_p, h, m, v, z, stats, stats2, w1cat, w2p, w3p, b2cat, b3cat, gcat, bcat, ln_w, ln_b = ctx.saved_tensors
+        nb, E, A, H = ctx.dims
+        B, Ep = e_p.shape
+        Ap = h.shape[1] // nb
+        dz, dg, dbeta, db3 = K.masknet_ffn_bwd(z, b3cat, gcat, bcat, stats2, d_hidden.contiguous(), nb)
+        dv = e_p.new_empty((B, nb * Ep))
+        dw3 = []
+        for i in range(nb):
+            dz_i = dz[:, i * H:(i + 1) * H]
+            dense_gemm.gemm(dz_i, False, w3p[i], False, out=dv[:, i * Ep:(i + 1) * Ep])
+            dw3.append(dense_gemm.gemm(dz_i, True, v[:, i * Ep:(i + 1) * Ep], False)[:, :E])
+        dm, de_p, db2, dln_w, dln_b = K.masknet_mask_bwd(e_p, m, b2cat, ln_w, ln_b, stats, dv, E, nb)
+        dh = e_p.new_empty((B, nb * Ap))
+        dw2 = []
+        for i in range(nb):
+            dm_i = dm[:, i * Ep:(i + 1) * Ep]
+            dense_gemm.gemm(dm_i, False, w2p[i], False, out=dh[:, i * Ap:(i + 1) * Ap])
+            dw2.append(dense_gemm.gemm(dm_i, True, h[:, i * Ap:(i + 1) * Ap], False)[:E, :A])
+        dh.mul_(h > 0)                                   # ReLU backward of the first mask-generator layer
+        db1 = dh.sum(0)
+        dw1 = dense_gemm.gemm(dh, True, e_p, False)
+        dense_gemm.gemm(dh, False, w1cat, False, out=de_p, beta=1.0)
+        grads = []
+        for i in range(nb):
+            grads += [dw1[i * Ap:i * Ap + A, :E], db1[i * Ap:i * Ap + A], dw2[i], db2[i * E:(i + 1) * E], dw3[i],
+                      db3[i], dg[i], dbeta[i]]
+        return (de_p[:, :E], dln_w, dln_b, *grads)
+
+
+def masknet_parallel(e: torch.Tensor, ln_w: torch.Tensor, ln_b: torch.Tensor, blocks: Sequence[Sequence[torch.Tensor]]):
+    """Fused MaskNetModule body in parallel mode: e [B, E] -> concat_i MaskBlock_i(LN(e), e) [B, nb H].  `blocks` holds
+    per block (W1, b1, W2, b2, W3, b3, gamma, beta) of mask_generator.0, mask_generator.2, ffn.0 and ffn.1.  The caller
+    checks masknet_usable first."""
+    return _MaskNetParallel.apply(e, ln_w, ln_b, *[p for blk in blocks for p in blk])

@@ -1146,6 +1146,75 @@ class CudaKernels:
         self.launches += 1 + int(B > 0)
         return d_fmb, d_base, dparams[:d], dparams[d:]
 
+    # ------------------------------------------------------------------ MaskNet (csrc/tzk_masknet.cuh)
+    # CTAs per SM of each launch (ptxas register counts at 128 threads: mask_fwd 45, mask_bwd 70, ffn_fwd 78,
+    # ffn_bwd 96); the grid fixes the order of the batch sums and depends only on the batch size and the device.
+    def _masknet_grid(self, B: int, per_sm: int, nb: int = 1) -> int:
+        """CTAs along the rows: min(B, per_sm x SMs / nb), nb = the launch's grid.y (one slice per mask block)."""
+        sms = getattr(self, "_sms", None)
+        if sms is None:
+            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
+        return max(1, min(int(B), -(-per_sm * sms // nb)))
+
+    def masknet_mask_fwd(self, e, m, b2, gamma, beta, E: int, nb: int):
+        """e [B, Ep] (first E columns live), m [B, nb Ep] -> (v [B, nb Ep], stats [B, 2]); Ep = pad4(E)."""
+        for t, nm in ((e, "e"), (m, "m"), (b2, "b2"), (gamma, "gamma"), (beta, "beta")):
+            _need(t, torch.float32, nm)
+        B = e.shape[0]
+        v = torch.empty_like(m)
+        stats = torch.empty((B, 2), dtype=torch.float32, device=e.device)
+        check(self._lib.tzk_masknet_mask_fwd(_ptr(e), e.shape[1], _ptr(m), _ptr(b2), _ptr(gamma), _ptr(beta), B, E, nb,
+                                             self._masknet_grid(B, 8), _ptr(v), _ptr(stats), _stream()),
+              "tzk_masknet_mask_fwd")
+        self.launches += int(B > 0)
+        return v, stats
+
+    def masknet_mask_bwd(self, e, m, b2, gamma, beta, stats, dv, E: int, nb: int):
+        """-> (dm [B, nb Ep], de [B, Ep], db2 [nb E], dgamma [E], dbeta [E])."""
+        for t, nm in ((e, "e"), (m, "m"), (b2, "b2"), (gamma, "gamma"), (beta, "beta"), (stats, "stats"),
+                      (dv, "dv")):
+            _need(t, torch.float32, nm)
+        B = e.shape[0]
+        P = (nb + 2) * E
+        grid = self._masknet_grid(B, 6)
+        dm = torch.empty_like(m)
+        de = torch.empty_like(e)
+        partials = self._workspace("masknet_mask_bwd", grid * P * 4, e.device)
+        dparams = torch.empty(P, dtype=torch.float32, device=e.device)
+        check(self._lib.tzk_masknet_mask_bwd(_ptr(e), e.shape[1], _ptr(m), _ptr(b2), _ptr(gamma), _ptr(beta),
+                                             _ptr(stats), _ptr(dv), B, E, nb, grid, _ptr(dm), _ptr(de),
+                                             _ptr(partials), _ptr(dparams), _stream()), "tzk_masknet_mask_bwd")
+        self.launches += 1 + int(B > 0)
+        return dm, de, dparams[:nb * E], dparams[nb * E:(nb + 1) * E], dparams[(nb + 1) * E:]
+
+    def masknet_ffn_fwd(self, z, b3, gamma, beta, nb: int):
+        """z [B, nb H] -> (y [B, nb H] = ReLU(LN_H(z_i + b3_i)) per block, stats [B, nb, 2])."""
+        for t, nm in ((z, "z"), (b3, "b3"), (gamma, "gamma"), (beta, "beta")):
+            _need(t, torch.float32, nm)
+        B, H = z.shape[0], z.shape[1] // nb
+        y = torch.empty_like(z)
+        stats = torch.empty((B, nb, 2), dtype=torch.float32, device=z.device)
+        check(self._lib.tzk_masknet_ffn_fwd(_ptr(z), _ptr(b3), _ptr(gamma), _ptr(beta), B, H, nb,
+                                            self._masknet_grid(B, 6, nb), _ptr(y), _ptr(stats), _stream()),
+              "tzk_masknet_ffn_fwd")
+        self.launches += int(B > 0)
+        return y, stats
+
+    def masknet_ffn_bwd(self, z, b3, gamma, beta, stats, dy, nb: int):
+        """-> (dz [B, nb H], dgamma [nb, H], dbeta [nb, H], db3 [nb, H])."""
+        for t, nm in ((z, "z"), (b3, "b3"), (gamma, "gamma"), (beta, "beta"), (stats, "stats"), (dy, "dy")):
+            _need(t, torch.float32, nm)
+        B, H = z.shape[0], z.shape[1] // nb
+        grid = self._masknet_grid(B, 5, nb)
+        dz = torch.empty_like(z)
+        partials = self._workspace("masknet_ffn_bwd", nb * grid * 3 * H * 4, z.device)
+        dparams = torch.empty((nb, 3, H), dtype=torch.float32, device=z.device)
+        check(self._lib.tzk_masknet_ffn_bwd(_ptr(z), _ptr(b3), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(dy), B, H,
+                                            nb, grid, _ptr(dz), _ptr(partials), _ptr(dparams), _stream()),
+              "tzk_masknet_ffn_bwd")
+        self.launches += 1 + int(B > 0)
+        return dz, dparams[:, 0], dparams[:, 1], dparams[:, 2]
+
 
 @dataclass
 class ColPlan:

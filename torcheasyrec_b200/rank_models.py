@@ -10,6 +10,7 @@ from typing import Any, Dict, List, Optional
 
 import contextlib
 import os
+import struct
 
 import torch
 import torch.nn.functional as F
@@ -726,8 +727,125 @@ class WuKong(RankModel):
         return self._output_to_prediction(y)
 
 
+def proto_float32(v: float) -> float:
+    """A `float` proto field as MessageToDict hands it to config_to_kwargs (protobuf's ToShortestFloat): the fewest
+    significant digits, from 6 up, that round-trip the stored float32 (0.3 stays 0.3, not 0.30000001192...)."""
+    f32 = struct.unpack("f", struct.pack("f", float(v)))[0]
+    precision = 6
+    rounded = float(f"{f32:.{precision}g}")
+    while struct.unpack("f", struct.pack("f", rounded))[0] != f32:
+        precision += 1
+        rounded = float(f"{f32:.{precision}g}")
+    return rounded
+
+
+class MaskBlock(nn.Module):
+    """tzrec/modules/masknet.py:20-85: ffn(feature_input * mask_generator(mask_input)), with the reference's
+    aggregation-width rule (reduction_ratio, when non-zero, overrides aggregation_dim) and its checks."""
+
+    def __init__(self, input_dim: int, mask_input_dim: int, hidden_dim: int, reduction_ratio: float = 1.0,
+                 aggregation_dim: int = 0) -> None:
+        super().__init__()
+        if not aggregation_dim and not reduction_ratio:
+            raise ValueError("Either aggregation_dim or reduction_ratio must be provided.")
+        if aggregation_dim:
+            self.aggregation_dim = aggregation_dim
+        if reduction_ratio:
+            self.aggregation_dim = int(input_dim * reduction_ratio)
+        assert self.aggregation_dim > 0, "aggregation_dim must be > 0, check your aggregation_dim or "
+        self.mask_generator = nn.Sequential(_Linear(mask_input_dim, self.aggregation_dim), nn.ReLU(),
+                                            _Linear(self.aggregation_dim, input_dim))
+        assert hidden_dim > 0, "hidden_dim must be > 0."
+        self._hidden_dim = hidden_dim
+        self.ffn = nn.Sequential(_Linear(input_dim, hidden_dim), nn.LayerNorm(hidden_dim), nn.ReLU())
+
+    def output_dim(self) -> int:
+        return self._hidden_dim
+
+    def fused_params(self):
+        """(W1, b1, W2, b2, W3, b3, gamma, beta) in Fn.masknet_parallel's order."""
+        g0, g2, f0, f1 = self.mask_generator[0], self.mask_generator[2], self.ffn[0], self.ffn[1]
+        return (g0.weight, g0.bias, g2.weight, g2.bias, f0.weight, f0.bias, f1.weight, f1.bias)
+
+    def forward(self, feature_input: torch.Tensor, mask_input: torch.Tensor) -> torch.Tensor:
+        weights = self.mask_generator(mask_input)
+        return self.ffn(feature_input * weights)
+
+
+class MaskNetModule(nn.Module):
+    """tzrec/modules/masknet.py:88-161.  In parallel mode, when Fn.masknet_usable holds, the blocks run as
+    Fn.masknet_parallel: the mask generators' first layers as one GEMM, LN(e) * mask and the FFN's bias + LayerNorm +
+    ReLU as fused kernels (csrc/tzk_masknet.cuh), every GEMM on 16-B aligned rows.  Serial mode, autocast, and shapes
+    outside the kernels' cover take the reference's torch formulation."""
+
+    def __init__(self, feature_dim: int, n_mask_blocks: int, mask_block: Dict[str, Any],
+                 top_mlp: Optional[Dict[str, Any]] = None, use_parallel: bool = True, **kwargs: Any) -> None:
+        super().__init__(**kwargs)
+        mask_block = dict(mask_block)
+        if "reduction_ratio" in mask_block:
+            mask_block["reduction_ratio"] = proto_float32(mask_block["reduction_ratio"])
+        self.ln_emb = nn.LayerNorm(feature_dim)
+        self.use_parallel = use_parallel
+        if self.use_parallel:
+            self.mask_blocks = nn.ModuleList([MaskBlock(feature_dim, feature_dim, **mask_block)
+                                              for _ in range(n_mask_blocks)])
+            self._output_dim = self.mask_blocks[0].output_dim() * n_mask_blocks
+        else:
+            self.mask_blocks = nn.ModuleList()
+            self._output_dim = feature_dim
+            for i in range(n_mask_blocks):
+                self.mask_blocks.append(MaskBlock(self._output_dim, feature_dim, **mask_block))
+                self._output_dim = self.mask_blocks[i].output_dim()
+        self.top_mlp = None
+        if top_mlp:
+            self.top_mlp = MLP(in_features=self._output_dim, **top_mlp)
+            self._output_dim = self.top_mlp.output_dim()
+
+    def output_dim(self) -> int:
+        return self._output_dim
+
+    def fused_usable(self, feature_emb: torch.Tensor) -> bool:
+        blk = self.mask_blocks[0] if len(self.mask_blocks) else None
+        return blk is not None and Fn.masknet_usable(feature_emb, self.ln_emb.normalized_shape[0], blk.output_dim(),
+                                                     len(self.mask_blocks), self.use_parallel)
+
+    def forward(self, feature_emb: torch.Tensor) -> torch.Tensor:
+        if self.fused_usable(feature_emb):
+            hidden = Fn.masknet_parallel(feature_emb, self.ln_emb.weight, self.ln_emb.bias,
+                                         [blk.fused_params() for blk in self.mask_blocks])
+        else:
+            ln_emb = self.ln_emb(feature_emb)
+            if self.use_parallel:
+                hidden = torch.concat([blk(ln_emb, feature_emb) for blk in self.mask_blocks], dim=-1)
+            else:
+                hidden = self.mask_blocks[0](ln_emb, feature_emb)
+                for i in range(1, len(self.mask_blocks)):
+                    hidden = self.mask_blocks[i](hidden, feature_emb)
+        if self.top_mlp is not None:
+            hidden = self.top_mlp(hidden)
+        return hidden
+
+
+class MaskNet(RankModel):
+    """tzrec/models/masknet.py:25-71: the first feature group through MaskNetModule and a bias-less output Linear."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self.init_input()
+        self.group_name = self.embedding_group.group_names()[0]
+        feature_dim = self.embedding_group.group_total_dim(self.group_name)
+        masknet_config = self._model_config.mask_net_module
+        self.mask_net_layer = MaskNetModule(feature_dim, **config_to_kwargs(masknet_config))
+        self.output_linear = _Linear(masknet_config.top_mlp.hidden_units[-1], self._num_class, bias=False)
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        features = self.build_input(batch)[self.group_name]
+        hidden = self.mask_net_layer(features)
+        return self._output_to_prediction(self.output_linear(hidden))
+
+
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
-                 "mmoe": MMoE, "wukong": WuKong}
+                 "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet}
 
 
 def create_model(model_config: Message, features: List[BaseFeature], labels: List[str], device=None) -> RankModel:
