@@ -627,6 +627,44 @@ int tzk_masknet_ffn_bwd(const float* z, const float* b3, const float* gamma, con
                         const float* dy, int64_t B, int32_t H, int32_t nb, int32_t grid, float* dz, float* partials,
                         float* dparams, tzk_stream_t stream);
 
+/* ---- PLE: the gates of one extraction layer (tzrec/modules/extraction_net.py:93-105 `_gate_forward`, called at
+ * :120-133), all of them in one launch each way.  n_gates gates (the T task gates, then the shared gate when the layer
+ * is not the last); gate g reads input gate_input[g] (one of n_inputs distinct [B, in_dim[i]] tensors) and mixes the
+ * gate_num_experts[g] experts listed in gate_experts[g] (indices into the n_experts [B, H] expert outputs, in the
+ * reference's stack order).  Gate weights [E_g, K_g] and biases [E_g] of nn.Linear.  fp32 row-major, fp32 FFMA.
+ * Cover: 1 <= n_gates <= 9, n_experts <= 64, 1 <= E_g <= 32 distinct experts, 1 <= H <= 1024, 1 <= K_i <= 1024, and
+ * sum_g E_g K_g <= 20480 floats (the weights stay in shared memory; the backward holds them and their gradient).
+ * The description travels by value as a kernel parameter (no host-to-device copy: graph-capturable); its device
+ * pointers are read when the call is made.
+ *   gate_fwd: -> y [n_gates, B, H] (y_g = sum_e softmax(x_g W_g^T + b_g)_e expert_e), p [B, sum E_g] (the softmax,
+ *             gate g at column sum_{g' < g} E_g').
+ *   gate_bwd: dy [n_gates, B, H] -> d_experts [n_experts, B, H] (written once per element, the gates summed in
+ *             order), d_inputs[i] [B, K_i] (sum over the gates reading input i), dparams = dW_0 | dW_1 | ... | db_0 |
+ *             db_1 | ... (sum_g E_g K_g + sum_g E_g floats): per-CTA partials (grid rows of that size) reduced in CTA
+ *             order, no float atomics.
+ *   gate_smem_bytes: dynamic shared memory of one CTA of the forward (backward = 0) or the backward (1) launch; 0 when
+ *             the description is outside the cover.  Needs no GPU. */
+#define TZK_PLE_MAX_GATES 9
+#define TZK_PLE_MAX_EXPERTS 64
+#define TZK_PLE_MAX_GATE_EXPERTS 32
+typedef struct tzk_ple_gate_args {
+  int64_t B;
+  int32_t H, n_experts, n_inputs, n_gates;
+  int32_t in_dim[TZK_PLE_MAX_GATES];
+  int32_t gate_input[TZK_PLE_MAX_GATES];
+  int32_t gate_num_experts[TZK_PLE_MAX_GATES];
+  uint8_t gate_experts[TZK_PLE_MAX_GATES][TZK_PLE_MAX_GATE_EXPERTS];
+  const float* experts[TZK_PLE_MAX_EXPERTS];
+  const float* inputs[TZK_PLE_MAX_GATES];
+  const float* weight[TZK_PLE_MAX_GATES];
+  const float* bias[TZK_PLE_MAX_GATES];
+  float* d_inputs[TZK_PLE_MAX_GATES]; /* gate_bwd only */
+} tzk_ple_gate_args;
+int64_t tzk_ple_gate_smem_bytes(const tzk_ple_gate_args* args_host, int32_t backward);
+int tzk_ple_gate_fwd(const tzk_ple_gate_args* args_host, int32_t grid, float* y, float* p, tzk_stream_t stream);
+int tzk_ple_gate_bwd(const tzk_ple_gate_args* args_host, const float* p, const float* dy, int32_t grid,
+                     float* d_experts, float* partials, float* dparams, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,6 +22,21 @@ class TzkOptArgs(ctypes.Structure):
                 ("eta", c_float), ("weight_decay_mode", c_int32), ("per_sample_weights", c_void_p)]
 
 
+PLE_MAX_GATES, PLE_MAX_EXPERTS, PLE_MAX_GATE_EXPERTS = 9, 64, 32
+
+
+class TzkPleGateArgs(ctypes.Structure):
+    """struct tzk_ple_gate_args (include/tzk.h): one PLE extraction layer's gates."""
+
+    _fields_ = [("B", c_int64), ("H", c_int32), ("n_experts", c_int32), ("n_inputs", c_int32), ("n_gates", c_int32),
+                ("in_dim", c_int32 * PLE_MAX_GATES), ("gate_input", c_int32 * PLE_MAX_GATES),
+                ("gate_num_experts", c_int32 * PLE_MAX_GATES),
+                ("gate_experts", (ctypes.c_uint8 * PLE_MAX_GATE_EXPERTS) * PLE_MAX_GATES),
+                ("experts", c_void_p * PLE_MAX_EXPERTS), ("inputs", c_void_p * PLE_MAX_GATES),
+                ("weight", c_void_p * PLE_MAX_GATES), ("bias", c_void_p * PLE_MAX_GATES),
+                ("d_inputs", c_void_p * PLE_MAX_GATES)]
+
+
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
 SIGNATURES = {
     "tzk_abi_version": (c_int32, []),
@@ -176,6 +191,10 @@ SIGNATURES = {
         c_int32, [P, c_int32, P, P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P, P, P]),
     "tzk_masknet_ffn_fwd": (c_int32, [P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P]),
     "tzk_masknet_ffn_bwd": (c_int32, [P, P, P, P, P, P, c_int64, c_int32, c_int32, c_int32, P, P, P, P]),
+    # PLE: every gate of one extraction layer, forward and backward (the layer described by TzkPleGateArgs)
+    "tzk_ple_gate_smem_bytes": (c_int64, [P, c_int32]),
+    "tzk_ple_gate_fwd": (c_int32, [P, c_int32, P, P, P]),
+    "tzk_ple_gate_bwd": (c_int32, [P, P, P, c_int32, P, P, P, P]),
 }
 
 _lib = None

@@ -130,7 +130,7 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "train_metrics": _f("TrainMetricConfig", rep=True), "kernel": _f(E, "PYTORCH"),
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
-                  "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet"}.get(k, "Generic"))
+                  "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE"}.get(k, "Generic"))
            for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
@@ -154,6 +154,9 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     "DINTower": {"input": _f(S), "attn_mlp": _f("MLP")},
     "MMoE": {"expert_mlp": _f("MLP"), "gate_mlp": _f("MLP"), "num_expert": _f(I, 3),
              "task_towers": _f("TaskTower", rep=True)},
+    "PLE": {"extraction_networks": _f("ExtractionNetwork", rep=True), "task_towers": _f("TaskTower", rep=True)},
+    "ExtractionNetwork": {"network_name": _f(S), "expert_num_per_task": _f(I), "share_num": _f(I, 0),
+                          "task_expert_net": _f("MLP"), "share_expert_net": _f("MLP")},
     "TaskTower": {"tower_name": _f(S), "label_name": _f(S), "metrics": _f("MetricConfig", rep=True),
                   "train_metrics": _f("TrainMetricConfig", rep=True), "losses": _f("LossConfig", rep=True),
                   "num_class": _f(I, 1), "mlp": _f("MLP"), "weight": _f(F, 1.0), "sample_weight_name": _f(S)},

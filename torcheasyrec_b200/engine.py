@@ -47,7 +47,7 @@ class Pipeline:
                  static_capacity: Optional[float] = None, exchange: str = "nccl") -> None:
         """`config`: path of a pipeline .config/.json, or the name of a built-in example
         (example_configs.BUILTINS: dlrm_criteo, deepfm_criteo, mmoe_taobao, multi_tower_din_taobao, masknet_criteo,
-        wukong_criteo)."""
+        ple_taobao, wukong_criteo)."""
         from . import example_configs
         from .config import parse_text
 

@@ -1,5 +1,5 @@
 """Generators for the pipeline configs BASELINE.json names (text format, same message tree as the reference's
-examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo}.config).
+examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo,ple_taobao}.config).
 
 The package does not depend on the reference's files, so the configs are re-derived here from their defining facts
 (SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table list and price boundaries, and the model
@@ -183,6 +183,25 @@ def mmoe_taobao() -> str:
             + _task_tower("ctr", "clk", None) + _task_tower("cvr", "buy", 1000) + "    }\n}\n")
 
 
+def _extraction_network(name: str, n: int, units: Sequence[int]) -> str:
+    return ("        extraction_networks {\n" f'            network_name: "{name}"\n'
+            f"            expert_num_per_task: {n}\n            share_num: {n}\n"
+            + _mlp("task_expert_net", units, "            ") + _mlp("share_expert_net", units, "            ")
+            + "        }\n")
+
+
+def ple_taobao() -> str:
+    """examples/ple_taobao.config: mmoe_taobao's features, group `all` and towers ctr/cvr; ple{3 extraction networks:
+    2 + 2 experts 1024-512-256, 3 + 3 experts 256-128-64, 4 + 4 experts 128-64-32 (per task + shared)}."""
+    return (_header("taobao_multitask_sample_v1_train", "taobao_multitask_sample_v1/ds=20170513", "ple_taobao",
+                    "FG_DAG", ["clk", "buy"], None, quota=False)
+            + _taobao_features()
+            + "model_config {\n" + _group("all", TAOBAO_MMOE_ORDER, "DEEP")
+            + "    ple {\n" + _extraction_network("layer1", 2, [1024, 512, 256])
+            + _extraction_network("layer2", 3, [256, 128, 64]) + _extraction_network("layer3", 4, [128, 64, 32])
+            + _task_tower("ctr", "clk", None) + _task_tower("cvr", "buy", 1000) + "    }\n}\n")
+
+
 def multi_tower_din_taobao() -> str:
     """examples/multi_tower_din_taobao.config: group deep (16) + SEQUENCE group seq (3 queries + click_50_seq)."""
     seq_feats = "".join(
@@ -205,7 +224,8 @@ def multi_tower_din_taobao() -> str:
 
 
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
-              "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo}
+              "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo,
+              "ple_taobao": ple_taobao}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
 EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}

@@ -588,3 +588,87 @@ def masknet_parallel(e: torch.Tensor, ln_w: torch.Tensor, ln_b: torch.Tensor, bl
     per block (W1, b1, W2, b2, W3, b3, gamma, beta) of mask_generator.0, mask_generator.2, ffn.0 and ffn.1.  The caller
     checks masknet_usable first."""
     return _MaskNetParallel.apply(e, ln_w, ln_b, *[p for blk in blocks for p in blk])
+
+
+# ------------------------------------------------------------------------------------------------ PLE gates
+PLE_MAX_GATES = 9             # csrc/tzk_ple.cuh: T <= 8 task gates + the shared gate
+PLE_MAX_EXPERTS = 64
+PLE_MAX_GATE_EXPERTS = 32
+PLE_MAX_WIDTH = 1024          # H and K
+PLE_MAX_WEIGHT_FLOATS = 20480  # sum_g E_g K_g, the gate weights held in shared memory
+
+
+def ple_gate_usable(inputs: Sequence[torch.Tensor], gate_input: Sequence[int], weights: Sequence[torch.Tensor],
+                    experts: Sequence[torch.Tensor], gate_experts: Sequence[Sequence[int]]) -> bool:
+    """True when the fused gate kernels (csrc/tzk_ple.cuh) cover this extraction layer: fp32 2-D tensors, autocast off,
+    at most 9 gates over at most 64 experts of one [B, H] shape with 1 <= H <= 1024, each gate over 1..32 distinct
+    experts and an input of width 1 <= K <= 1024, sum_g E_g K_g <= 20480, on CUDA (on the CPU only a test backend that
+    implements the PLE kernels)."""
+    t = experts[0] if len(experts) else None
+    if t is None or autocast_dtype(t) is not None:
+        return False
+    if any(x.dtype != torch.float32 or x.dim() != 2 or x.device != t.device
+           for x in (*inputs, *experts, *weights)):
+        return False
+    B, H = t.shape
+    if any(tuple(e.shape) != (B, H) for e in experts) or any(x.shape[0] != B for x in inputs):
+        return False
+    if not (1 <= len(gate_input) <= PLE_MAX_GATES and len(experts) <= PLE_MAX_EXPERTS and 1 <= H <= PLE_MAX_WIDTH
+            and all(1 <= x.shape[1] <= PLE_MAX_WIDTH for x in inputs)):
+        return False
+    total = 0
+    for g, ids in enumerate(gate_experts):
+        K = inputs[gate_input[g]].shape[1]
+        if not (1 <= len(ids) <= PLE_MAX_GATE_EXPERTS and len(set(ids)) == len(ids)
+                and tuple(weights[g].shape) == (len(ids), K)):
+            return False
+        total += len(ids) * K
+    if total > PLE_MAX_WEIGHT_FLOATS:
+        return False
+    return t.is_cuda or (_backend is not None and hasattr(_backend, "ple_gate_fwd"))
+
+
+class _PleGates(torch.autograd.Function):
+    """Every gate of one extraction layer: y_g = softmax(x_g W_g^T + b_g) @ stack(experts of g), as [n_gates, B, H]."""
+
+    @staticmethod
+    def forward(ctx, spec, *tensors):
+        gate_input, gate_experts, n_in, n_exp = spec
+        G = len(gate_input)
+        inputs = [x.contiguous() for x in tensors[:n_in]]
+        weights = [w.contiguous() for w in tensors[n_in:n_in + G]]
+        biases = [b.contiguous() for b in tensors[n_in + G:n_in + 2 * G]]
+        experts = [e.contiguous() for e in tensors[n_in + 2 * G:]]
+        y, p = backend().ple_gate_fwd(inputs, gate_input, weights, biases, experts, gate_experts)
+        ctx.save_for_backward(*inputs, *weights, *biases, *experts, p)
+        ctx.spec = spec
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        gate_input, gate_experts, n_in, n_exp = ctx.spec
+        G = len(gate_input)
+        saved = ctx.saved_tensors
+        inputs, weights = list(saved[:n_in]), list(saved[n_in:n_in + G])
+        biases, experts, p = list(saved[n_in + G:n_in + 2 * G]), list(saved[n_in + 2 * G:-1]), saved[-1]
+        d_inputs, d_experts, dW, db = backend().ple_gate_bwd(inputs, gate_input, weights, biases, experts,
+                                                             gate_experts, p, dy.contiguous())
+        return (None, *d_inputs, *dW, *db, *d_experts.unbind(0))
+
+
+def ple_gates(inputs: Sequence[torch.Tensor], gate_input: Sequence[int], weights: Sequence[torch.Tensor],
+              biases: Sequence[torch.Tensor], experts: Sequence[torch.Tensor],
+              gate_experts: Sequence[Sequence[int]]) -> List[torch.Tensor]:
+    """Fused gates of one PLE extraction layer (csrc/tzk_ple.cuh): gate g reads inputs[gate_input[g]] through the
+    Linear (weights[g], biases[g]) and mixes experts[gate_experts[g]] in that order -> [y_g [B, H] per gate].  The
+    caller checks ple_gate_usable first."""
+    spec = (tuple(gate_input), tuple(tuple(ids) for ids in gate_experts), len(inputs), len(experts))
+    y = _PleGates.apply(spec, *inputs, *weights, *biases, *experts)
+    return list(y.unbind(0))
+
+
+def torch_ple_gate(selector: torch.Tensor, experts: Sequence[torch.Tensor], gate: torch.nn.Module) -> torch.Tensor:
+    """ExtractionNet._gate_forward (tzrec/modules/extraction_net.py:93-105): the reference's torch formulation."""
+    vec = torch.stack(list(experts), dim=1)
+    g = torch.softmax(gate(selector), dim=1).unsqueeze(1)
+    return torch.matmul(g, vec).squeeze(1)

@@ -1215,6 +1215,86 @@ class CudaKernels:
         self.launches += 1 + int(B > 0)
         return dz, dparams[:, 0], dparams[:, 1], dparams[:, 2]
 
+    # ------------------------------------------------------------------ PLE gates (csrc/tzk_ple.cuh)
+    # Resident CTAs per SM: ptxas register counts at 256 threads (gate_fwd 58 -> 4, gate_bwd 79 -> 3), fewer when the
+    # layer's shared memory (tzk_ple_gate_smem_bytes) allows fewer.  The grid fixes the order of the batch sums and
+    # depends only on the batch size, the layer's shapes and the device.
+    def _ple_args(self, inputs, gate_input, weights, biases, experts, gate_experts, d_inputs=None):
+        from ._lib import TzkPleGateArgs
+
+        a = TzkPleGateArgs()
+        a.B, a.H = experts[0].shape[0], experts[0].shape[1]
+        a.n_experts, a.n_inputs, a.n_gates = len(experts), len(inputs), len(gate_input)
+        for i, x in enumerate(inputs):
+            _need(x, torch.float32, f"inputs[{i}]")
+            a.in_dim[i], a.inputs[i] = x.shape[1], x.data_ptr()
+            if d_inputs is not None:
+                a.d_inputs[i] = d_inputs[i].data_ptr()
+        for j, e in enumerate(experts):
+            _need(e, torch.float32, f"experts[{j}]")
+            if tuple(e.shape) != (a.B, a.H):
+                raise TzkError("ple gates: every expert output must have the same [B, H] shape")
+            a.experts[j] = e.data_ptr()
+        for g, (w, b) in enumerate(zip(weights, biases)):
+            _need(w, torch.float32, f"weight[{g}]")
+            _need(b, torch.float32, f"bias[{g}]")
+            a.gate_input[g], a.gate_num_experts[g] = gate_input[g], len(gate_experts[g])
+            for e, x in enumerate(gate_experts[g]):
+                a.gate_experts[g][e] = x
+            a.weight[g], a.bias[g] = w.data_ptr(), b.data_ptr()
+        return a
+
+    def _ple_grid(self, a, B: int, rows_per_cta: int, per_sm_regs: int, backward: int) -> int:
+        sms = getattr(self, "_sms", None)
+        if sms is None:
+            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
+        smem = int(self._lib.tzk_ple_gate_smem_bytes(ctypes.byref(a), backward))
+        if smem == 0:
+            raise TzkError("ple gates: layer outside the kernels' cover (Fn.ple_gate_usable)")
+        per_sm = max(1, min(per_sm_regs, (227 * 1024) // (smem + 1024)))
+        return max(1, min(-(-int(B) // rows_per_cta), per_sm * sms))
+
+    def ple_gate_fwd(self, inputs, gate_input, weights, biases, experts, gate_experts):
+        """One extraction layer's gates -> (y [n_gates, B, H], p [B, sum E_g] the softmax of every gate)."""
+        a = self._ple_args(inputs, gate_input, weights, biases, experts, gate_experts)
+        B, H, G = a.B, a.H, a.n_gates
+        dev = experts[0].device
+        y = torch.empty((G, B, H), dtype=torch.float32, device=dev)
+        p = torch.empty((B, sum(len(e) for e in gate_experts)), dtype=torch.float32, device=dev)
+        grid = self._ple_grid(a, B, 8, 4, 0)
+        check(self._lib.tzk_ple_gate_fwd(ctypes.byref(a), grid, _ptr(y), _ptr(p), _stream()), "tzk_ple_gate_fwd")
+        self.launches += int(B > 0)
+        return y, p
+
+    def ple_gate_bwd(self, inputs, gate_input, weights, biases, experts, gate_experts, p, dy):
+        """dy [n_gates, B, H] -> (d_inputs [B, K_i] per input, d_experts [n_experts, B, H], dW_g per gate, db_g per
+        gate)."""
+        _need(p, torch.float32, "p")
+        _need(dy, torch.float32, "dy")
+        d_inputs = [torch.empty_like(x) for x in inputs]
+        a = self._ple_args(inputs, gate_input, weights, biases, experts, gate_experts, d_inputs)
+        B, H = a.B, a.H
+        dev = experts[0].device
+        sizes = [w.numel() for w in weights]
+        Es = [len(e) for e in gate_experts]
+        P = sum(sizes) + sum(Es)
+        grid = self._ple_grid(a, B, 16, 3, 1)
+        d_experts = torch.empty((len(experts), B, H), dtype=torch.float32, device=dev)
+        partials = self._workspace("ple_gate_bwd", grid * P * 4, dev)
+        dparams = torch.empty(P, dtype=torch.float32, device=dev)
+        check(self._lib.tzk_ple_gate_bwd(ctypes.byref(a), _ptr(p), _ptr(dy), grid, _ptr(d_experts), _ptr(partials),
+                                         _ptr(dparams), _stream()), "tzk_ple_gate_bwd")
+        self.launches += 1 + int(B > 0)
+        dW, o = [], 0
+        for w, n in zip(weights, sizes):
+            dW.append(dparams[o:o + n].view_as(w))
+            o += n
+        db = []
+        for e in Es:
+            db.append(dparams[o:o + e])
+            o += e
+        return d_inputs, d_experts, dW, db
+
 
 @dataclass
 class ColPlan:

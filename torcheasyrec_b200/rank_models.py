@@ -1,4 +1,4 @@
-"""Model shells that consume the hot path: DLRM, DeepFM, MMoE, MultiTowerDIN (+ their dense blocks).
+"""Model shells that consume the hot path: DLRM, DeepFM, MMoE, PLE, MultiTowerDIN (+ their dense blocks).
 
 These are the callers of §8a rows A7-A10 (SURVEY.md §2 row 4): tzrec/models/{rank_model,dlrm,deepfm,mmoe,
 multi_tower_din,multi_task_rank}.py and the dense blocks of tzrec/modules/{mlp,mmoe,sequence,task_tower}.py.
@@ -553,23 +553,15 @@ class MultiTowerDIN(RankModel):
         return self._output_to_prediction(self.output_mlp(x))
 
 
-class MMoE(RankModel):
-    """tzrec/models/mmoe.py:24-86 + multi_task_rank.py:50-65 (one BCE loss per tower, summed)."""
+class MultiTaskRank(RankModel):
+    """tzrec/models/multi_task_rank.py:25-196 for BCE towers: one prediction pair, loss, and metric head per task tower
+    (suffix `_<tower_name>`).  What the reference honours per tower and this repo does not (sample weights, task-space
+    indicator labels, non-BCE losses) is refused at construction instead of silently training with plain mean BCE."""
 
     def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
         super().__init__(model_config, features, labels, sample_weights, **kwargs)
         self._task_tower_cfgs = list(self._model_config.task_towers)
-        self.init_input()
-        self.group_name = self.embedding_group.group_names()[0]
-        self.mmoe = MMoEModule(
-            in_features=self.embedding_group.group_total_dim(self.group_name),
-            expert_mlp=config_to_kwargs(self._model_config.expert_mlp), num_expert=self._model_config.num_expert,
-            num_task=len(self._task_tower_cfgs),
-            gate_mlp=config_to_kwargs(self._model_config.gate_mlp) if self._model_config.HasField("gate_mlp") else None)
-        self._task_tower = nn.ModuleList()
         for cfg in self._task_tower_cfgs:
-            # what the reference honours per tower (models/multi_task_rank.py:97-125) and this repo does not: refuse it
-            # instead of silently training with plain mean BCE
             for fld in ("sample_weight_name", "task_space_indicator_label"):
                 if cfg._spec(fld) is not None and cfg.HasField(fld) and getattr(cfg, fld):
                     raise NotImplementedError(f"task tower {cfg.tower_name}: {fld} is outside the hot-path scope")
@@ -577,15 +569,12 @@ class MMoE(RankModel):
                 if lc.WhichOneof("loss") not in (None, "binary_cross_entropy"):
                     raise NotImplementedError(f"task tower {cfg.tower_name}: loss {lc.WhichOneof('loss')} is outside "
                                               "the hot-path scope (BCE-with-logits only)")
-            mlp = config_to_kwargs(cfg.mlp) if cfg.HasField("mlp") else None
-            self._task_tower.append(TaskTower(self.mmoe.output_dim(), cfg.num_class, mlp=mlp))
 
-    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
-        grouped = self.build_input(batch)
-        task_inputs = self.mmoe(grouped[self.group_name])
+    def _multi_task_output_to_prediction(self, tower_outputs: List[torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """multi_task_rank.py:50-65: tower i's output under the suffix `_<tower_name>`."""
         preds = {}
-        for i, cfg in enumerate(self._task_tower_cfgs):
-            preds.update(self._output_to_prediction(self._task_tower[i](task_inputs[i]), suffix=f"_{cfg.tower_name}"))
+        for cfg, out in zip(self._task_tower_cfgs, tower_outputs):
+            preds.update(self._output_to_prediction(out, suffix=f"_{cfg.tower_name}"))
         return preds
 
     def _metric_heads(self):
@@ -601,6 +590,129 @@ class MMoE(RankModel):
             out[f"binary_cross_entropy_{cfg.tower_name}"] = cfg.weight * bce_with_logits(
                 predictions[f"logits_{cfg.tower_name}"], label)
         return out
+
+
+class MMoE(MultiTaskRank):
+    """tzrec/models/mmoe.py:24-86 + multi_task_rank.py:50-65 (one BCE loss per tower, summed)."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self.init_input()
+        self.group_name = self.embedding_group.group_names()[0]
+        self.mmoe = MMoEModule(
+            in_features=self.embedding_group.group_total_dim(self.group_name),
+            expert_mlp=config_to_kwargs(self._model_config.expert_mlp), num_expert=self._model_config.num_expert,
+            num_task=len(self._task_tower_cfgs),
+            gate_mlp=config_to_kwargs(self._model_config.gate_mlp) if self._model_config.HasField("gate_mlp") else None)
+        self._task_tower = nn.ModuleList()
+        for cfg in self._task_tower_cfgs:
+            mlp = config_to_kwargs(cfg.mlp) if cfg.HasField("mlp") else None
+            self._task_tower.append(TaskTower(self.mmoe.output_dim(), cfg.num_class, mlp=mlp))
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        grouped = self.build_input(batch)
+        task_inputs = self.mmoe(grouped[self.group_name])
+        return self._multi_task_output_to_prediction([tower(x) for tower, x in zip(self._task_tower, task_inputs)])
+
+
+class ExtractionNet(nn.Module):
+    """tzrec/modules/extraction_net.py:20-133: one PLE extraction layer.  `expert_num_per_task` experts per task on that
+    task's input and `share_num` shared experts on the shared input (each an MLP); task gate i mixes
+    [task i experts..., shared experts...], the shared gate (not in the last layer) mixes [every task expert...,
+    shared experts...].  When Fn.ple_gate_usable holds, all of the layer's gates run as one fused call
+    (Fn.ple_gates, csrc/tzk_ple.cuh); otherwise the reference's torch formulation."""
+
+    def __init__(self, in_extraction_networks: List[int], in_shared_expert: int, network_name: str, share_num: int,
+                 expert_num_per_task: int, share_expert_net: Dict[str, Any], task_expert_net: Dict[str, Any],
+                 final_flag: bool = False) -> None:
+        super().__init__()
+        self.name = network_name
+        self._final_flag = final_flag
+        self._shared_layers = nn.ModuleList([MLP(in_shared_expert, **share_expert_net) for _ in range(share_num)])
+        self._shared_gate = None
+        if not final_flag:
+            self._shared_gate = nn.Linear(in_shared_expert, len(in_extraction_networks) * expert_num_per_task + share_num)
+        self._task_layers = nn.ModuleList()
+        self._task_gates = nn.ModuleList()
+        self._output_dims = []
+        for in_feature in in_extraction_networks:
+            self._task_layers.append(nn.ModuleList([MLP(in_feature, **task_expert_net)
+                                                    for _ in range(expert_num_per_task)]))
+            self._task_gates.append(nn.Linear(in_feature, expert_num_per_task + share_num))
+            self._output_dims.append(task_expert_net["hidden_units"][-1])
+        self._output_dims.append(share_expert_net["hidden_units"][-1])
+
+    def output_dim(self) -> List[int]:
+        return self._output_dims
+
+    def gate_layout(self):
+        """(gate_input, gate_experts) of Fn.ple_gates for the layer's experts in the order
+        [task 0 experts..., task 1 experts..., ..., shared experts...]; input 0 is the shared input, input 1 + i task
+        i's (the caller merges inputs that are the same tensor)."""
+        T, S = len(self._task_layers), len(self._shared_layers)
+        per = len(self._task_layers[0]) if T else 0
+        shared = list(range(T * per, T * per + S))
+        gate_input = [1 + i for i in range(T)]
+        gate_experts = [list(range(i * per, (i + 1) * per)) + shared for i in range(T)]
+        if self._shared_gate is not None:
+            gate_input.append(0)
+            gate_experts.append(list(range(T * per + S)))
+        return gate_input, gate_experts
+
+    def forward(self, extraction_network_fea: List[torch.Tensor], shared_expert_fea: torch.Tensor):
+        shared_expert = [layer(shared_expert_fea) for layer in self._shared_layers]
+        task_experts = [[layer(extraction_network_fea[i]) for layer in layers]
+                        for i, layers in enumerate(self._task_layers)]
+        experts = [e for te in task_experts for e in te] + shared_expert
+        gate_input, gate_experts = self.gate_layout()
+        candidates = [shared_expert_fea] + list(extraction_network_fea)
+        inputs = []                       # the distinct tensors the gates read, by identity (one in the first layer)
+        for i in gate_input:
+            if not any(candidates[i] is u for u in inputs):
+                inputs.append(candidates[i])
+        gate_input = [next(j for j, u in enumerate(inputs) if u is candidates[i]) for i in gate_input]
+        gates = list(self._task_gates) + ([self._shared_gate] if self._shared_gate is not None else [])
+        weights = [g.weight for g in gates]
+        if Fn.ple_gate_usable(inputs, gate_input, weights, experts, gate_experts):
+            outs = Fn.ple_gates(inputs, gate_input, weights, [g.bias for g in gates], experts, gate_experts)
+        else:
+            outs = [Fn.torch_ple_gate(inputs[gate_input[g]], [experts[x] for x in gate_experts[g]], gates[g])
+                    for g in range(len(gates))]
+        T = len(self._task_layers)
+        return outs[:T], (outs[T] if self._shared_gate is not None else None)
+
+
+class PLE(MultiTaskRank):
+    """tzrec/models/ple.py:26-112: the first feature group through the stacked extraction layers, then one task tower
+    per task on its branch of the last layer."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self._task_nums = len(self._task_tower_cfgs)
+        self._layer_nums = len(self._model_config.extraction_networks)
+        self.init_input()
+        self.group_name = self.embedding_group.group_names()[0]
+        feature_in = self.embedding_group.group_total_dim(self.group_name)
+        self._extraction_nets = nn.ModuleList()
+        in_extraction_networks, in_shared_expert = [feature_in] * self._task_nums, feature_in
+        for i, cfg in enumerate(self._model_config.extraction_networks):
+            extraction = ExtractionNet(in_extraction_networks, in_shared_expert, final_flag=i == self._layer_nums - 1,
+                                       **config_to_kwargs(cfg))
+            self._extraction_nets.append(extraction)
+            output_dims = extraction.output_dim()
+            in_extraction_networks, in_shared_expert = output_dims[:-1], output_dims[-1]
+        self._task_tower = nn.ModuleList()
+        for i, cfg in enumerate(self._task_tower_cfgs):
+            mlp = config_to_kwargs(cfg.mlp) if cfg.HasField("mlp") else None
+            self._task_tower.append(TaskTower(in_extraction_networks[i], cfg.num_class, mlp=mlp))
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        net = self.build_input(batch)[self.group_name]
+        extraction_network_fea, shared_expert_fea = [net] * self._task_nums, net
+        for extraction_net in self._extraction_nets:
+            extraction_network_fea, shared_expert_fea = extraction_net(extraction_network_fea, shared_expert_fea)
+        return self._multi_task_output_to_prediction(
+            [tower(x) for tower, x in zip(self._task_tower, extraction_network_fea)])
 
 
 class MultiTower(MultiTowerDIN):
@@ -845,7 +957,7 @@ class MaskNet(RankModel):
 
 
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
-                 "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet}
+                 "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE}
 
 
 def create_model(model_config: Message, features: List[BaseFeature], labels: List[str], device=None) -> RankModel:
