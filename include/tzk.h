@@ -665,6 +665,41 @@ int tzk_ple_gate_fwd(const tzk_ple_gate_args* args_host, int32_t grid, float* y,
 int tzk_ple_gate_bwd(const tzk_ple_gate_args* args_host, const float* p, const float* dy, int32_t grid,
                      float* d_experts, float* partials, float* dparams, tzk_stream_t stream);
 
+/* ---- PEPNet: the gate-neural-unit product (tzrec/modules/personalized_net.py: GateNU.forward :50-59 scaling
+ * EPNet.forward :90-110 and the body of PPNet.forward's loop :187-195), up to 8 segments in one launch each way.
+ * Segment s is [B, N] (4 <= N <= 1024, N % 4 == 0, row pitches multiples of 4 floats, 16-B aligned pointers):
+ *   gate_fwd: y = act(x + bx) * gamma sigmoid(z + bz)       act: identity or ReLU; bx may be NULL (no bias)
+ *   gate_bwd: dy -> dx = dy * gamma s * act'(x + bx), dz = dy * act(x + bx) * gamma s (1 - s), s = sigmoid(z + bz)
+ *             recomputed from x and z; dparams = dbx_0 | dbz_0 | dbx_1 | dbz_1 | ... (2 N_s floats per segment) as
+ *             per-CTA partials (grid rows of that size) reduced in CTA order, no float atomics.
+ * x, z, y, dy, dx, dz use the pitches ldx (x, dx), ldz (z, dz) and ldy (y, dy).  fp32.  The description travels by
+ * value as a kernel parameter (no host-to-device copy: graph-capturable). */
+#define TZK_PEPNET_MAX_SEGS 8
+#define TZK_PEPNET_IDENTITY 0
+#define TZK_PEPNET_RELU 1
+typedef struct tzk_pepnet_seg {
+  const float* x;
+  const float* bx;
+  const float* z;
+  const float* bz;
+  float* y;        /* gate_fwd only */
+  const float* dy; /* gate_bwd only */
+  float* dx;       /* gate_bwd only */
+  float* dz;       /* gate_bwd only */
+  int64_t ldx, ldz, ldy;
+  int32_t N, act;
+  float gamma;
+  int32_t pad_;
+} tzk_pepnet_seg;
+typedef struct tzk_pepnet_gate_args {
+  int64_t B;
+  int32_t n_segs, pad_;
+  tzk_pepnet_seg seg[TZK_PEPNET_MAX_SEGS];
+} tzk_pepnet_gate_args;
+int tzk_pepnet_gate_fwd(const tzk_pepnet_gate_args* args_host, int32_t grid, tzk_stream_t stream);
+int tzk_pepnet_gate_bwd(const tzk_pepnet_gate_args* args_host, int32_t grid, float* partials, float* dparams,
+                        tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

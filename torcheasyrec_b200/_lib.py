@@ -37,6 +37,23 @@ class TzkPleGateArgs(ctypes.Structure):
                 ("d_inputs", c_void_p * PLE_MAX_GATES)]
 
 
+PEPNET_MAX_SEGS, PEPNET_IDENTITY, PEPNET_RELU = 8, 0, 1
+
+
+class TzkPepnetSeg(ctypes.Structure):
+    """struct tzk_pepnet_seg (include/tzk.h): one [B, N] segment of the PEPNet gate product."""
+
+    _fields_ = [("x", c_void_p), ("bx", c_void_p), ("z", c_void_p), ("bz", c_void_p), ("y", c_void_p),
+                ("dy", c_void_p), ("dx", c_void_p), ("dz", c_void_p), ("ldx", c_int64), ("ldz", c_int64),
+                ("ldy", c_int64), ("N", c_int32), ("act", c_int32), ("gamma", c_float), ("pad_", c_int32)]
+
+
+class TzkPepnetGateArgs(ctypes.Structure):
+    """struct tzk_pepnet_gate_args (include/tzk.h): up to 8 segments sharing the batch size."""
+
+    _fields_ = [("B", c_int64), ("n_segs", c_int32), ("pad_", c_int32), ("seg", TzkPepnetSeg * PEPNET_MAX_SEGS)]
+
+
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
 SIGNATURES = {
     "tzk_abi_version": (c_int32, []),
@@ -195,6 +212,9 @@ SIGNATURES = {
     "tzk_ple_gate_smem_bytes": (c_int64, [P, c_int32]),
     "tzk_ple_gate_fwd": (c_int32, [P, c_int32, P, P, P]),
     "tzk_ple_gate_bwd": (c_int32, [P, P, P, c_int32, P, P, P, P]),
+    # PEPNet: the gate-neural-unit product of up to 8 segments (the segments described by TzkPepnetGateArgs)
+    "tzk_pepnet_gate_fwd": (c_int32, [P, c_int32, P]),
+    "tzk_pepnet_gate_bwd": (c_int32, [P, c_int32, P, P, P]),
 }
 
 _lib = None

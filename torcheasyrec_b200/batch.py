@@ -77,12 +77,14 @@ def _draw_ids(rng: np.random.Generator, rows: int, n: int, dist: str) -> np.ndar
 
 
 def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Sequence[str], seed: int = 0,
-                    id_dist: str = "uniform", seq_len_mix: bool = True) -> Batch:
+                    id_dist: str = "uniform", seq_len_mix: bool = True,
+                    label_cardinality: Optional[Dict[str, int]] = None) -> Batch:
     """Host (CPU) batch with the A0 layout for any id/raw/sequence feature list.
 
     Non-sequence id features get exactly one id per sample (Criteo / Taobao, L=1); grouped sequence features
     draw a length per sample from the mixture {0, 1, U[2,max], max} the reference's mock data uses
-    (tzrec/tests/utils.py:157-182)."""
+    (tzrec/tests/utils.py:157-182).  Labels are {0, 1} (1 with probability 0.25), except a label named in
+    `label_cardinality`, which is drawn uniformly over [0, cardinality) (e.g. PEPNet's domain label)."""
     rng = np.random.default_rng(seed)
     B = batch_size
     by_group: Dict[str, List[BaseFeature]] = {}
@@ -129,5 +131,8 @@ def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Se
         if dense_keys:
             batch.dense_features[dg] = KeyedTensor(dense_keys, dense_dims, torch.from_numpy(np.concatenate(dense_vals, axis=1)))
     for name in labels:
-        batch.labels[name] = torch.from_numpy((rng.random(B) < 0.25).astype(np.float32))
+        if label_cardinality and name in label_cardinality:
+            batch.labels[name] = torch.from_numpy(rng.integers(0, label_cardinality[name], size=B).astype(np.float32))
+        else:
+            batch.labels[name] = torch.from_numpy((rng.random(B) < 0.25).astype(np.float32))
     return batch

@@ -130,7 +130,8 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "train_metrics": _f("TrainMetricConfig", rep=True), "kernel": _f(E, "PYTORCH"),
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
-                  "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE"}.get(k, "Generic"))
+                  "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE",
+                  "pepnet": "PEPNet"}.get(k, "Generic"))
            for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
@@ -157,9 +158,14 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     "PLE": {"extraction_networks": _f("ExtractionNetwork", rep=True), "task_towers": _f("TaskTower", rep=True)},
     "ExtractionNetwork": {"network_name": _f(S), "expert_num_per_task": _f(I), "share_num": _f(I, 0),
                           "task_expert_net": _f("MLP"), "share_expert_net": _f("MLP")},
+    "PEPNet": {"epnet_hidden_unit": _f(I), "epnet_gamma": _f(F, 2.0), "ppnet_hidden_units": _f(I, rep=True),
+               "ppnet_activation": _f(S, "nn.ReLU"), "ppnet_dropout_ratio": _f(F, rep=True), "ppnet_gamma": _f(F, 2.0),
+               "domain_input_name": _f(S), "task_domain_num": _f(I, 1), "task_towers": _f("TaskTower", rep=True)},
     "TaskTower": {"tower_name": _f(S), "label_name": _f(S), "metrics": _f("MetricConfig", rep=True),
                   "train_metrics": _f("TrainMetricConfig", rep=True), "losses": _f("LossConfig", rep=True),
-                  "num_class": _f(I, 1), "mlp": _f("MLP"), "weight": _f(F, 1.0), "sample_weight_name": _f(S)},
+                  "num_class": _f(I, 1), "mlp": _f("MLP"), "weight": _f(F, 1.0), "sample_weight_name": _f(S),
+                  "task_space_indicator_label": _f(S), "in_task_space_weight": _f(F, 1.0),
+                  "out_task_space_weight": _f(F, 1.0)},
     "LossConfig": {"binary_cross_entropy": _f("Generic"), "softmax_cross_entropy": _f("Generic"),
                    "l2_loss": _f("Generic"), "jrc_loss": _f("Generic"), "binary_focal_loss": _f("Generic")},
     "MetricConfig": {"auc": _f("AUC"), "multiclass_auc": _f("Generic"), "recall_at_k": _f("Generic"),

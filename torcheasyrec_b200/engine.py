@@ -47,7 +47,7 @@ class Pipeline:
                  static_capacity: Optional[float] = None, exchange: str = "nccl") -> None:
         """`config`: path of a pipeline .config/.json, or the name of a built-in example
         (example_configs.BUILTINS: dlrm_criteo, deepfm_criteo, mmoe_taobao, multi_tower_din_taobao, masknet_criteo,
-        ple_taobao, wukong_criteo)."""
+        ple_taobao, pepnet_taobao, wukong_criteo)."""
         from . import example_configs
         from .config import parse_text
 
@@ -127,7 +127,11 @@ class Pipeline:
         return out
 
     def synthetic_batch(self, batch_size: int, seed: int = 0, id_dist: str = "uniform") -> Batch:
-        b = synthetic_batch(self.features, batch_size, self.labels, seed=seed, id_dist=id_dist)
+        mc = self.cfg.model_config
+        pep = mc.pepnet if mc.WhichOneof("model") == "pepnet" else None
+        card = ({pep.domain_input_name: pep.task_domain_num}
+                if pep is not None and pep.HasField("domain_input_name") else None)
+        b = synthetic_batch(self.features, batch_size, self.labels, seed=seed, id_dist=id_dist, label_cardinality=card)
         for kjt in b.sparse_features.values():
             kjt.length_per_key()  # host-side, before the copy: keeps the device path free of syncs
         return b

@@ -1,5 +1,6 @@
 """Generators for the pipeline configs BASELINE.json names (text format, same message tree as the reference's
-examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo,ple_taobao}.config).
+examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo,ple_taobao,
+pepnet_taobao}.config).
 
 The package does not depend on the reference's files, so the configs are re-derived here from their defining facts
 (SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table list and price boundaries, and the model
@@ -202,6 +203,26 @@ def ple_taobao() -> str:
             + _task_tower("ctr", "clk", None) + _task_tower("cvr", "buy", 1000) + "    }\n}\n")
 
 
+def pepnet_taobao() -> str:
+    """examples/pepnet_taobao.config: mmoe_taobao's features and towers ctr/cvr, `occupation` also a label; groups all
+    (mmoe_taobao's 16), domain (occupation), uia (13 user and item features); pepnet{3 domains by occupation, PPNet
+    512-256 with dropout 0.1}; cvr weighs its loss by the clk task space (in 1, out 0)."""
+    uia = ["user_id", "cms_segid", "cms_group_id", "final_gender_code", "age_level", "pvalue_level", "shopping_level",
+           "new_user_class_level", "adgroup_id", "cate_id", "campaign_id", "brand", "price"]
+    cvr = _task_tower("cvr", "buy", 1000)
+    cvr = cvr[:cvr.rindex("        }\n")] + ('            task_space_indicator_label: "clk"\n'
+                                           "            in_task_space_weight: 1\n"
+                                           "            out_task_space_weight: 0\n        }\n")
+    return (_header("taobao_multitask_sample_v1_train", "taobao_multitask_sample_v1/ds=20170513", "pepnet_taobao",
+                    "FG_DAG", ["clk", "buy", "occupation"], None, quota=False)
+            + _taobao_features()
+            + "model_config {\n" + _group("all", TAOBAO_MMOE_ORDER, "DEEP") + _group("domain", ["occupation"], "DEEP")
+            + _group("uia", uia, "DEEP")
+            + "    pepnet {\n        domain_input_name: 'occupation'\n        task_domain_num: 3\n"
+            "        ppnet_hidden_units: [512, 256]\n        ppnet_dropout_ratio: [0.1, 0.1]\n"
+            + _task_tower("ctr", "clk", None) + cvr + "    }\n}\n")
+
+
 def multi_tower_din_taobao() -> str:
     """examples/multi_tower_din_taobao.config: group deep (16) + SEQUENCE group seq (3 queries + click_50_seq)."""
     seq_feats = "".join(
@@ -225,7 +246,7 @@ def multi_tower_din_taobao() -> str:
 
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
               "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo,
-              "ple_taobao": ple_taobao}
+              "ple_taobao": ple_taobao, "pepnet_taobao": pepnet_taobao}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
 EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}

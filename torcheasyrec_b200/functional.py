@@ -672,3 +672,190 @@ def torch_ple_gate(selector: torch.Tensor, experts: Sequence[torch.Tensor], gate
     vec = torch.stack(list(experts), dim=1)
     g = torch.softmax(gate(selector), dim=1).unsqueeze(1)
     return torch.matmul(g, vec).squeeze(1)
+
+
+# ------------------------------------------------------------------------------------------------ PEPNet gates
+PEPNET_MAX_TASKS = 8           # csrc/tzk_pepnet.cuh: one segment per task in one launch
+PEPNET_MAX_WIDTH = 1024        # N of a segment
+
+
+def pepnet_usable(main: torch.Tensor, other: torch.Tensor, gate_hidden: Sequence[int], widths: Sequence[int],
+                  n_tasks: int = 1, activation: Optional[str] = None) -> bool:
+    """True when the fused PEPNet path covers an EPNet (activation None: identity product, `other` the domain input) or
+    a PPNet (`activation` its ppnet_activation, `other` the uia input): fp32 2-D inputs, autocast off, the gate input
+    width other + main, every gate hidden width and every product width a multiple of 4, product widths <= 1024, 1 <=
+    n_tasks <= 8, activation nn.ReLU (PPNet), on CUDA with the dense GEMM library loaded and TF32 off (on the CPU only
+    a test backend that implements the PEPNet kernels)."""
+    if autocast_dtype(main) is not None or activation not in (None, "nn.ReLU"):
+        return False
+    if any(t.dtype != torch.float32 or t.dim() != 2 or t.device != main.device for t in (main, other)):
+        return False
+    if other.shape[0] != main.shape[0] or (other.shape[1] + main.shape[1]) % 4 != 0:
+        return False
+    if not (1 <= n_tasks <= PEPNET_MAX_TASKS and all(h >= 4 and h % 4 == 0 for h in gate_hidden)
+            and all(4 <= n <= PEPNET_MAX_WIDTH and n % 4 == 0 for n in widths)):
+        return False
+    if main.is_cuda:
+        from . import dense_gemm
+
+        return _backend is None and dense_gemm.available() and not torch.backends.cuda.matmul.allow_tf32
+    return _backend is not None and hasattr(_backend, "pepnet_gate_fwd")
+
+
+def _relu_bwd_colsum(dh: torch.Tensor, h: torch.Tensor):
+    """(dh * (h > 0), its column sums) of a [B, N] layer, N % 4 == 0: act_bwd_colsum on column blocks of 256, 128, ...,
+    4 (the widths it covers), into one [B, N] buffer."""
+    if not dh.is_cuda:
+        d = dh * (h > 0)
+        return d, d.sum(0)
+    K = backend()
+    out = torch.empty_like(dh)
+    sums, c, N = [], 0, dh.shape[1]
+    while c < N:
+        w = 256
+        while w > N - c:
+            w //= 2
+        _, s = K.act_bwd_colsum(dh[:, c:c + w], h[:, c:c + w], True, out=out[:, c:c + w])
+        sums.append(s)
+        c += w
+    return out, torch.cat(sums)
+
+
+class _PepnetGateHidden(torch.autograd.Function):
+    """Every GateNU of an EPNet or PPNet up to its sigmoid (tzrec/modules/personalized_net.py GateNU.dense_layers
+    0..2), on the one gate input G = [other | main.detach()] (formed once, not per task):
+      h = ReLU(G W1cat^T + b1cat)        one GEMM over every gate, then bias_act
+      z_k = h_k W2_k^T                   one GEMM per gate, into column slot place[k] of output group place[k][0]
+    The second layers' biases and the sigmoid belong to the product (_PepnetProduct).  Backward: dh_k = dz_k W2_k, the
+    ReLU backward and db1 with act_bwd_colsum, dW1cat = dh^T G and d_other = dh W1cat[:, :U] as one GEMM each."""
+
+    @staticmethod
+    def forward(ctx, spec, other, main, *params):
+        from . import dense_gemm
+
+        K = backend()
+        groups, place = spec
+        G = len(place)
+        w1s, b1s, w2s = params[:G], params[G:2 * G], params[2 * G:]
+        g_in = torch.cat([other, main], dim=1)
+        w1cat, b1cat = torch.cat(w1s).contiguous(), torch.cat(b1s).contiguous()
+        h = dense_gemm.gemm(g_in, False, w1cat, True)
+        if h.is_cuda:
+            K.bias_act(h, b1cat, True)
+        else:
+            h.add_(b1cat).relu_()
+        B = g_in.shape[0]
+        zs = [g_in.new_empty((B, w)) for w in groups]
+        off = 0
+        for k in range(G):
+            (grp, col), a, n = place[k], w1s[k].shape[0], w2s[k].shape[0]
+            dense_gemm.gemm(h[:, off:off + a], False, w2s[k], True, out=zs[grp][:, col:col + n])
+            off += a
+        ctx.save_for_backward(g_in, h, w1cat, *w2s)
+        ctx.spec, ctx.U = spec, other.shape[1]
+        return tuple(zs)
+
+    @staticmethod
+    def backward(ctx, *dzs):
+        from . import dense_gemm
+
+        g_in, h, w1cat, *w2s = ctx.saved_tensors
+        groups, place = ctx.spec
+        dh = torch.empty_like(h)
+        dw2, hidden, off = [], [], 0
+        for k, w2 in enumerate(w2s):
+            (grp, col), a, n = place[k], w2.shape[1], w2.shape[0]
+            dz = _rows_contig(dzs[grp])[:, col:col + n]
+            dense_gemm.gemm(dz, False, w2, False, out=dh[:, off:off + a])
+            dw2.append(dense_gemm.gemm(dz, True, h[:, off:off + a], False))
+            hidden.append(a)
+            off += a
+        dh, db1 = _relu_bwd_colsum(dh, h)
+        dw1 = dense_gemm.gemm(dh, True, g_in, False)
+        d_other = dense_gemm.gemm(dh, False, w1cat[:, :ctx.U], False) if ctx.needs_input_grad[1] else None
+        dw1s, db1s, off = [], [], 0
+        for a in hidden:
+            dw1s.append(dw1[off:off + a])
+            db1s.append(db1[off:off + a])
+            off += a
+        return (None, d_other, None, *dw1s, *db1s, *dw2)
+
+
+class _PepnetProduct(torch.autograd.Function):
+    """y_i = act(x_i + bx_i) * gamma sigmoid(z_i + bz_i) for T segments of width N side by side in y [B, T N]
+    (csrc/tzk_pepnet.cuh, one launch each way).  x_i is inputs[0] itself (EPNet: no weights, identity), the i-th slot
+    of one GEMM of the shared input against the stacked weights (PPNet depth 0), or one GEMM per task input (deeper
+    depths).  z [B, T N] is _PepnetGateHidden's output group of this depth."""
+
+    @staticmethod
+    def forward(ctx, spec, z, *tensors):
+        from . import dense_gemm
+
+        n_in, T, relu, gamma = spec
+        inputs, rest = tensors[:n_in], tensors[n_in:]
+        has_w = len(rest) == 3 * T
+        ws, bs, bzs = (rest[:T], rest[T:2 * T], rest[2 * T:]) if has_w else ((), (None,) * T, rest)
+        B, N = z.shape[0], z.shape[1] // T
+        z = _rows_contig(z)
+        if not has_w:
+            x = _rows_contig(inputs[0])
+        elif n_in == 1:
+            x = dense_gemm.gemm(inputs[0], False, torch.cat(ws), True)
+        else:
+            x = z.new_empty((B, T * N))
+            for i in range(T):
+                dense_gemm.gemm(inputs[i], False, ws[i], True, out=x[:, i * N:(i + 1) * N])
+        y = z.new_empty((B, T * N))
+        backend().pepnet_gate_fwd([(x[:, i * N:(i + 1) * N], bs[i], z[:, i * N:(i + 1) * N], bzs[i],
+                                    y[:, i * N:(i + 1) * N], relu, gamma) for i in range(T)])
+        ctx.save_for_backward(x, z, *inputs, *ws, *[b for b in bs if b is not None], *bzs)
+        ctx.spec, ctx.has_w = spec, has_w
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from . import dense_gemm
+
+        n_in, T, relu, gamma = ctx.spec
+        x, z, *rest = ctx.saved_tensors
+        inputs = rest[:n_in]
+        ws, bs, bzs = (rest[n_in:n_in + T], rest[n_in + T:n_in + 2 * T], rest[n_in + 2 * T:]) if ctx.has_w \
+            else ((), (None,) * T, rest[n_in:])
+        N = z.shape[1] // T
+        dy = _rows_contig(dy)
+        dx, dz = torch.empty_like(x), torch.empty_like(z)
+        cols = [slice(i * N, (i + 1) * N) for i in range(T)]
+        sums = backend().pepnet_gate_bwd([(x[:, c], bs[i], z[:, c], bzs[i], None, relu, gamma) for i, c in enumerate(cols)],
+                                         [dy[:, c] for c in cols], [dx[:, c] for c in cols], [dz[:, c] for c in cols])
+        dbzs = [s[1] for s in sums]
+        if not ctx.has_w:
+            return (None, dz, dx, *dbzs)
+        if n_in == 1:
+            d_in = [dense_gemm.gemm(dx, False, torch.cat(ws), False)]
+            dw = dense_gemm.gemm(dx, True, inputs[0], False)
+            dws = [dw[c] for c in cols]
+        else:
+            d_in = [dense_gemm.gemm(dx[:, c], False, ws[i], False) for i, c in enumerate(cols)]
+            dws = [dense_gemm.gemm(dx[:, c], True, inputs[i], False) for i, c in enumerate(cols)]
+        return (None, dz, *d_in, *dws, *[s[0] for s in sums], *dbzs)
+
+
+def pepnet_gate_hidden(other: torch.Tensor, main: torch.Tensor, gates, groups: Sequence[int], place) -> List[torch.Tensor]:
+    """Fused first layers of the GateNUs `gates` (modules with dense_layers.0 / .2) on [other | main.detach()]:
+    -> one [B, groups[g]] tensor per output group, gate k's pre-bias second layer at place[k] = (group, column).  The
+    caller checks pepnet_usable first."""
+    l1 = [g.dense_layers[0] for g in gates]
+    params = [m.weight for m in l1] + [m.bias for m in l1] + [g.dense_layers[2].weight for g in gates]
+    spec = (tuple(groups), tuple(tuple(p) for p in place))
+    return list(_PepnetGateHidden.apply(spec, other, main.detach(), *params))
+
+
+def pepnet_product(z: torch.Tensor, gates, gamma: float, inputs: Sequence[torch.Tensor], linears=(),
+                   relu: bool = False) -> torch.Tensor:
+    """Fused GateNU product of T = len(gates) segments side by side: [B, T N] with slot i = act(x_i + b_i) *
+    gamma sigmoid(z_i + gates[i].dense_layers.2.bias), x_i = inputs[0] (no linears), inputs[0] through linears[i]
+    (one shared input) or inputs[i] through linears[i].  The caller checks pepnet_usable first."""
+    T = len(gates)
+    params = ([m.weight for m in linears] + [m.bias for m in linears]) if linears else []
+    params += [g.dense_layers[2].bias for g in gates]
+    return _PepnetProduct.apply((len(inputs), T, bool(relu), float(gamma)), z, *inputs, *params)

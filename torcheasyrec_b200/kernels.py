@@ -946,18 +946,23 @@ class CudaKernels:
         self.launches += 1
         return y
 
-    def act_bwd_colsum(self, dy: torch.Tensor, y: Optional[torch.Tensor], relu: bool, want_dz: bool = True):
+    def act_bwd_colsum(self, dy: torch.Tensor, y: Optional[torch.Tensor], relu: bool, want_dz: bool = True,
+                       out: Optional[torch.Tensor] = None):
+        """`out`: where dz goes (a [M, N] view with contiguous rows, which may be dy itself); None allocates it."""
         dy, ld_dy = _rows2d(dy, "dy")
         M, N = dy.shape
         ld_y = 0
         if y is not None:
             y, ld_y = _rows2d(y, "y")
-        dz = torch.empty((M, N), dtype=torch.float32, device=dy.device) if want_dz else None
+        if out is not None:
+            dz, ld_dz = _rows2d(out, "out")
+        else:
+            dz, ld_dz = (torch.empty((M, N), dtype=torch.float32, device=dy.device) if want_dz else None), N
         colsum = torch.empty(N, dtype=torch.float32, device=dy.device)
         nb = self._lib.tzk_act_bwd_colsum_workspace_bytes(M, N)
         ws = self._workspace("colsum", nb, dy.device)
-        check(self._lib.tzk_act_bwd_colsum(_ptr(dy), ld_dy, _ptr(y), ld_y, M, N, int(relu), _ptr(dz), N, _ptr(colsum),
-                                           _ptr(ws), ws.numel(), _stream()), "tzk_act_bwd_colsum")
+        check(self._lib.tzk_act_bwd_colsum(_ptr(dy), ld_dy, _ptr(y), ld_y, M, N, int(relu), _ptr(dz), ld_dz,
+                                           _ptr(colsum), _ptr(ws), ws.numel(), _stream()), "tzk_act_bwd_colsum")
         self.launches += 2
         return dz, colsum
     # ------------------------------------------------------------------ narrow layers + BCE head
@@ -1294,6 +1299,71 @@ class CudaKernels:
             db.append(dparams[o:o + e])
             o += e
         return d_inputs, d_experts, dW, db
+
+    # ------------------------------------------------------------------ PEPNet gate product (csrc/tzk_pepnet.cuh)
+    # Resident CTAs per SM: ptxas register counts at 256 threads (gate_fwd 35 -> 6, gate_bwd 72 -> 3).  The grid fixes
+    # the order of the batch sums and depends only on the batch size, the segments' widths and the device.
+    def _pepnet_args(self, segs, dys=None, dxs=None, dzs=None):
+        """segs: [(x, bx, z, bz, y, relu, gamma)], x / z / y [B, N] views with contiguous rows, bx None or [N]."""
+        from ._lib import PEPNET_MAX_SEGS, PEPNET_IDENTITY, PEPNET_RELU, TzkPepnetGateArgs
+
+        if not 1 <= len(segs) <= PEPNET_MAX_SEGS:
+            raise TzkError(f"pepnet gates: 1..{PEPNET_MAX_SEGS} segments, got {len(segs)}")
+        a = TzkPepnetGateArgs()
+        a.B, a.n_segs = segs[0][0].shape[0], len(segs)
+        for s, (x, bx, z, bz, y, relu, gamma) in enumerate(segs):
+            x, ldx = _rows2d(x, f"x[{s}]")
+            z, ldz = _rows2d(z, f"z[{s}]")
+            g = a.seg[s]
+            g.x, g.z, g.bz = x.data_ptr(), z.data_ptr(), _need(bz, torch.float32, f"bz[{s}]").data_ptr()
+            g.bx = None if bx is None else _need(bx, torch.float32, f"bx[{s}]").data_ptr()
+            g.ldx, g.ldz, g.N = ldx, ldz, x.shape[1]
+            g.act, g.gamma = (PEPNET_RELU if relu else PEPNET_IDENTITY), float(gamma)
+            if y is not None:
+                y, g.ldy = _rows2d(y, f"y[{s}]")
+                g.y = y.data_ptr()
+            if dys is not None:
+                dy, g.ldy = _rows2d(dys[s], f"dy[{s}]")
+                _, ld_dx = _rows2d(dxs[s], f"dx[{s}]")
+                _, ld_dz = _rows2d(dzs[s], f"dz[{s}]")
+                if (ld_dx, ld_dz) != (ldx, ldz):
+                    raise TzkError("pepnet_gate_bwd: dx / dz must have the row pitches of x / z")
+                g.dy, g.dx, g.dz = dy.data_ptr(), dxs[s].data_ptr(), dzs[s].data_ptr()
+            if tuple(z.shape) != tuple(x.shape) or x.shape[0] != a.B:
+                raise TzkError("pepnet gates: x and z of a segment must have one [B, N] shape")
+        return a
+
+    def _pepnet_grid(self, a, per_sm: int) -> int:
+        sms = getattr(self, "_sms", None)
+        if sms is None:
+            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
+        rows = min(256 // (a.seg[s].N // 4) for s in range(a.n_segs))
+        return max(1, min(-(-int(a.B) // rows), -(-per_sm * sms // a.n_segs)))
+
+    def pepnet_gate_fwd(self, segs):
+        """y = act(x + bx) * gamma sigmoid(z + bz) into every segment's y (written in place)."""
+        a = self._pepnet_args(segs)
+        check(self._lib.tzk_pepnet_gate_fwd(ctypes.byref(a), self._pepnet_grid(a, 6), _stream()),
+              "tzk_pepnet_gate_fwd")
+        self.launches += int(a.B > 0)
+
+    def pepnet_gate_bwd(self, segs, dys, dxs, dzs):
+        """dys -> dxs, dzs (written in place), returns [(dbx, dbz)] per segment."""
+        a = self._pepnet_args(segs, dys, dxs, dzs)
+        P = sum(2 * s[0].shape[1] for s in segs)
+        dev = segs[0][0].device
+        grid = self._pepnet_grid(a, 3)
+        partials = self._workspace("pepnet_gate_bwd", grid * P * 4, dev)
+        dparams = torch.empty(P, dtype=torch.float32, device=dev)
+        check(self._lib.tzk_pepnet_gate_bwd(ctypes.byref(a), grid, _ptr(partials), _ptr(dparams), _stream()),
+              "tzk_pepnet_gate_bwd")
+        self.launches += 1 + int(a.B > 0)
+        out, o = [], 0
+        for s in segs:
+            N = s[0].shape[1]
+            out.append((dparams[o:o + N], dparams[o + N:o + 2 * N]))
+            o += 2 * N
+        return out
 
 
 @dataclass

@@ -1,4 +1,4 @@
-"""Model shells that consume the hot path: DLRM, DeepFM, MMoE, PLE, MultiTowerDIN (+ their dense blocks).
+"""Model shells that consume the hot path: DLRM, DeepFM, MMoE, PLE, PEPNet, MultiTowerDIN (+ their dense blocks).
 
 These are the callers of §8a rows A7-A10 (SURVEY.md §2 row 4): tzrec/models/{rank_model,dlrm,deepfm,mmoe,
 multi_tower_din,multi_task_rank}.py and the dense blocks of tzrec/modules/{mlp,mmoe,sequence,task_tower}.py.
@@ -555,16 +555,17 @@ class MultiTowerDIN(RankModel):
 
 class MultiTaskRank(RankModel):
     """tzrec/models/multi_task_rank.py:25-196 for BCE towers: one prediction pair, loss, and metric head per task tower
-    (suffix `_<tower_name>`).  What the reference honours per tower and this repo does not (sample weights, task-space
-    indicator labels, non-BCE losses) is refused at construction instead of silently training with plain mean BCE."""
+    (suffix `_<tower_name>`).  A tower with `task_space_indicator_label` weighs its per-sample BCE as
+    multi_task_rank.py:97-142 does.  What the reference honours per tower and this repo does not (sample weights,
+    non-BCE losses) is refused at construction instead of silently training with plain mean BCE."""
 
     def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
         super().__init__(model_config, features, labels, sample_weights, **kwargs)
         self._task_tower_cfgs = list(self._model_config.task_towers)
         for cfg in self._task_tower_cfgs:
-            for fld in ("sample_weight_name", "task_space_indicator_label"):
-                if cfg._spec(fld) is not None and cfg.HasField(fld) and getattr(cfg, fld):
-                    raise NotImplementedError(f"task tower {cfg.tower_name}: {fld} is outside the hot-path scope")
+            fld = "sample_weight_name"
+            if cfg._spec(fld) is not None and cfg.HasField(fld) and getattr(cfg, fld):
+                raise NotImplementedError(f"task tower {cfg.tower_name}: {fld} is outside the hot-path scope")
             for lc in (cfg.losses if cfg._spec("losses") is not None else []):
                 if lc.WhichOneof("loss") not in (None, "binary_cross_entropy"):
                     raise NotImplementedError(f"task tower {cfg.tower_name}: loss {lc.WhichOneof('loss')} is outside "
@@ -587,9 +588,32 @@ class MultiTaskRank(RankModel):
         out = {}
         for cfg in self._task_tower_cfgs:
             label = batch.labels[cfg.label_name].to(torch.float32)
-            out[f"binary_cross_entropy_{cfg.tower_name}"] = cfg.weight * bce_with_logits(
-                predictions[f"logits_{cfg.tower_name}"], label)
+            logits = predictions[f"logits_{cfg.tower_name}"]
+            if _task_space_label(cfg):
+                out[f"binary_cross_entropy_{cfg.tower_name}"] = task_space_weighted_bce(
+                    logits, label, batch.labels[cfg.task_space_indicator_label], cfg.in_task_space_weight,
+                    cfg.out_task_space_weight, cfg.weight)
+            else:
+                out[f"binary_cross_entropy_{cfg.tower_name}"] = cfg.weight * bce_with_logits(logits, label)
         return out
+
+
+def _task_space_label(cfg) -> Optional[str]:
+    fld = "task_space_indicator_label"
+    return getattr(cfg, fld) if cfg._spec(fld) is not None and cfg.HasField(fld) and getattr(cfg, fld) else None
+
+
+def task_space_weighted_bce(logits: torch.Tensor, label: torch.Tensor, indicator: torch.Tensor, in_weight: float,
+                            out_weight: float, weight: float) -> torch.Tensor:
+    """multi_task_rank.py:105-125 + rank_model.py:233-261 for a tower with task_space_indicator_label and no sample
+    weight: mean(bce_none * w), w = div_no_nan(v, mean(v)) * weight, v = in [ind > 0] + out (1 - [ind > 0]).  Device
+    work only (capturable): an all-out-of-space batch with out_weight 0 gives w = 0, not NaN."""
+    logits = logits.float()
+    in_space = (indicator > 0).float()
+    w = torch.ones(1, device=logits.device) * (in_weight * in_space + out_weight * (1 - in_space))
+    w = torch.nan_to_num(torch.div(w, torch.mean(w)), nan=0.0, posinf=0.0, neginf=0.0)
+    w = w * weight
+    return torch.mean(F.binary_cross_entropy_with_logits(logits, label, reduction="none") * w)
 
 
 class MMoE(MultiTaskRank):
@@ -713,6 +737,210 @@ class PLE(MultiTaskRank):
             extraction_network_fea, shared_expert_fea = extraction_net(extraction_network_fea, shared_expert_fea)
         return self._multi_task_output_to_prediction(
             [tower(x) for tower, x in zip(self._task_tower, extraction_network_fea)])
+
+
+class GateNU(nn.Module):
+    """tzrec/modules/personalized_net.py:20-59: gamma * sigmoid(Linear(ReLU(Linear(x))))."""
+
+    def __init__(self, input_dim: int, hidden_dim: int, output_dim: int, gamma: float = 2.0) -> None:
+        super().__init__()
+        self._gamma = gamma
+        self._output_dim = output_dim
+        self.dense_layers = nn.Sequential(nn.Linear(input_dim, hidden_dim), nn.ReLU(), nn.Linear(hidden_dim, output_dim),
+                                          nn.Sigmoid())
+
+    def output_dim(self) -> int:
+        return self._output_dim
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return self._gamma * self.dense_layers(x)
+
+
+class EPNet(nn.Module):
+    """tzrec/modules/personalized_net.py:62-110: GateNU([domain | main.detach()]) * main.  When Fn.pepnet_usable holds,
+    the gate's first layer, its second layer and the sigmoid product run as Fn.pepnet_gate_hidden +
+    Fn.pepnet_product (csrc/tzk_pepnet.cuh); otherwise the reference's torch formulation."""
+
+    def __init__(self, main_dim: int, domain_dim: int, hidden_dim: int, gamma: float = 2.0) -> None:
+        super().__init__()
+        self._domain_dim, self._main_dim, self._hidden_dim = domain_dim, main_dim, hidden_dim
+        self.gate_nu = GateNU(input_dim=domain_dim + main_dim, hidden_dim=hidden_dim, output_dim=main_dim, gamma=gamma)
+
+    def output_dim(self) -> int:
+        return self.gate_nu.output_dim()
+
+    def forward(self, main_emb: torch.Tensor, domain_emb: torch.Tensor) -> torch.Tensor:
+        if Fn.pepnet_usable(main_emb, domain_emb, [self._hidden_dim], [self._main_dim]):
+            z = Fn.pepnet_gate_hidden(domain_emb, main_emb, [self.gate_nu], [self._main_dim], [(0, 0)])[0]
+            return Fn.pepnet_product(z, [self.gate_nu], self.gate_nu._gamma, [main_emb])
+        gate_input = torch.cat([domain_emb, main_emb.detach()], dim=-1)
+        return self.gate_nu(gate_input) * main_emb
+
+
+class PPNet(nn.Module):
+    """tzrec/modules/personalized_net.py:113-196: per task i and depth j (module index i * len_hidden + j),
+    y_ij = Dropout(act(Linear_ij(y_i,j-1)) * GateNU_ij([uia | main.detach()])), y_i,-1 = main.  When Fn.pepnet_usable
+    holds: every GateNU's first layer over all tasks and depths as one GEMM on the gate input formed once
+    (Fn.pepnet_gate_hidden), then per depth one fused product over all tasks (Fn.pepnet_product; depth 0's linears as
+    one GEMM of the shared input) and the reference's Dropout modules; otherwise the reference's torch formulation."""
+
+    def __init__(self, main_feature: int, uia_feature: int, num_task: int, hidden_units: List[int],
+                 activation: Optional[str] = "nn.ReLU", dropout_ratio=None, gamma: float = 2.0) -> None:
+        super().__init__()
+        self.main_feature, self.uia_feature, self.num_task = main_feature, uia_feature, num_task
+        self.hidden_units = list(hidden_units)
+        self.len_hidden = len(self.hidden_units)
+        self._activation, self._gamma = activation, gamma
+        self.linears = nn.ModuleList()
+        self.activations = nn.ModuleList()
+        self.dropout_ratios = nn.ModuleList()
+        self.gate_nus = nn.ModuleList()
+        n = len(self.hidden_units)
+        if dropout_ratio is None:
+            dropout_ratio = [0.0] * n
+        elif isinstance(dropout_ratio, list):
+            if len(dropout_ratio) == 0:
+                dropout_ratio = [0.0] * n
+            elif len(dropout_ratio) == 1:
+                dropout_ratio = dropout_ratio * n
+            else:
+                assert len(dropout_ratio) == n, ("length of dropout_ratio and hidden_units must be same, "
+                                                 f"but got {len(dropout_ratio)} vs {n}")
+        else:
+            dropout_ratio = [dropout_ratio] * n
+        for _ in range(self.num_task):
+            output = main_feature
+            for i, hidden_unit in enumerate(self.hidden_units):
+                self.linears.append(nn.Linear(output, hidden_unit))
+                self.activations.append(_create_activation(activation))
+                self.dropout_ratios.append(nn.Dropout(dropout_ratio[i]))
+                self.gate_nus.append(GateNU(input_dim=main_feature + uia_feature, hidden_dim=hidden_unit,
+                                            output_dim=hidden_unit, gamma=gamma))
+                output = hidden_unit
+
+    def output_dim(self) -> List[int]:
+        return [self.hidden_units[-1]] * self.num_task
+
+    def task_output_dim(self) -> int:
+        return self.hidden_units[-1]
+
+    def fused_usable(self, main_emb: torch.Tensor, uia_emb: torch.Tensor) -> bool:
+        return Fn.pepnet_usable(main_emb, uia_emb, self.hidden_units, self.hidden_units, self.num_task,
+                                self._activation)
+
+    def forward(self, main_emb: torch.Tensor, uia_emb: torch.Tensor) -> List[torch.Tensor]:
+        T, L = self.num_task, self.len_hidden
+        if self.fused_usable(main_emb, uia_emb):
+            gates = list(self.gate_nus)
+            place = [(j, i * self.hidden_units[j]) for i in range(T) for j in range(L)]
+            zs = Fn.pepnet_gate_hidden(uia_emb, main_emb, gates, [T * h for h in self.hidden_units], place)
+            outs = [main_emb]
+            for j, h in enumerate(self.hidden_units):
+                ks = [i * L + j for i in range(T)]
+                y = Fn.pepnet_product(zs[j], [gates[k] for k in ks], self._gamma, outs,
+                                      [self.linears[k] for k in ks], relu=True)
+                outs = [self.dropout_ratios[k](y[:, i * h:(i + 1) * h]) for i, k in enumerate(ks)]
+            return outs
+        task_outputs = []
+        for i in range(T):
+            gate_input = torch.cat([uia_emb, main_emb.detach()], dim=-1)
+            x = main_emb
+            for j in range(L):
+                k = i * L + j
+                x = self.linears[k](x)
+                x = self.activations[k](x)
+                x = x * self.gate_nus[k](gate_input)
+                x = self.dropout_ratios[k](x)
+            task_outputs.append(x)
+        return task_outputs
+
+
+def _float32(v: float) -> float:
+    """A `float` proto field as the reference's model reads it straight off the message: the stored float32's value."""
+    return struct.unpack("f", struct.pack("f", float(v)))[0]
+
+
+class PEPNet(MultiTaskRank):
+    """tzrec/models/pepnet.py:27-244: group `all` through EPNet (when a `domain` group exists) and PPNet (when a `uia`
+    group exists), then the task towers; with domain_input_name, task_domain_num towers per task (`_task_tower.{i D +
+    j}`) whose predictions are `logits_<tower>_<j>` / `probs_<tower>_<j>`, and the loss and the metrics see the tower
+    of each sample's domain label as `logits_<tower>` / `probs_<tower>`.
+
+    The selection is sum_j [d == j] out_j (exact; only the selected tower receives a gradient), so it never indexes
+    memory with a label value: a domain label outside [0, D) selects 0 where the reference's torch.gather raises."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self.init_input()
+        eg = self.embedding_group
+        self._main_group_name, self._domain_group_name, self._uia_group_name = "all", "domain", "uia"
+        if not eg.has_group(self._main_group_name):
+            raise Exception("all feature group not found.")
+        self._main_group_dim = eg.group_total_dim(self._main_group_name)
+        self._task_input_dim = self._main_group_dim
+        cfg = self._model_config
+        self.epnet = None
+        if eg.has_group(self._domain_group_name):
+            self.epnet = EPNet(self._main_group_dim, eg.group_total_dim(self._domain_group_name),
+                               hidden_dim=cfg.epnet_hidden_unit if cfg.HasField("epnet_hidden_unit")
+                               else self._main_group_dim, gamma=_float32(cfg.epnet_gamma))
+            self._task_input_dim = self.epnet.output_dim()
+        self.ppnet = None
+        if eg.has_group(self._uia_group_name):
+            self.ppnet = PPNet(self._main_group_dim, eg.group_total_dim(self._uia_group_name),
+                               num_task=len(self._task_tower_cfgs), hidden_units=list(cfg.ppnet_hidden_units),
+                               activation=cfg.ppnet_activation,
+                               dropout_ratio=[_float32(r) for r in cfg.ppnet_dropout_ratio],
+                               gamma=_float32(cfg.ppnet_gamma))
+            self._task_input_dim = self.ppnet.task_output_dim()
+        self._domain_input_name = cfg.domain_input_name if cfg.HasField("domain_input_name") else None
+        self._task_domain_num = cfg.task_domain_num
+        self._task_tower = nn.ModuleList()
+        for tc in self._task_tower_cfgs:
+            mlp = config_to_kwargs(tc.mlp) if tc.HasField("mlp") else None
+            for _ in range(self._task_domain_num if self._domain_input_name else 1):
+                self._task_tower.append(TaskTower(self._task_input_dim, tc.num_class, mlp=mlp))
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        grouped = self.build_input(batch)
+        x = grouped[self._main_group_name]
+        if self.epnet is not None:
+            x = self.epnet(x, grouped[self._domain_group_name])
+        task_inputs = self.ppnet(x, grouped[self._uia_group_name]) if self.ppnet is not None else [x]
+        preds = {}
+        D = self._task_domain_num
+        for i, tc in enumerate(self._task_tower_cfgs):
+            task_input = task_inputs[i] if self.ppnet is not None else task_inputs[0]
+            if self._domain_input_name:
+                for j in range(D):
+                    preds.update(self._output_to_prediction(self._task_tower[i * D + j](task_input),
+                                                            suffix=f"_{tc.tower_name}_{j}"))
+            else:
+                preds.update(self._output_to_prediction(self._task_tower[i](task_input), suffix=f"_{tc.tower_name}"))
+        return preds
+
+    def _select_domain_task_output(self, predictions: Dict[str, torch.Tensor], batch: Batch) -> Dict[str, torch.Tensor]:
+        """pepnet.py:176-203 by comparison: `<name>` = sum_j [d == j] `<name>_<j>` for every per-domain prediction."""
+        if not self._domain_input_name:
+            return predictions
+        d = batch.labels[self._domain_input_name]
+        out = {}
+        for tc in self._task_tower_cfgs:
+            for kind in ("logits", "probs"):
+                name = f"{kind}_{tc.tower_name}"
+                sel = None
+                for j in range(self._task_domain_num):
+                    v = predictions[f"{name}_{j}"]
+                    term = (d == j).to(v.dtype) * v
+                    sel = term if sel is None else sel + term
+                out[name] = sel
+        return out
+
+    def loss(self, predictions, batch):
+        return super().loss(self._select_domain_task_output(predictions, batch), batch)
+
+    def update_metric(self, predictions, batch, losses=None) -> None:
+        super().update_metric(self._select_domain_task_output(predictions, batch), batch, losses)
 
 
 class MultiTower(MultiTowerDIN):
@@ -957,7 +1185,8 @@ class MaskNet(RankModel):
 
 
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
-                 "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE}
+                 "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE,
+                 "pepnet": PEPNet}
 
 
 def create_model(model_config: Message, features: List[BaseFeature], labels: List[str], device=None) -> RankModel:
