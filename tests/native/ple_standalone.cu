@@ -5,7 +5,6 @@
 #include "cuda_cpu_shim.h"
 #include <math.h>
 #include <stdint.h>
-#define TZK_SET_MAX_SMEM(kernel, bytes) (void)(bytes)
 #include "../../torcheasyrec_b200/csrc/tzk_ple.cuh"
 
 extern "C" int64_t ple_smem_bytes(const tzk_ple_gate_args* c, int backward) {

@@ -23,9 +23,7 @@
 #include "cuda_cpu_shim.h"   // host execution for tests/test_tower_bwd2_cpu.py
 #else
 #include <cuda_runtime.h>
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#include "../../torcheasyrec_b200/csrc/tzk_launch.cuh"
 #endif
 #include <stdint.h>
 

@@ -237,6 +237,21 @@ def test_kernels_source_grid_stride(kern, E, H, nb):
     _run_ffn(kern, H, nb, 257, grid=5, seed=12)
 
 
+def test_kernel_source_empty_batch_zeroes_dparams(kern):
+    """B = 0: no backward kernel runs and the batch sums add no partial rows, so dparams comes back all zeros (the FFN's
+    for every mask block)."""
+    E, H, nb, grid = 33, 16, 3, 5
+    z = np.zeros(1, np.float32)                               # inputs: never read
+    P_ = (nb + 2) * E
+    part, dpar = np.full((grid, P_), np.nan, np.float32), np.full(P_, np.nan, np.float32)
+    assert kern.mn_mask_bwd(_p(z), M.pad4(E), _p(z), _p(z), _p(z), _p(z), _p(z), _p(z), 0, E, nb, grid, _p(z), _p(z),
+                            _p(part), _p(dpar)) == 0
+    np.testing.assert_array_equal(dpar, np.zeros(P_, np.float32))
+    part, dpar = np.full((nb, grid, 3 * H), np.nan, np.float32), np.full((nb, 3, H), np.nan, np.float32)
+    assert kern.mn_ffn_bwd(_p(z), _p(z), _p(z), _p(z), _p(z), _p(z), 0, H, nb, grid, _p(z), _p(part), _p(dpar)) == 0
+    np.testing.assert_array_equal(dpar, np.zeros((nb, 3, H), np.float32))
+
+
 def test_kernel_source_refuses_uncovered_shapes(kern):
     z = np.zeros(1 << 16, np.float32)
     for E, nb in [(1025, 1), (0, 1), (24, 0), (24, 9)]:

@@ -217,6 +217,20 @@ def test_kernel_source_widest_segment(kern):
     _run_segments(kern, 3, [(1024, True, True, 2.0, 0)], grid=2, seed=6)
 
 
+def test_kernel_source_empty_batch_zeroes_dparams(kern):
+    """B = 0: no backward kernel runs and the batch sums add no partial rows, so dparams comes back all zeros."""
+    widths, grid = [8, 12, 64], 5
+    a = TzkPepnetGateArgs()
+    a.B, a.n_segs = 0, len(widths)
+    for s, N in enumerate(widths):                            # no rows: the segments' buffers may be null
+        g = a.seg[s]
+        g.N, g.ldx, g.ldz, g.ldy, g.act, g.gamma = N, N, N, N, PEPNET_RELU, 2.0
+    P_ = 2 * sum(widths)
+    part, dpar = np.full((grid, P_), np.nan, np.float32), np.full(P_, np.nan, np.float32)
+    assert kern.pepnet_gate_bwd(ctypes.byref(a), grid, part.ctypes.data, dpar.ctypes.data) == 0
+    np.testing.assert_array_equal(dpar, np.zeros(P_, np.float32))
+
+
 def test_kernel_source_refuses_uncovered_segments(kern):
     x = np.zeros((2, 2048), np.float32)
 

@@ -216,6 +216,23 @@ def test_kernel_source_grid_stride(kern):
     _run_layer(kern, 257, 7, [19] * 3, gi, ge, ne, grid=5, seed=5)
 
 
+def test_kernel_source_empty_batch_zeroes_dparams(kern):
+    """B = 0: no backward kernel runs and the batch sums add no partial rows, so dparams comes back all zeros."""
+    in_dims, gi, ge, ne, H = _taobao_layer(1)
+    grid = 5
+    inputs = [np.zeros((0, k), np.float32) for k in in_dims]
+    weights = [np.zeros((len(ids), in_dims[gi[g]]), np.float32) for g, ids in enumerate(ge)]
+    biases = [np.zeros(len(ids), np.float32) for ids in ge]
+    experts = [np.zeros((0, H), np.float32) for _ in range(ne)]
+    a = _args(0, H, inputs, gi, weights, biases, experts, ge, [np.zeros((0, k), np.float32) for k in in_dims])
+    P_ = sum(w.size for w in weights) + sum(len(ids) for ids in ge)
+    z = np.zeros(1, np.float32)                               # p, dy, d_experts: never touched
+    part, dpar = np.full((grid, P_), np.nan, np.float32), np.full(P_, np.nan, np.float32)
+    assert kern.ple_gate_bwd(ctypes.byref(a), z.ctypes.data, z.ctypes.data, grid, z.ctypes.data, part.ctypes.data,
+                             dpar.ctypes.data) == 0
+    np.testing.assert_array_equal(dpar, np.zeros(P_, np.float32))
+
+
 def test_kernel_source_refuses_uncovered_layers(kern):
     z = np.zeros(4, np.float32)
 

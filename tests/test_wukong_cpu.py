@@ -201,6 +201,21 @@ def test_kernel_source_is_deterministic(kern):
     np.testing.assert_array_equal(outs[0][1], outs[1][1])
 
 
+def test_kernel_source_empty_batch_zeroes_dparams(kern):
+    """B = 0: no backward kernel runs and the batch sums add no partial rows, so dparams comes back all zeros."""
+    n, d, k, f, l, grid = 27, 16, 24, 16, 16, 5
+    z = np.zeros(1, np.float32)                               # inputs: never read
+    P_ = 3 * n * k + n * l + n * (f + l)
+    part, dpar = np.full((grid, P_), np.nan, np.float32), np.full(P_, np.nan, np.float32)
+    assert kern.wk_mix_bwd(_p(z), _p(z), _p(z), _p(z), _p(z), _p(z), _p(z), _p(z), 0, n, d, k, f, l, grid, _p(z),
+                           _p(part), _p(dpar)) == 0
+    np.testing.assert_array_equal(dpar, np.zeros(P_, np.float32))
+    opart, odpar = np.full((grid, 2 * d), np.nan, np.float32), np.full(2 * d, np.nan, np.float32)
+    assert kern.wk_out_bwd(_p(z), _p(z), _p(z), _p(z), _p(z), 0, d, f, l, grid, _p(z), _p(z), _p(opart),
+                           _p(odpar)) == 0
+    np.testing.assert_array_equal(odpar, np.zeros(2 * d, np.float32))
+
+
 def test_kernel_source_refuses_uncovered_shapes(kern):
     z = np.zeros(4096, np.float32)
     for n, d, k, f, l in [(65, 16, 8, 8, 8), (8, 12, 8, 4, 4), (8, 16, 33, 4, 4), (8, 16, 8, 40, 25), (8, 16, 8, 0, 8)]:

@@ -12,7 +12,8 @@ SOURCES = ["tzk_core.cu", "tzk_gather.cu", "tzk_bwd.cu", "tzk_dist.cu", "tzk_den
            "tzk_interact_bf16.cu", "tzk_metrics.cu", "tzk_wukong.cu",
            "tzk_masknet.cu", "tzk_ple.cu", "tzk_pepnet.cu"]
 HEADERS = ["tzk_common.cuh", "tzk_tower_bwd2.cuh", "tzk_interact_tc.cuh", "tzk_tower_tail.cuh", "tzk_interact_bf16.cuh",
-           "tzk_metrics.cuh", "tzk_wukong.cuh", "tzk_masknet.cuh", "tzk_ple.cuh", "tzk_pepnet.cuh",
+           "tzk_metrics.cuh", "tzk_wukong.cuh", "tzk_masknet.cuh", "tzk_ple.cuh", "tzk_pepnet.cuh", "tzk_launch.cuh",
+           "tzk_batch_sum.cuh",
 "tzk_sm90_ptx.h", "tzk_tma.h", "tzk_wgrad3x.cuh", "tzk_wgmma.cuh", os.path.join("..", "..", "include", "tzk.h")]
 LIB = os.path.join(HERE, "libtzk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -67,7 +68,7 @@ def build_gemm3x(force: bool = False) -> str:
     """libtzk_gemm3x.so: hand-written TMA + mma.sync 3xTF32 GEMMs of the wide tower layer (forward, dgrad, wgrad)."""
     src = os.path.join(HERE, "tzk_gemm3x.cu")
     lib = os.path.join(HERE, "libtzk_gemm3x.so")
-    deps = [src] + [os.path.join(HERE, h) for h in ("tzk_sm90_ptx.h", "tzk_tma.h", "tzk_wgrad3x.cuh")]
+    deps = [src] + [os.path.join(HERE, h) for h in ("tzk_launch.cuh", "tzk_sm90_ptx.h", "tzk_tma.h", "tzk_wgrad3x.cuh")]
     if force or _mtime(lib) < max(_mtime(d) for d in deps):
         subprocess.run([NVCC, *FLAGS, "-shared", src, "-o", lib + ".tmp"], check=True)
         os.replace(lib + ".tmp", lib)

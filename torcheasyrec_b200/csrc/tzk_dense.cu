@@ -8,9 +8,7 @@
 using namespace tzk;
 
 // ---- tensor-core variant of the DLRM interaction (mma.sync m16n8k8, 3xTF32) -------------------------------------------
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#include "tzk_launch.cuh"
 namespace tzk_itc {
 __device__ __forceinline__ uint32_t cvt_tf32(float x) {
   uint32_t r;

@@ -26,9 +26,8 @@
 #else
 #include <cuda.h>
 #include <cuda_runtime.h>
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(1024) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(1024) type name[]   // TMA swizzled tiles
+#include "tzk_launch.cuh"
 #endif
 
 namespace {

@@ -6,7 +6,7 @@
 
 using namespace tzk;
 
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
+#include "tzk_launch.cuh"
 namespace tzk_ib16 {
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);       // .x (low half) = lo

@@ -26,9 +26,8 @@ typedef void* tzk_stream_t;
 #else
 #include <cuda.h>
 #include "tzk_common.cuh"
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(1024) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(1024) type name[]   // TMA swizzled tiles
+#include "tzk_launch.cuh"
 #endif
 
 namespace {

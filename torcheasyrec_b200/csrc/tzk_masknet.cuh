@@ -12,15 +12,16 @@
 //
 // One CTA of 128 threads per row (grid-stride over rows); thread t owns columns t + 128 j, so every per-column batch
 // sum is accumulated by one thread in a fixed order (registers, or shared memory for the nb-dependent db2), written as
-// the CTA's row of a partials buffer, and reduce_kernel adds the rows in CTA order.  No float atomics: the result
-// depends only on the grid, which the host derives from B and the SM count, so a replayed graph gives the eager bits.
+// the CTA's row of a partials buffer, and tzk_batch_sum::reduce adds the rows in CTA order (tzk_batch_sum.cuh).
 //
-// fp32 FFMA throughout.  Plain CUDA (no PTX): the includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_masknet.cu;
-// g++ + tests/native/cuda_cpu_shim.h: tests/test_masknet_cpu.py runs this source on the host against a float64
-// restatement).
+// fp32 FFMA throughout.  Plain CUDA (no PTX): nvcc builds it in tzk_masknet.cu; g++ + tests/native/cuda_cpu_shim.h:
+// tests/test_masknet_cpu.py runs this source on the host against a float64 restatement.
 #pragma once
 #include <math.h>
 #include <stdint.h>
+
+#include "tzk_batch_sum.cuh"
+#include "tzk_launch.cuh"
 
 namespace tzk_masknet {
 constexpr int kThreads = 128;
@@ -35,28 +36,6 @@ inline int pad4(int n) { return (n + 3) / 4 * 4; }
 // shapes the kernels cover (the Python side's masknet_usable states the same)
 inline bool usable(int E, int H, int nb) {
   return E >= 1 && pad4(E) <= kMaxWidth && H >= 4 && H <= kMaxWidth && H % 4 == 0 && nb >= 1 && nb <= kMaxBlocks;
-}
-
-// sums over the CTA in a fixed order (xor butterfly in each warp, then the warps in order); every thread gets both
-// totals.  Two barriers.
-__device__ __forceinline__ void block_sum2(float& a, float& b, float* s_red) {
-  for (int o = 16; o > 0; o >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-  }
-  const int w = threadIdx.x / 32;
-  if (threadIdx.x % 32 == 0) {
-    s_red[w] = a;
-    s_red[kWarps + w] = b;
-  }
-  __syncthreads();
-  a = s_red[0];
-  b = s_red[kWarps];
-  for (int i = 1; i < kWarps; ++i) {
-    a += s_red[i];
-    b += s_red[kWarps + i];
-  }
-  __syncthreads();
 }
 
 // e [B, lde] (first E columns), m [B, nb Ep], b2 [nb E], gamma / beta [E] -> v [B, nb Ep], stats [B, 2]
@@ -76,7 +55,7 @@ mask_fwd_kernel(const float* __restrict__ e, int lde, const float* __restrict__ 
       x[j] = c < E ? e[b * lde + c] : 0.f;
       s += x[j];
     }
-    block_sum2(s, unused, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(s, unused, s_red);
     const float mean = s / (float)E;
     float sq = 0.f;
 #pragma unroll
@@ -85,7 +64,7 @@ mask_fwd_kernel(const float* __restrict__ e, int lde, const float* __restrict__ 
       const float d = x[j] - mean;
       if (c < E) sq += d * d;
     }
-    block_sum2(sq, unused, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(sq, unused, s_red);
     const float rstd = 1.0f / sqrtf(sq / (float)E + kEps);
 #pragma unroll
     for (int j = 0; j < kVpt; ++j) {
@@ -162,7 +141,7 @@ mask_bwd_kernel(const float* __restrict__ e, int lde, const float* __restrict__ 
       sg += g[j];
       sgx += g[j] * xh[j];
     }
-    block_sum2(sg, sgx, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(sg, sgx, s_red);
     const float mg = sg / (float)E, mgx = sgx / (float)E;
 #pragma unroll
     for (int j = 0; j < kVpt; ++j) {
@@ -206,7 +185,7 @@ ffn_fwd_kernel(const float* __restrict__ z, const float* __restrict__ b3, const 
       x[j] = c < H ? zr[c] + __ldg(b3i + c) : 0.f;
       s += x[j];
     }
-    block_sum2(s, unused, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(s, unused, s_red);
     const float mean = s / (float)H;
     float sq = 0.f;
 #pragma unroll
@@ -215,7 +194,7 @@ ffn_fwd_kernel(const float* __restrict__ z, const float* __restrict__ b3, const 
       const float d = x[j] - mean;
       if (c < H) sq += d * d;
     }
-    block_sum2(sq, unused, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(sq, unused, s_red);
     const float rstd = 1.0f / sqrtf(sq / (float)H + kEps);
     float* yr = y + b * ld + (int64_t)i * H;
 #pragma unroll
@@ -264,7 +243,7 @@ ffn_bwd_kernel(const float* __restrict__ z, const float* __restrict__ b3, const 
       sg += g[j];
       sgx += g[j] * xh[j];
     }
-    block_sum2(sg, sgx, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(sg, sgx, s_red);
     const float mg = sg / (float)H, mgx = sgx / (float)H;
 #pragma unroll
     for (int j = 0; j < kVpt; ++j) {
@@ -288,17 +267,6 @@ ffn_bwd_kernel(const float* __restrict__ z, const float* __restrict__ b3, const 
   }
 }
 
-// out[s, e] = sum over the G rows of partials [S][G][P], in row order; blockIdx.y = s
-__global__ void __launch_bounds__(256) reduce_kernel(const float* __restrict__ partials, int G, int P,
-                                                     float* __restrict__ out) {
-  const int e = blockIdx.x * 256 + threadIdx.x;
-  if (e >= P) return;
-  const float* p = partials + (int64_t)blockIdx.y * G * P;
-  float acc = 0.f;
-  for (int g = 0; g < G; ++g) acc += p[(int64_t)g * P + e];
-  out[(int64_t)blockIdx.y * P + e] = acc;
-}
-
 // ---- launchers (return 0, or 1 on unsupported arguments) -------------------------------------------------------------
 inline size_t mask_bwd_smem(int Ep, int nb) { return sizeof(float) * (size_t)nb * Ep; }
 
@@ -317,14 +285,10 @@ inline int mask_bwd(const float* e, int lde, const float* m, const float* b2, co
                     float* partials, float* dparams, cudaStream_t stream) {
   const int Ep = pad4(E);
   if (!usable(E, 4, nb) || lde < E || grid < 1) return 1;
-  const int P = (nb + 2) * E;
-  if (B == 0) {
-    TZK_LAUNCH((reduce_kernel), dim3((P + 255) / 256, 1), 256, 0, stream, partials, 0, P, dparams);
-    return 0;
-  }
-  TZK_LAUNCH((mask_bwd_kernel), grid, kThreads, mask_bwd_smem(Ep, nb), stream, e, lde, m, b2, gamma, beta, stats, dv,
-             B, E, Ep, nb, dm, de, partials);
-  TZK_LAUNCH((reduce_kernel), dim3((P + 255) / 256, 1), 256, 0, stream, partials, grid, P, dparams);
+  if (B > 0)
+    TZK_LAUNCH((mask_bwd_kernel), grid, kThreads, mask_bwd_smem(Ep, nb), stream, e, lde, m, b2, gamma, beta, stats,
+               dv, B, E, Ep, nb, dm, de, partials);
+  tzk_batch_sum::reduce(partials, B > 0 ? grid : 0, (nb + 2) * E, 1, dparams, stream);
   return 0;
 }
 
@@ -341,14 +305,10 @@ inline int ffn_bwd(const float* z, const float* b3, const float* gamma, const fl
                    const float* dy, int64_t B, int H, int nb, int grid, float* dz, float* partials, float* dparams,
                    cudaStream_t stream) {
   if (!usable(1, H, nb) || grid < 1) return 1;
-  const int P = 3 * H;
-  if (B == 0) {
-    TZK_LAUNCH((reduce_kernel), dim3((P + 255) / 256, nb), 256, 0, stream, partials, 0, P, dparams);
-    return 0;
-  }
-  TZK_LAUNCH((ffn_bwd_kernel), dim3(grid, nb), kThreads, 0, stream, z, b3, gamma, beta, stats, dy, B, H, nb, dz,
-             partials);
-  TZK_LAUNCH((reduce_kernel), dim3((P + 255) / 256, nb), 256, 0, stream, partials, grid, P, dparams);
+  if (B > 0)
+    TZK_LAUNCH((ffn_bwd_kernel), dim3(grid, nb), kThreads, 0, stream, z, b3, gamma, beta, stats, dy, B, H, nb, dz,
+               partials);
+  tzk_batch_sum::reduce(partials, B > 0 ? grid : 0, 3 * H, nb, dparams, stream);
   return 0;
 }
 }  // namespace tzk_masknet

@@ -2,9 +2,7 @@
 // own, so no kernel of the training step is recompiled by it.
 #include "tzk_common.cuh"
 
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#include "tzk_launch.cuh"
 #include "tzk_metrics.cuh"
 
 using namespace tzk;

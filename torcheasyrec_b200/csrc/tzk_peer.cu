@@ -38,9 +38,7 @@
 #else
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#include "tzk_launch.cuh"
 #endif
 #include <stdint.h>
 #include <stdlib.h>

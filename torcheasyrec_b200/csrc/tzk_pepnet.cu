@@ -2,8 +2,6 @@
 // its own, so no existing kernel is recompiled by it.
 #include "tzk_common.cuh"
 
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #include "tzk_pepnet.cuh"
 
 using namespace tzk;

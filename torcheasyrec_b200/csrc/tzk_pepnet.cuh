@@ -11,17 +11,18 @@
 // buffer are fine), so every access is 128-bit.  blockIdx.y is the segment; a CTA of 256 threads covers R = 256 / (N/4)
 // rows per step (thread t owns column quad t % (N/4) of row t / (N/4)) and walks the rows grid-stride.  In the backward
 // each thread keeps its quad's batch sums in registers, the R rows of the CTA are added in row order through shared
-// memory into the CTA's row of a partials buffer, and reduce_kernel adds the rows in CTA order.  No float atomics: the
-// sums depend only on the grid, which the host derives from B, the shapes and the SM count, so a replayed graph gives
-// the eager bits.
+// memory into the CTA's row of a partials buffer, and tzk_batch_sum::reduce adds the rows in CTA order
+// (tzk_batch_sum.cuh).
 //
-// fp32 throughout.  Plain CUDA (no PTX): the includer provides TZK_LAUNCH (nvcc: tzk_pepnet.cu; g++ +
-// tests/native/cuda_cpu_shim.h: tests/test_pepnet_cpu.py runs this source on the host against float64).
+// fp32 throughout.  Plain CUDA (no PTX): nvcc builds it in tzk_pepnet.cu; g++ + tests/native/cuda_cpu_shim.h:
+// tests/test_pepnet_cpu.py runs this source on the host against float64.
 #pragma once
 #include <math.h>
 #include <stdint.h>
 
 #include "../../include/tzk.h"
+#include "tzk_batch_sum.cuh"
+#include "tzk_launch.cuh"
 
 namespace tzk_pepnet {
 constexpr int kThreads = 256;
@@ -132,16 +133,6 @@ __global__ void __launch_bounds__(kThreads) gate_bwd_kernel(const __grid_constan
   }
 }
 
-// out[e] = sum over the G rows of partials [G][P], in row order
-__global__ void __launch_bounds__(256) reduce_kernel(const float* __restrict__ partials, int G, int64_t P,
-                                                     float* __restrict__ out) {
-  const int64_t e = (int64_t)blockIdx.x * 256 + threadIdx.x;
-  if (e >= P) return;
-  float acc = 0.f;
-  for (int g = 0; g < G; ++g) acc += partials[(int64_t)g * P + e];
-  out[e] = acc;
-}
-
 // ---- launchers (return 0, or 1 on arguments outside the cover) --------------------------------------------------------
 inline int gate_fwd(const tzk_pepnet_gate_args& a, int grid, cudaStream_t stream) {
   if (check(a, false) != 0 || grid < 1) return 1;
@@ -154,13 +145,8 @@ inline int gate_fwd(const tzk_pepnet_gate_args& a, int grid, cudaStream_t stream
 inline int gate_bwd(const tzk_pepnet_gate_args& a, int grid, float* partials, float* dparams, cudaStream_t stream) {
   if (check(a, true) != 0 || grid < 1) return 1;
   const int64_t P = partial_floats(a);
-  const unsigned rb = (unsigned)((P + 255) / 256);
-  if (a.B == 0) {
-    TZK_LAUNCH((reduce_kernel), dim3(rb), 256, 0, stream, partials, 0, P, dparams);
-    return 0;
-  }
-  TZK_LAUNCH((gate_bwd_kernel), dim3(grid, a.n_segs), kThreads, 0, stream, a, partials, P);
-  TZK_LAUNCH((reduce_kernel), dim3(rb), 256, 0, stream, partials, grid, P, dparams);
+  if (a.B > 0) TZK_LAUNCH((gate_bwd_kernel), dim3(grid, a.n_segs), kThreads, 0, stream, a, partials, P);
+  tzk_batch_sum::reduce(partials, a.B > 0 ? grid : 0, P, 1, dparams, stream);
   return 0;
 }
 }  // namespace tzk_pepnet

@@ -2,10 +2,6 @@
 // own, so no existing kernel is recompiled by it.
 #include "tzk_common.cuh"
 
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
-#define TZK_SET_MAX_SMEM(kernel, bytes) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes))
 #include "tzk_ple.cuh"
 
 using namespace tzk;

@@ -18,16 +18,17 @@
 // The backward's batch sums are owned, element by element, by one thread of the CTA: each CTA walks tiles of kTile
 // samples, the warps write the tile's dlogits to shared memory, then thread t adds them into its own elements of the
 // shared dW / db accumulators in sample order.  At the end each CTA writes its accumulators as one row of `partials`
-// and reduce_kernel adds the rows in CTA order.  No float atomics: the result depends only on the grid, which the host
-// derives from B, the shapes and the SM count, so a replayed graph gives the eager bits.
+// and tzk_batch_sum::reduce adds the rows in CTA order (tzk_batch_sum.cuh).
 //
-// Plain CUDA (no PTX): the includer provides TZK_DYN_SMEM / TZK_LAUNCH / TZK_SET_MAX_SMEM (nvcc: tzk_ple.cu; g++ +
-// tests/native/cuda_cpu_shim.h: tests/test_ple_cpu.py runs this source on the host against a float64 restatement).
+// Plain CUDA (no PTX): nvcc builds it in tzk_ple.cu; g++ + tests/native/cuda_cpu_shim.h: tests/test_ple_cpu.py runs
+// this source on the host against a float64 restatement.
 #pragma once
 #include <math.h>
 #include <stdint.h>
 
 #include "../../include/tzk.h"
+#include "tzk_batch_sum.cuh"
+#include "tzk_launch.cuh"
 
 namespace tzk_ple {
 constexpr int kThreads = 256;
@@ -270,16 +271,6 @@ __global__ void __launch_bounds__(kThreads) gate_bwd_kernel(const __grid_constan
   for (int i = threadIdx.x; i < a.sumEK + a.sumE; i += kThreads) out[i] = sdW[i];
 }
 
-// out[e] = sum over the G rows of partials [G][P], in row order
-__global__ void __launch_bounds__(256) reduce_kernel(const float* __restrict__ partials, int G, int P,
-                                                     float* __restrict__ out) {
-  const int e = blockIdx.x * 256 + threadIdx.x;
-  if (e >= P) return;
-  float acc = 0.f;
-  for (int g = 0; g < G; ++g) acc += partials[(int64_t)g * P + e];
-  out[e] = acc;
-}
-
 // ---- host side -------------------------------------------------------------------------------------------------------
 // Params from the C-ABI description, with the derived fields (sumE, sumEK, eoff, woff, pos); 0, or 1 when the layer is
 // outside the kernels' cover: 1 <= n_gates <= 9, 1 <= n_experts <= 64, 1 <= n_inputs <= 9, 1 <= H <= 1024,
@@ -334,7 +325,7 @@ inline int gate_fwd(const Params& a, int grid, float* y, float* p, cudaStream_t 
   if (grid < 1) return 1;
   if (a.B == 0) return 0;
   const size_t smem = fwd_smem(a);
-  TZK_SET_MAX_SMEM(gate_fwd_kernel, smem);
+  tzk_batch_sum::opt_in_smem(gate_fwd_kernel, smem);
   TZK_LAUNCH((gate_fwd_kernel), grid, kThreads, smem, stream, a, y, p);
   return 0;
 }
@@ -343,15 +334,12 @@ inline int gate_fwd(const Params& a, int grid, float* y, float* p, cudaStream_t 
 inline int gate_bwd(const Params& a, const float* p, const float* dy, int grid, float* d_experts, float* partials,
                     float* dparams, cudaStream_t stream) {
   if (grid < 1) return 1;
-  const int P = a.sumEK + a.sumE;
-  if (a.B == 0) {
-    TZK_LAUNCH((reduce_kernel), (P + 255) / 256, 256, 0, stream, partials, 0, P, dparams);
-    return 0;
+  if (a.B > 0) {
+    const size_t smem = bwd_smem(a);
+    tzk_batch_sum::opt_in_smem(gate_bwd_kernel, smem);
+    TZK_LAUNCH((gate_bwd_kernel), grid, kThreads, smem, stream, a, p, dy, d_experts, partials);
   }
-  const size_t smem = bwd_smem(a);
-  TZK_SET_MAX_SMEM(gate_bwd_kernel, smem);
-  TZK_LAUNCH((gate_bwd_kernel), grid, kThreads, smem, stream, a, p, dy, d_experts, partials);
-  TZK_LAUNCH((reduce_kernel), (P + 255) / 256, 256, 0, stream, partials, grid, P, dparams);
+  tzk_batch_sum::reduce(partials, a.B > 0 ? grid : 0, a.sumEK + a.sumE, 1, dparams, stream);
   return 0;
 }
 }  // namespace tzk_ple

@@ -13,9 +13,7 @@
 #include "tzk_common.cuh"
 
 // second backward implementation (plain CUDA, also compiled for the host by the CPU tests)
-#define TZK_DYN_SMEM(type, name) extern __shared__ __align__(16) type name[]
-#define TZK_UNPAREN(...) __VA_ARGS__
-#define TZK_LAUNCH(kernel, grid, block, smem, stream, ...) TZK_UNPAREN kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
+#include "tzk_launch.cuh"
 #include "tzk_tower_bwd2.cuh"
 #include "tzk_tower_tail.cuh"
 

@@ -7,23 +7,24 @@
 //   out_bwd / mix_bwd: the exact gradients.  F and z are recomputed from X / (fmb_out, base), not stored.
 //
 // Weight, gamma and beta gradients are sums over the batch: every CTA accumulates its own samples (grid-stride, always
-// the same samples for a given grid) in a fixed order into its row of a partials buffer, then reduce_kernel adds the
-// rows in CTA order.  No float atomics: the result depends only on the grid, which the host derives from B and the SM
-// count, so a replayed graph gives the eager step's bits.
+// the same samples for a given grid) in a fixed order into its row of a partials buffer, which tzk_batch_sum::reduce
+// adds in CTA order (tzk_batch_sum.cuh).
 //
 // fp32 FFMA throughout (the reference runs fp32 with TF32 off).  Every product of the layer is a matrix of at most
 // 64 x 32 x 64: too small for an MMA tile to pay for its fragment shuffles; see DESIGN.md (WuKong).
 //
-// Plain CUDA (no PTX): the includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_wukong.cu; g++ +
-// tests/native/cuda_cpu_shim.h: tests/test_wukong_cpu.py runs this source on the host against a float64 restatement).
+// Plain CUDA (no PTX): nvcc builds it in tzk_wukong.cu; g++ + tests/native/cuda_cpu_shim.h: tests/test_wukong_cpu.py
+// runs this source on the host against a float64 restatement.
 #pragma once
 #include <math.h>
 #include <stdint.h>
 
+#include "tzk_batch_sum.cuh"
+#include "tzk_launch.cuh"
+
 namespace tzk_wukong {
 constexpr int kThreads = 128;
 constexpr float kEps = 1e-5f;                 // nn.LayerNorm's default eps, both norms of the layer
-constexpr size_t kSmemDefault = 48 * 1024;    // above this a kernel must opt in to more dynamic shared memory
 
 // shapes the kernels cover (the Python side's wukong_usable states the same)
 inline bool usable(int n, int d, int k, int f, int l) {
@@ -37,28 +38,6 @@ __host__ __device__ inline int64_t mix_params(int n, int k, int f, int l, bool p
 }
 
 constexpr int kWarps = kThreads / 32;
-
-// sums over the CTA in a fixed order (xor butterfly in each warp, then the warps in order); every thread gets both
-// totals.  Two barriers.
-__device__ __forceinline__ void block_sum2(float& a, float& b, float* s_red) {
-  for (int o = 16; o > 0; o >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-  }
-  const int w = threadIdx.x / 32;
-  if (threadIdx.x % 32 == 0) {
-    s_red[w] = a;
-    s_red[kWarps + w] = b;
-  }
-  __syncthreads();
-  a = s_red[0];
-  b = s_red[kWarps];
-  for (int i = 1; i < kWarps; ++i) {
-    a += s_red[i];
-    b += s_red[kWarps + i];
-  }
-  __syncthreads();
-}
 
 inline size_t mix_fwd_smem(int n, int d, int k, int f, int l, bool proj) {
   const int m = f + l;
@@ -123,14 +102,14 @@ mix_fwd_kernel(const float* __restrict__ x, const float* __restrict__ wf, const 
       part += acc;
     }
     float unused = 0.f;
-    block_sum2(part, unused, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(part, unused, s_red);
     const float mean = part / (float)nk;
     float sq = 0.f;
     for (int e = t; e < nk; e += kThreads) {
       const float c = s_f[e] - mean;
       sq += c * c;
     }
-    block_sum2(sq, unused, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(sq, unused, s_red);
     const float rstd = 1.0f / sqrtf(sq / (float)nk + kEps);
     float* ob = ln_f + b * nk;
     for (int e = t; e < nk; e += kThreads) ob[e] = (s_f[e] - mean) * rstd * __ldg(gf + e) + __ldg(bf + e);
@@ -203,7 +182,7 @@ mix_bwd_kernel(const float* __restrict__ x, const float* __restrict__ wf, const 
       sg += g;
       sgx += g * xh;
     }
-    block_sum2(sg, sgx, s_red);
+    tzk_batch_sum::block_sum2<kWarps>(sg, sgx, s_red);
     const float mg = sg / (float)nk, mgx = sgx / (float)nk;
     for (int e = t; e < nk; e += kThreads) s_f[e] = rstd * (s_g[e] - mg - s_f[e] * mgx);
     __syncthreads();
@@ -255,16 +234,6 @@ mix_bwd_kernel(const float* __restrict__ x, const float* __restrict__ wf, const 
   }
   __syncthreads();
   for (int e = t; e < P; e += kThreads) partials[(int64_t)blockIdx.x * P + e] = s_acc[e];
-}
-
-// out[e] = sum over the G rows of partials [G, P], in row order
-__global__ void __launch_bounds__(256) reduce_kernel(const float* __restrict__ partials, int G, int P,
-                                                     float* __restrict__ out) {
-  const int e = blockIdx.x * 256 + threadIdx.x;
-  if (e >= P) return;
-  float acc = 0.f;
-  for (int g = 0; g < G; ++g) acc += partials[(int64_t)g * P + e];
-  out[e] = acc;
 }
 
 template <int D>
@@ -336,28 +305,13 @@ out_bwd_kernel(const float* __restrict__ fmb, const float* __restrict__ base, co
 }
 
 // ---- launchers (return 0, or 1 on unsupported arguments) -------------------------------------------------------------
-inline int reduce(const float* partials, int G, int P, float* out, cudaStream_t stream) {
-  TZK_LAUNCH((reduce_kernel), (P + 255) / 256, 256, 0, stream, partials, G, P, out);
-  return 0;
-}
-
-template <class K>
-inline void opt_in_smem(K kernel, size_t smem) {
-#ifndef TZK_CPU_SHIM
-  if (smem > kSmemDefault) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-#else
-  (void)kernel;
-  (void)smem;
-#endif
-}
-
 inline int mix_fwd(const float* x, const float* wf, const float* gf, const float* bf, const float* wl, const float* wr,
                    int64_t B, int n, int d, int k, int f, int l, int grid, float* ln_f, float* stats, float* base,
                    cudaStream_t stream) {
   if (!usable(n, d, k, f, l) || grid < 1) return 1;
   if (B == 0) return 0;
   const size_t smem = mix_fwd_smem(n, d, k, f, l, wr != nullptr);
-  opt_in_smem(mix_fwd_kernel, smem);
+  tzk_batch_sum::opt_in_smem(mix_fwd_kernel, smem);
   TZK_LAUNCH((mix_fwd_kernel), grid, kThreads, smem, stream, x, wf, gf, bf, wl, wr, B, n, d, k, f, l, ln_f, stats,
              base);
   return 0;
@@ -368,16 +322,14 @@ inline int mix_bwd(const float* x, const float* wf, const float* gf, const float
                    const float* stats, const float* d_ln_f, const float* d_base, int64_t B, int n, int d, int k, int f,
                    int l, int grid, float* dx, float* partials, float* dparams, cudaStream_t stream) {
   if (!usable(n, d, k, f, l) || grid < 1) return 1;
-  const int P = (int)mix_params(n, k, f, l, wr != nullptr);
-  if (B == 0) {
-    TZK_LAUNCH((reduce_kernel), (P + 255) / 256, 256, 0, stream, partials, 0, P, dparams);
-    return 0;
+  if (B > 0) {
+    const size_t smem = mix_bwd_smem(n, d, k, f, l, wr != nullptr);
+    tzk_batch_sum::opt_in_smem(mix_bwd_kernel, smem);
+    TZK_LAUNCH((mix_bwd_kernel), grid, kThreads, smem, stream, x, wf, gf, wl, wr, stats, d_ln_f, d_base, B, n, d, k,
+               f, l, dx, partials);
   }
-  const size_t smem = mix_bwd_smem(n, d, k, f, l, wr != nullptr);
-  opt_in_smem(mix_bwd_kernel, smem);
-  TZK_LAUNCH((mix_bwd_kernel), grid, kThreads, smem, stream, x, wf, gf, wl, wr, stats, d_ln_f, d_base, B, n, d, k, f,
-             l, dx, partials);
-  return reduce(partials, grid, P, dparams, stream);
+  tzk_batch_sum::reduce(partials, B > 0 ? grid : 0, mix_params(n, k, f, l, wr != nullptr), 1, dparams, stream);
+  return 0;
 }
 
 inline int out_fwd(const float* fmb, const float* base, const float* gamma, const float* beta, int64_t B, int d, int f,
@@ -402,16 +354,15 @@ inline int out_bwd(const float* fmb, const float* base, const float* gamma, cons
   if (!(d == 4 || d == 8 || d == 16 || d == 32) || f < 1 || l < 1 || grid < 1) return 1;
   const int64_t R = B * (f + l);
   const int m = f + l;
-  if (R == 0) {
-    TZK_LAUNCH((reduce_kernel), 1, 256, 0, stream, partials, 0, 2 * d, dparams);
-    return 0;
+  if (R > 0) {
+    switch (d) {
+      case 4: TZK_LAUNCH((out_bwd_kernel<4>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
+      case 8: TZK_LAUNCH((out_bwd_kernel<8>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
+      case 16: TZK_LAUNCH((out_bwd_kernel<16>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
+      default: TZK_LAUNCH((out_bwd_kernel<32>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
+    }
   }
-  switch (d) {
-    case 4: TZK_LAUNCH((out_bwd_kernel<4>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
-    case 8: TZK_LAUNCH((out_bwd_kernel<8>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
-    case 16: TZK_LAUNCH((out_bwd_kernel<16>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
-    default: TZK_LAUNCH((out_bwd_kernel<32>), grid, kThreads, 0, stream, fmb, base, gamma, stats, dy, R, f, m, d_fmb, d_base, partials); break;
-  }
-  return reduce(partials, grid, 2 * d, dparams, stream);
+  tzk_batch_sum::reduce(partials, R > 0 ? grid : 0, 2 * d, 1, dparams, stream);
+  return 0;
 }
 }  // namespace tzk_wukong

@@ -7,6 +7,7 @@ implementation here: host-logic tests inject their own checker backend (tests/or
 """
 
 import ctypes
+import math
 import os
 import threading
 from dataclasses import dataclass
@@ -1070,15 +1071,26 @@ class CudaKernels:
                                               _ptr(invalid), _stream()), "tzk_binned_auc_update")
         self.launches += int(n > 0)
 
-    # ------------------------------------------------------------------ WuKong layer (csrc/tzk_wukong.cuh)
-    def _wukong_grid(self, work: int, per_sm: int) -> int:
-        """CTAs of a WuKong launch: min(work, per_sm x SMs).  The weight-gradient partials are per CTA, so the grid
-        fixes the reduction order; it depends only on the batch size and the device."""
+    # ------------------------------------------------------------------ batch sums of the dense models' kernels
+    # (csrc/tzk_batch_sum.cuh).  Every CTA of a backward launch writes its share of the weight, gamma, beta and bias
+    # gradients as one row of `partials`, and the rows are added in CTA order: the grid fixes the order of the sums, so
+    # it depends only on the work, the shapes and the device.
+    def _grid(self, work: int, per_sm: int, slices: int = 1) -> int:
+        """CTAs along the work of a launch with `slices` CTAs in grid.y: min(work, ceil(per_sm x SMs / slices))."""
         sms = getattr(self, "_sms", None)
         if sms is None:
             sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
-        return max(1, min(int(work), per_sm * sms))
+        return max(1, min(int(work), -(-per_sm * sms // slices)))
 
+    def _batch_sums(self, key: str, grid: int, shapes, device):
+        """(partials, dparams, views): the cached workspace `key` for `grid` rows of partials, dparams, and dparams cut
+        into views of `shapes` in the order the kernel writes them."""
+        sizes = [math.prod(s) for s in shapes]
+        partials = self._workspace(key, grid * sum(sizes) * 4, device)
+        dparams = torch.empty(sum(sizes), dtype=torch.float32, device=device)
+        return partials, dparams, [v.view(s) for v, s in zip(dparams.split(sizes), shapes)]
+
+    # ------------------------------------------------------------------ WuKong layer (csrc/tzk_wukong.cuh)
     def wukong_mix_fwd(self, x, w_fmb, gamma, beta, w_lcb, w_res, f: int):
         """x [B, n, d] -> (ln_f [B, n k], stats [B, 2], base [B, f + l, d]); w_res None: identity residual."""
         for t, nm in ((x, "x"), (w_fmb, "w_fmb"), (gamma, "gamma"), (beta, "beta"), (w_lcb, "w_lcb")):
@@ -1092,7 +1104,7 @@ class CudaKernels:
         stats = torch.empty((B, 2), dtype=torch.float32, device=x.device)
         base = torch.empty((B, m, d), dtype=torch.float32, device=x.device)
         check(self._lib.tzk_wukong_mix_fwd(_ptr(x), _ptr(w_fmb), _ptr(gamma), _ptr(beta), _ptr(w_lcb), _ptr(w_res), B,
-                                           n, d, k, f, l, self._wukong_grid(B, 8), _ptr(ln_f), _ptr(stats), _ptr(base),
+                                           n, d, k, f, l, self._grid(B, 8), _ptr(ln_f), _ptr(stats), _ptr(base),
                                            _stream()), "tzk_wukong_mix_fwd")
         self.launches += int(B > 0)
         return ln_f, stats, base
@@ -1107,20 +1119,15 @@ class CudaKernels:
         B, n, d = x.shape
         k, l = w_fmb.shape[1], w_lcb.shape[1]
         m = f + l
-        nk, nr = n * k, (n * m if w_res is not None else 0)
-        P = 3 * nk + n * l + nr
-        grid = self._wukong_grid(B, 4)       # mix_bwd_kernel: 4 resident CTAs per SM (launch bounds)
+        grid = self._grid(B, 4)       # mix_bwd_kernel: 4 resident CTAs per SM (launch bounds)
         dx = torch.empty_like(x)
-        partials = self._workspace("wukong_mix_bwd", grid * P * 4, x.device)
-        dparams = torch.empty(P, dtype=torch.float32, device=x.device)
+        partials, dparams, (dw_fmb, dw_lcb, dw_res, dgamma, dbeta) = self._batch_sums(
+            "wukong_mix_bwd", grid, [(n, k), (n, l), (n, m if w_res is not None else 0), (n * k,), (n * k,)], x.device)
         check(self._lib.tzk_wukong_mix_bwd(_ptr(x), _ptr(w_fmb), _ptr(gamma), _ptr(w_lcb), _ptr(w_res), _ptr(stats),
                                            _ptr(d_ln_f), _ptr(d_base), B, n, d, k, f, l, grid, _ptr(dx),
                                            _ptr(partials), _ptr(dparams), _stream()), "tzk_wukong_mix_bwd")
         self.launches += 1 + int(B > 0)
-        o = [0, nk, nk + n * l, nk + n * l + nr, 2 * nk + n * l + nr, P]
-        dw_res = dparams[o[2]:o[3]].view(n, m) if w_res is not None else None
-        return (dx, dparams[o[0]:o[1]].view(n, k), dparams[o[3]:o[4]], dparams[o[4]:o[5]],
-                dparams[o[1]:o[2]].view(n, l), dw_res)
+        return dx, dw_fmb, dgamma, dbeta, dw_lcb, (dw_res if w_res is not None else None)
 
     def wukong_out_fwd(self, fmb_out, base, gamma, beta, f: int):
         """fmb_out [B, f d], base [B, m, d] -> (y [B, m, d], stats [B, m, 2])."""
@@ -1130,7 +1137,7 @@ class CudaKernels:
         y = torch.empty_like(base)
         stats = torch.empty((B, m, 2), dtype=torch.float32, device=base.device)
         check(self._lib.tzk_wukong_out_fwd(_ptr(fmb_out), _ptr(base), _ptr(gamma), _ptr(beta), B, d, f, m - f,
-                                           self._wukong_grid(-(-B * m // 128), 8), _ptr(y), _ptr(stats), _stream()),
+                                           self._grid(-(-B * m // 128), 8), _ptr(y), _ptr(stats), _stream()),
               "tzk_wukong_out_fwd")
         self.launches += int(B > 0)
         return y, stats
@@ -1140,26 +1147,19 @@ class CudaKernels:
         for t, nm in ((fmb_out, "fmb_out"), (base, "base"), (gamma, "gamma"), (stats, "stats"), (dy, "dy")):
             _need(t, torch.float32, nm)
         B, m, d = base.shape
-        grid = self._wukong_grid(-(-B * m // 128), 4)
+        grid = self._grid(-(-B * m // 128), 4)
         d_fmb = torch.empty_like(fmb_out)
         d_base = torch.empty_like(base)
-        partials = self._workspace("wukong_out_bwd", grid * 2 * d * 4, base.device)
-        dparams = torch.empty(2 * d, dtype=torch.float32, device=base.device)
+        partials, dparams, (dgamma, dbeta) = self._batch_sums("wukong_out_bwd", grid, [(d,), (d,)], base.device)
         check(self._lib.tzk_wukong_out_bwd(_ptr(fmb_out), _ptr(base), _ptr(gamma), _ptr(stats), _ptr(dy), B, d, f,
                                            m - f, grid, _ptr(d_fmb), _ptr(d_base), _ptr(partials), _ptr(dparams),
                                            _stream()), "tzk_wukong_out_bwd")
         self.launches += 1 + int(B > 0)
-        return d_fmb, d_base, dparams[:d], dparams[d:]
+        return d_fmb, d_base, dgamma, dbeta
 
     # ------------------------------------------------------------------ MaskNet (csrc/tzk_masknet.cuh)
     # CTAs per SM of each launch (ptxas register counts at 128 threads: mask_fwd 45, mask_bwd 70, ffn_fwd 78,
-    # ffn_bwd 96); the grid fixes the order of the batch sums and depends only on the batch size and the device.
-    def _masknet_grid(self, B: int, per_sm: int, nb: int = 1) -> int:
-        """CTAs along the rows: min(B, per_sm x SMs / nb), nb = the launch's grid.y (one slice per mask block)."""
-        sms = getattr(self, "_sms", None)
-        if sms is None:
-            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
-        return max(1, min(int(B), -(-per_sm * sms // nb)))
+    # ffn_bwd 96); the FFN launches have one grid.y slice per mask block.
 
     def masknet_mask_fwd(self, e, m, b2, gamma, beta, E: int, nb: int):
         """e [B, Ep] (first E columns live), m [B, nb Ep] -> (v [B, nb Ep], stats [B, 2]); Ep = pad4(E)."""
@@ -1169,7 +1169,7 @@ class CudaKernels:
         v = torch.empty_like(m)
         stats = torch.empty((B, 2), dtype=torch.float32, device=e.device)
         check(self._lib.tzk_masknet_mask_fwd(_ptr(e), e.shape[1], _ptr(m), _ptr(b2), _ptr(gamma), _ptr(beta), B, E, nb,
-                                             self._masknet_grid(B, 8), _ptr(v), _ptr(stats), _stream()),
+                                             self._grid(B, 8), _ptr(v), _ptr(stats), _stream()),
               "tzk_masknet_mask_fwd")
         self.launches += int(B > 0)
         return v, stats
@@ -1180,17 +1180,16 @@ class CudaKernels:
                       (dv, "dv")):
             _need(t, torch.float32, nm)
         B = e.shape[0]
-        P = (nb + 2) * E
-        grid = self._masknet_grid(B, 6)
+        grid = self._grid(B, 6)
         dm = torch.empty_like(m)
         de = torch.empty_like(e)
-        partials = self._workspace("masknet_mask_bwd", grid * P * 4, e.device)
-        dparams = torch.empty(P, dtype=torch.float32, device=e.device)
+        partials, dparams, (db2, dgamma, dbeta) = self._batch_sums("masknet_mask_bwd", grid, [(nb * E,), (E,), (E,)],
+                                                                   e.device)
         check(self._lib.tzk_masknet_mask_bwd(_ptr(e), e.shape[1], _ptr(m), _ptr(b2), _ptr(gamma), _ptr(beta),
                                              _ptr(stats), _ptr(dv), B, E, nb, grid, _ptr(dm), _ptr(de),
                                              _ptr(partials), _ptr(dparams), _stream()), "tzk_masknet_mask_bwd")
         self.launches += 1 + int(B > 0)
-        return dm, de, dparams[:nb * E], dparams[nb * E:(nb + 1) * E], dparams[(nb + 1) * E:]
+        return dm, de, db2, dgamma, dbeta
 
     def masknet_ffn_fwd(self, z, b3, gamma, beta, nb: int):
         """z [B, nb H] -> (y [B, nb H] = ReLU(LN_H(z_i + b3_i)) per block, stats [B, nb, 2])."""
@@ -1200,7 +1199,7 @@ class CudaKernels:
         y = torch.empty_like(z)
         stats = torch.empty((B, nb, 2), dtype=torch.float32, device=z.device)
         check(self._lib.tzk_masknet_ffn_fwd(_ptr(z), _ptr(b3), _ptr(gamma), _ptr(beta), B, H, nb,
-                                            self._masknet_grid(B, 6, nb), _ptr(y), _ptr(stats), _stream()),
+                                            self._grid(B, 6, nb), _ptr(y), _ptr(stats), _stream()),
               "tzk_masknet_ffn_fwd")
         self.launches += int(B > 0)
         return y, stats
@@ -1210,15 +1209,14 @@ class CudaKernels:
         for t, nm in ((z, "z"), (b3, "b3"), (gamma, "gamma"), (beta, "beta"), (stats, "stats"), (dy, "dy")):
             _need(t, torch.float32, nm)
         B, H = z.shape[0], z.shape[1] // nb
-        grid = self._masknet_grid(B, 5, nb)
+        grid = self._grid(B, 5, nb)
         dz = torch.empty_like(z)
-        partials = self._workspace("masknet_ffn_bwd", nb * grid * 3 * H * 4, z.device)
-        dparams = torch.empty((nb, 3, H), dtype=torch.float32, device=z.device)
+        partials, dparams, (g3,) = self._batch_sums("masknet_ffn_bwd", grid, [(nb, 3, H)], z.device)
         check(self._lib.tzk_masknet_ffn_bwd(_ptr(z), _ptr(b3), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(dy), B, H,
                                             nb, grid, _ptr(dz), _ptr(partials), _ptr(dparams), _stream()),
               "tzk_masknet_ffn_bwd")
         self.launches += 1 + int(B > 0)
-        return dz, dparams[:, 0], dparams[:, 1], dparams[:, 2]
+        return dz, g3[:, 0], g3[:, 1], g3[:, 2]
 
     # ------------------------------------------------------------------ PLE gates (csrc/tzk_ple.cuh)
     # Resident CTAs per SM: ptxas register counts at 256 threads (gate_fwd 58 -> 4, gate_bwd 79 -> 3), fewer when the
@@ -1250,14 +1248,11 @@ class CudaKernels:
         return a
 
     def _ple_grid(self, a, B: int, rows_per_cta: int, per_sm_regs: int, backward: int) -> int:
-        sms = getattr(self, "_sms", None)
-        if sms is None:
-            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
         smem = int(self._lib.tzk_ple_gate_smem_bytes(ctypes.byref(a), backward))
         if smem == 0:
             raise TzkError("ple gates: layer outside the kernels' cover (Fn.ple_gate_usable)")
         per_sm = max(1, min(per_sm_regs, (227 * 1024) // (smem + 1024)))
-        return max(1, min(-(-int(B) // rows_per_cta), per_sm * sms))
+        return self._grid(-(-int(B) // rows_per_cta), per_sm)
 
     def ple_gate_fwd(self, inputs, gate_input, weights, biases, experts, gate_experts):
         """One extraction layer's gates -> (y [n_gates, B, H], p [B, sum E_g] the softmax of every gate)."""
@@ -1280,25 +1275,14 @@ class CudaKernels:
         a = self._ple_args(inputs, gate_input, weights, biases, experts, gate_experts, d_inputs)
         B, H = a.B, a.H
         dev = experts[0].device
-        sizes = [w.numel() for w in weights]
-        Es = [len(e) for e in gate_experts]
-        P = sum(sizes) + sum(Es)
         grid = self._ple_grid(a, B, 16, 3, 1)
         d_experts = torch.empty((len(experts), B, H), dtype=torch.float32, device=dev)
-        partials = self._workspace("ple_gate_bwd", grid * P * 4, dev)
-        dparams = torch.empty(P, dtype=torch.float32, device=dev)
+        partials, dparams, views = self._batch_sums(
+            "ple_gate_bwd", grid, [tuple(w.shape) for w in weights] + [(len(e),) for e in gate_experts], dev)
         check(self._lib.tzk_ple_gate_bwd(ctypes.byref(a), _ptr(p), _ptr(dy), grid, _ptr(d_experts), _ptr(partials),
                                          _ptr(dparams), _stream()), "tzk_ple_gate_bwd")
         self.launches += 1 + int(B > 0)
-        dW, o = [], 0
-        for w, n in zip(weights, sizes):
-            dW.append(dparams[o:o + n].view_as(w))
-            o += n
-        db = []
-        for e in Es:
-            db.append(dparams[o:o + e])
-            o += e
-        return d_inputs, d_experts, dW, db
+        return d_inputs, d_experts, views[:len(weights)], views[len(weights):]
 
     # ------------------------------------------------------------------ PEPNet gate product (csrc/tzk_pepnet.cuh)
     # Resident CTAs per SM: ptxas register counts at 256 threads (gate_fwd 35 -> 6, gate_bwd 72 -> 3).  The grid fixes
@@ -1334,11 +1318,8 @@ class CudaKernels:
         return a
 
     def _pepnet_grid(self, a, per_sm: int) -> int:
-        sms = getattr(self, "_sms", None)
-        if sms is None:
-            sms = self._sms = max(1, int(self._lib.tzk_sm_count()))
         rows = min(256 // (a.seg[s].N // 4) for s in range(a.n_segs))
-        return max(1, min(-(-int(a.B) // rows), -(-per_sm * sms // a.n_segs)))
+        return self._grid(-(-int(a.B) // rows), per_sm, a.n_segs)
 
     def pepnet_gate_fwd(self, segs):
         """y = act(x + bx) * gamma sigmoid(z + bz) into every segment's y (written in place)."""
@@ -1350,20 +1331,14 @@ class CudaKernels:
     def pepnet_gate_bwd(self, segs, dys, dxs, dzs):
         """dys -> dxs, dzs (written in place), returns [(dbx, dbz)] per segment."""
         a = self._pepnet_args(segs, dys, dxs, dzs)
-        P = sum(2 * s[0].shape[1] for s in segs)
         dev = segs[0][0].device
         grid = self._pepnet_grid(a, 3)
-        partials = self._workspace("pepnet_gate_bwd", grid * P * 4, dev)
-        dparams = torch.empty(P, dtype=torch.float32, device=dev)
+        partials, dparams, views = self._batch_sums("pepnet_gate_bwd", grid,
+                                                    [(s[0].shape[1],) for s in segs for _ in range(2)], dev)
         check(self._lib.tzk_pepnet_gate_bwd(ctypes.byref(a), grid, _ptr(partials), _ptr(dparams), _stream()),
               "tzk_pepnet_gate_bwd")
         self.launches += 1 + int(a.B > 0)
-        out, o = [], 0
-        for s in segs:
-            N = s[0].shape[1]
-            out.append((dparams[o:o + N], dparams[o + N:o + 2 * N]))
-            o += 2 * N
-        return out
+        return list(zip(views[0::2], views[1::2]))
 
 
 @dataclass
