@@ -700,6 +700,17 @@ int tzk_pepnet_gate_fwd(const tzk_pepnet_gate_args* args_host, int32_t grid, tzk
 int tzk_pepnet_gate_bwd(const tzk_pepnet_gate_args* args_host, int32_t grid, float* partials, float* dparams,
                         tzk_stream_t stream);
 
+/* ---- JRC loss (tzrec/loss/jrc_loss.py) and its gradient in one call, O(B) memory.  logits [B, 2] with row pitch
+ * ld >= 2, labels [B] fp32 (0 or 1), session_ids [B] int64 (ids in [0, 2^key_bits); key_bits 64 for any id),
+ * weights [B] or NULL.  loss[0] = (1/B) sum_i w_i (alpha ce_i + (1 - alpha) ge_i) with w_i = 1 when weights is NULL;
+ * dlogits [B, 2] contiguous = d loss / d logits.  NaN loss (finite gradient) for B = 0 and, with weights NULL, for a
+ * batch without a positive or a negative; a label outside {0, 1} gives a NaN loss and gradient row.  Deterministic
+ * (no float atomics), no host synchronisation: graph-capturable. */
+size_t tzk_jrc_loss_workspace_bytes(int64_t B);
+int tzk_jrc_loss(const float* logits, int64_t ld, const float* labels, const int64_t* session_ids,
+                 const float* weights, int64_t B, float alpha, int32_t key_bits, float* loss, float* dlogits,
+                 void* workspace, size_t workspace_bytes, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -215,6 +215,9 @@ SIGNATURES = {
     # PEPNet: the gate-neural-unit product of up to 8 segments (the segments described by TzkPepnetGateArgs)
     "tzk_pepnet_gate_fwd": (c_int32, [P, c_int32, P]),
     "tzk_pepnet_gate_bwd": (c_int32, [P, c_int32, P, P, P]),
+    # JRC loss: session sort, per-session sums, loss and d loss / d logits in one call
+    "tzk_jrc_loss_workspace_bytes": (c_size_t, [c_int64]),
+    "tzk_jrc_loss": (c_int32, [P, c_int64, P, P, P, c_int64, c_float, c_int32, P, P, P, c_size_t, P]),
 }
 
 _lib = None

@@ -131,7 +131,7 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
                   "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE",
-                  "pepnet": "PEPNet"}.get(k, "Generic"))
+                  "pepnet": "PEPNet", "dbmtl": "DBMTL"}.get(k, "Generic"))
            for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
@@ -166,13 +166,23 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
                   "num_class": _f(I, 1), "mlp": _f("MLP"), "weight": _f(F, 1.0), "sample_weight_name": _f(S),
                   "task_space_indicator_label": _f(S), "in_task_space_weight": _f(F, 1.0),
                   "out_task_space_weight": _f(F, 1.0)},
+    "DBMTL": {"mask_net": _f("MaskNetModule"), "bottom_mlp": _f("MLP"), "expert_mlp": _f("MLP"), "gate_mlp": _f("MLP"),
+              "num_expert": _f(I, 3), "task_towers": _f("BayesTaskTower", rep=True)},
     "LossConfig": {"binary_cross_entropy": _f("Generic"), "softmax_cross_entropy": _f("Generic"),
-                   "l2_loss": _f("Generic"), "jrc_loss": _f("Generic"), "binary_focal_loss": _f("Generic")},
+                   "l2_loss": _f("Generic"), "jrc_loss": _f("JRCLoss"), "binary_focal_loss": _f("Generic")},
+    "JRCLoss": {"session_name": _f(S), "alpha": _f(F, 0.5)},
+    "SeqEncoderConfig": {"din_encoder": _f("DINEncoder"), "simple_attention": _f("Generic"),
+                         "pooling_encoder": _f("Generic"), "multi_window_din_encoder": _f("Generic"),
+                         "self_attention_encoder": _f("Generic")},
+    "DINEncoder": {"name": _f(S), "input": _f(S), "attn_mlp": _f("MLP"), "max_seq_length": _f(I, 0)},
     "MetricConfig": {"auc": _f("AUC"), "multiclass_auc": _f("Generic"), "recall_at_k": _f("Generic"),
                      "mean_absolute_error": _f("Generic"), "mean_squared_error": _f("Generic"),
                      "accuracy": _f("Generic"), "grouped_auc": _f("Generic")},
     "AUC": {"thresholds": _f(I, 200)},
 }
+
+SCHEMA["BayesTaskTower"] = dict(SCHEMA["TaskTower"], relation_tower_names=_f(S, rep=True), relation_mlp=_f("MLP"),
+                                pareto_min_loss_weight=_f(F, 0.0))
 
 ONEOFS: Dict[str, Dict[str, List[str]]] = {
     "SparseOptimizer": {"optimizer": ["sgd_optimizer", "adagrad_optimizer", "adam_optimizer", "lars_sgd_optimizer",
@@ -190,6 +200,8 @@ ONEOFS: Dict[str, Dict[str, List[str]]] = {
     "MetricConfig": {"metric": ["auc", "multiclass_auc", "recall_at_k", "mean_absolute_error",
                                 "mean_squared_error", "accuracy", "grouped_auc"]},
     "RawFeature": {"dense_emb": ["autodis", "mlp"]},
+    "SeqEncoderConfig": {"seq_module": ["din_encoder", "simple_attention", "pooling_encoder",
+                                        "multi_window_din_encoder", "self_attention_encoder"]},
 }
 
 

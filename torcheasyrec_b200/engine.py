@@ -12,6 +12,7 @@ import contextlib
 import os
 from typing import Any, Dict, Iterable, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from .batch import Batch, synthetic_batch
@@ -127,11 +128,29 @@ class Pipeline:
         return out
 
     def synthetic_batch(self, batch_size: int, seed: int = 0, id_dist: str = "uniform") -> Batch:
+        """A seeded host batch (batch.synthetic_batch).  For a model with a jrc_loss tower, the session feature's ids are
+        drawn over min(ceil(B / 8), table rows) values, so sessions average 8 samples: uniform ids over a table as large
+        as Taobao's users would make almost every session a singleton, whose JRC term is 0."""
         mc = self.cfg.model_config
         pep = mc.pepnet if mc.WhichOneof("model") == "pepnet" else None
         card = ({pep.domain_input_name: pep.task_domain_num}
                 if pep is not None and pep.HasField("domain_input_name") else None)
         b = synthetic_batch(self.features, batch_size, self.labels, seed=seed, id_dist=id_dist, label_cardinality=card)
+        sessions = {lc.jrc_loss.session_name for tc in getattr(getattr(mc, mc.WhichOneof("model")), "task_towers", None) or []
+                    for lc in tc.losses if lc.WhichOneof("loss") == "jrc_loss"}
+        if sessions:
+            from .features import BASE_DATA_GROUP
+
+            kjt = b.sparse_features[BASE_DATA_GROUP]
+            rng = np.random.default_rng(seed + 1)
+            lens = kjt.lengths()
+            rows = {f.name: f.num_embeddings for f in self.features}
+            for name in sorted(sessions):
+                f = kjt.keys().index(name)
+                hi = min(-(-batch_size // 8), rows.get(name) or -(-batch_size // 8))
+                s = int(lens[:f * batch_size].sum())
+                n = int(lens[f * batch_size:(f + 1) * batch_size].sum())
+                kjt.values()[s:s + n] = torch.from_numpy(rng.integers(0, hi, size=n))
         for kjt in b.sparse_features.values():
             kjt.length_per_key()  # host-side, before the copy: keeps the device path free of syncs
         return b

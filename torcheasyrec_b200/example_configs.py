@@ -244,9 +244,76 @@ def multi_tower_din_taobao() -> str:
             + "    }\n    metrics {\n        auc {}\n    }\n    losses {\n        binary_cross_entropy {}\n    }\n}\n")
 
 
+def _dbmtl_towers(thresholds: int, loss: str, num_class: str = "") -> str:
+    def tower(name, label, auc, extra=""):
+        return ("        task_towers {\n"
+                f'            tower_name: "{name}"\n            label_name: "{label}"\n{num_class}'
+                + _mlp("mlp", [256, 128, 64], "            ")
+                + f"            metrics {{\n                {auc}\n            }}\n"
+                f"            losses {{\n                {loss}\n            }}\n{extra}        }}\n")
+    rel = '            relation_tower_names: "ctr"\n' + _mlp("relation_mlp", [64], "            ")
+    return tower("ctr", "clk", "auc {}") + tower("cvr", "buy", f"auc {{ thresholds: {thresholds} }}", rel)
+
+
+def dbmtl_taobao() -> str:
+    """examples/dbmtl_taobao.config: mmoe_taobao's features and group `all`; dbmtl{bottom MLP 512; towers ctr and cvr
+    with MLP 256-128-64, cvr related to ctr through a relation MLP 64}."""
+    return (_header("taobao_multitask_sample_v1_train", "taobao_multitask_sample_v1/ds=20170513", "dbmtl_taobao",
+                    "FG_DAG", ["clk", "buy"], None, quota=False)
+            + _taobao_features()
+            + "model_config {\n" + _group("all", TAOBAO_MMOE_ORDER, "DEEP")
+            + "    dbmtl {\n" + _mlp("bottom_mlp", [512], "        ")
+            + _dbmtl_towers(1000, "binary_cross_entropy {}") + "    }\n}\n")
+
+
+def _taobao_bucketized_features() -> str:
+    """The FG_NONE Taobao features of the bucketized examples: ids without expressions, price as 101 buckets, pid 2."""
+    out = [_id_feature(n, None, r) for n, r in TAOBAO_USER + TAOBAO_ITEM]
+    return "".join(out) + _id_feature("price", None, 101) + _id_feature("pid", None, 2)
+
+
+def dbmtl_taobao_jrc() -> str:
+    """examples/dbmtl_taobao_jrc.config: dbmtl_taobao on the bucketized FG_NONE features, with two-class towers trained
+    by the JRC loss over sessions of `user_id` (cvr auc with 10000 thresholds)."""
+    return (_header("taobao_multitask_sample_bucketized_train_jrc", "taobao_multitask_sample_bucketized_v1/ds=20170513",
+                    "taobao/dbmtl_jrc", "FG_NONE", ["clk", "buy"], None, quota=False)
+            + _taobao_bucketized_features()
+            + "model_config {\n" + _group("all", TAOBAO_MMOE_ORDER, "DEEP")
+            + "    dbmtl {\n" + _mlp("bottom_mlp", [512], "        ")
+            + _dbmtl_towers(10000, 'jrc_loss {\n                    session_name: "user_id"\n                }',
+                            "            num_class: 2\n") + "    }\n}\n")
+
+
+def dbmtl_taobao_seq() -> str:
+    """examples/dbmtl_taobao_seq.config: dbmtl_taobao on the bucketized FG_NONE features plus click_50_seq (adgroup_id,
+    cate_id, brand; up to 100), whose sequence group sits inside the DEEP group `all` with a DIN encoder (attention MLP
+    32-8); BCE towers, cvr auc with 10000 thresholds."""
+    seq_feats = "".join(
+        "        features {\n            id_feature {\n"
+        f'                feature_name: "{n}"\n                num_buckets: {r}\n                embedding_dim: 16\n'
+        "            }\n        }\n" for n, r in [("adgroup_id", 846812), ("cate_id", 12961), ("brand", 461498)])
+    seq = ('feature_configs {\n    sequence_feature {\n        sequence_name: "click_50_seq",\n'
+           '        sequence_length: 100\n        sequence_delim: "|"\n' + seq_feats + "    }\n}\n")
+    names = "".join(f'            feature_names: "{f}"\n' for f in
+                    ["adgroup_id", "cate_id", "brand", "click_50_seq__adgroup_id", "click_50_seq__cate_id",
+                     "click_50_seq__brand"])
+    group = _group("all", TAOBAO_MMOE_ORDER, "DEEP")
+    group = group[:group.rindex("    }\n")] + (
+        '        sequence_groups {\n            group_name: "click_50_seq"\n' + names + "        }\n"
+        "        sequence_encoders {\n            din_encoder {\n" + _mlp("attn_mlp", [32, 8], "                ")
+        + "            }\n        }\n    }\n")
+    return (_header("taobao_multitask_sample_bucketized_train", "taobao_multitask_sample_bucketized_v1/ds=20170513",
+                    "taobao/dbmtl_seq", "FG_NONE", ["clk", "buy"], None, quota=False)
+            + _taobao_bucketized_features() + seq
+            + "model_config {\n" + group
+            + "    dbmtl {\n" + _mlp("bottom_mlp", [512], "        ")
+            + _dbmtl_towers(10000, "binary_cross_entropy {}") + "    }\n}\n")
+
+
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
               "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo,
-              "ple_taobao": ple_taobao, "pepnet_taobao": pepnet_taobao}
+              "ple_taobao": ple_taobao, "pepnet_taobao": pepnet_taobao, "dbmtl_taobao": dbmtl_taobao,
+              "dbmtl_taobao_jrc": dbmtl_taobao_jrc, "dbmtl_taobao_seq": dbmtl_taobao_seq}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
 EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}

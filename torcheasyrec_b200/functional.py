@@ -859,3 +859,85 @@ def pepnet_product(z: torch.Tensor, gates, gamma: float, inputs: Sequence[torch.
     params = ([m.weight for m in linears] + [m.bias for m in linears]) if linears else []
     params += [g.dense_layers[2].bias for g in gates]
     return _PepnetProduct.apply((len(inputs), T, bool(relu), float(gamma)), z, *inputs, *params)
+
+
+# --------------------------------------------------------------------------------------------------------
+# JRC loss (tzrec/loss/jrc_loss.py; csrc/tzk_jrc.cuh)
+# --------------------------------------------------------------------------------------------------------
+def torch_jrc_loss(logits: torch.Tensor, labels: torch.Tensor, session_ids: torch.Tensor, alpha: float,
+                   reduction: str = "mean") -> torch.Tensor:
+    """The JRC loss in O(B) torch ops: per sample alpha ce_i + (1 - alpha) ge_i, with ge_i the log-softmax of the
+    sample's own logit of its class against the same-class logits of the other class's samples of its session.
+    `reduction` "none": the [B] per-sample losses; "mean": their mean, NaN when the batch lacks a positive or a negative
+    (as the reference's empty cross-entropy mean times 0), with the gradient of the finite terms.  A label outside
+    {0, 1} gives a NaN term where the reference raises.  torch.unique reads the number of sessions on the host."""
+    logits = logits.float()
+    l0, l1 = logits[:, 0], logits[:, 1]
+    y = labels.float()
+    pos, neg = y == 1, y == 0
+    _, inv = torch.unique(session_ids, return_inverse=True)
+    U = int(inv.max()) + 1 if inv.numel() else 0
+
+    def side(x, member):
+        # per session: (max, sum exp(x - max)) over the members; the shift is a constant for autograd
+        xd = torch.where(member, x.detach(), torch.full_like(x, float("-inf")))
+        M = torch.full((U,), float("-inf"), dtype=x.dtype, device=x.device).scatter_reduce(0, inv, xd, "amax")
+        Ms = torch.where(torch.isfinite(M), M, torch.zeros_like(M))
+        xs = torch.where(member, x, Ms[inv])
+        S = torch.zeros(U, dtype=x.dtype, device=x.device).index_add(0, inv, torch.exp(xs - Ms[inv]) * member)
+        return M[inv], S[inv]
+
+    M1, S1 = side(l1, neg)                 # the negatives' l1, against which a positive competes
+    M0, S0 = side(l0, pos)                 # the positives' l0, against which a negative competes
+    x = torch.where(pos, l1, l0)
+    M, S = torch.where(pos, M1, M0), torch.where(pos, S1, S0)
+    m = torch.maximum(x.detach(), M)
+    ge = m - x + torch.log(torch.exp(x - m) + S * torch.exp(M - m))
+    invalid = torch.where(pos | neg, torch.zeros_like(y), torch.full_like(y, float("nan")))
+    ce = torch.logsumexp(logits, dim=1) - x + invalid
+    loss = alpha * ce + (1.0 - alpha) * ge
+    if reduction == "none":
+        return loss
+    nan_unless_both = torch.where(pos.any() & neg.any(), 0.0, float("nan")).to(loss.dtype)
+    return loss.mean() + nan_unless_both
+
+
+class _JrcLoss(torch.autograd.Function):
+    """The loss and d loss / d logits in one tzk_jrc_loss call; the backward scales the saved gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, session_ids, weights, alpha, key_bits):
+        loss, dlogits = backend().jrc_loss(_rows_contig(logits), labels, session_ids, weights, alpha, key_bits)
+        ctx.save_for_backward(dlogits)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        (dlogits,) = ctx.saved_tensors
+        return dlogits * g, None, None, None, None, None
+
+
+def jrc_usable(logits: torch.Tensor) -> bool:
+    """True when tzk_jrc_loss computes the loss: 2-D [B, 2] logits on CUDA (on the CPU only a test backend that
+    implements it)."""
+    if logits.dim() != 2 or logits.shape[1] != 2:
+        return False
+    if logits.is_cuda:
+        return _backend is None or hasattr(_backend, "jrc_loss")
+    return _backend is not None and hasattr(_backend, "jrc_loss")
+
+
+def jrc_loss(logits: torch.Tensor, labels: torch.Tensor, session_ids: torch.Tensor, alpha: float,
+             weights: Optional[torch.Tensor] = None, key_bits: int = 64) -> torch.Tensor:
+    """Scalar JRC loss: the mean of the per-sample losses (weights None, with the reference's NaN for a batch without a
+    positive or a negative) or the mean of the per-sample losses times `weights` [B].  The logits are taken in fp32, as
+    autocast runs cross_entropy.  session_ids must lie in [0, 2^key_bits).  Device work only on the fused path
+    (capturable); otherwise torch_jrc_loss, which reads the session count on the host."""
+    logits = logits.float()
+    if jrc_usable(logits):
+        y = labels.to(torch.float32).contiguous()
+        w = None if weights is None else weights.to(torch.float32).expand(logits.shape[0]).contiguous()
+        return _JrcLoss.apply(logits, y, session_ids.to(torch.int64).contiguous(), w, float(alpha), int(key_bits))
+    if weights is None:
+        return torch_jrc_loss(logits, labels, session_ids, alpha, "mean")
+    return torch.mean(torch_jrc_loss(logits, labels, session_ids, alpha, "none") * weights)

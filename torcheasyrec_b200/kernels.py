@@ -1340,6 +1340,30 @@ class CudaKernels:
         self.launches += 1 + int(a.B > 0)
         return list(zip(views[0::2], views[1::2]))
 
+    # ------------------------------------------------------------------ JRC loss (csrc/tzk_jrc.cuh)
+    def jrc_loss(self, logits: torch.Tensor, labels: torch.Tensor, session_ids: torch.Tensor,
+                 weights: Optional[torch.Tensor], alpha: float, key_bits: int = 64):
+        """logits [B, 2] fp32 (contiguous rows), labels [B] fp32, session_ids [B] int64 in [0, 2^key_bits), weights [B]
+        fp32 or None (mean reduction) -> (loss [scalar], d loss / d logits [B, 2])."""
+        logits, ld = _rows2d(logits, "logits")
+        _need(labels, torch.float32, "labels")
+        _need(session_ids, torch.int64, "session_ids")
+        if weights is not None:
+            _need(weights, torch.float32, "weights")
+        B = logits.shape[0]
+        if logits.shape[1] != 2 or labels.numel() != B or session_ids.numel() != B or (
+                weights is not None and weights.numel() != B):
+            raise TzkError("jrc_loss: need logits [B, 2] and B labels, session ids (and weights)")
+        dev = logits.device
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        dlogits = torch.empty((B, 2), dtype=torch.float32, device=dev)
+        ws = self._workspace("jrc", self._lib.tzk_jrc_loss_workspace_bytes(B), dev)
+        check(self._lib.tzk_jrc_loss(_ptr(logits), ld, _ptr(labels), _ptr(session_ids), _ptr(weights), B, float(alpha),
+                                     int(key_bits), _ptr(loss), _ptr(dlogits), _ptr(ws), ws.numel(), _stream()),
+              "tzk_jrc_loss")
+        self.launches += 6 if B > 0 else 1            # iota, pass 1-3 and two carries; B = 0: one carry (CUB's sort not counted)
+        return loss, dlogits
+
 
 @dataclass
 class ColPlan:

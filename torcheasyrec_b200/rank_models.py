@@ -212,6 +212,19 @@ class DINEncoder(nn.Module):
         return torch.matmul(scores, sequence).squeeze(1)
 
 
+def _create_seq_encoder(seq_encoder_config: Message, group_total_dim: Dict[str, int]) -> nn.Module:
+    """tzrec/modules/sequence.py:370-394 for the encoder kinds built here (din_encoder): the encoder of a DEEP group's
+    sequence group, with query_dim / sequence_dim from `<input>.query` / `<input>.sequence`."""
+    kind = seq_encoder_config.WhichOneof("seq_module")
+    if kind != "din_encoder":
+        raise NotImplementedError(f"sequence encoder {kind} is outside the hot-path scope (din_encoder only)")
+    cfg = seq_encoder_config.din_encoder
+    kw = config_to_kwargs(cfg)
+    kw.pop("name", None)
+    return DINEncoder(sequence_dim=group_total_dim[f"{cfg.input}.sequence"],
+                      query_dim=group_total_dim[f"{cfg.input}.query"], **kw)
+
+
 # --------------------------------------------------------------------------------------------------------
 # models
 # --------------------------------------------------------------------------------------------------------
@@ -245,7 +258,13 @@ class RankModel(nn.Module):
             kw = dict(wide_embedding_dim=self._model_config.wide_embedding_dim or None,
                       wide_init_fn=self._model_config.wide_init_fn if self._model_config.HasField("wide_init_fn") else None)
         self.embedding_group = EmbeddingGroup(self._features, list(self._base_model_config.feature_groups),
-                                              device=self._device, **kw)
+                                              device=self._device, seq_encoder_factory=_create_seq_encoder, **kw)
+        # DIN encoders of DEEP groups read their sequence rows jagged, as MultiTowerDIN's attention towers do
+        # (TZK_DIN_JAGGED=0 keeps the padded [B, T, D] form)
+        din_inputs = [enc.din_encoder.input for fg in self._base_model_config.feature_groups
+                      for enc in fg.sequence_encoders if enc.WhichOneof("seq_module") == "din_encoder"]
+        if din_inputs and os.environ.get("TZK_DIN_JAGGED", "1") != "0":
+            self.embedding_group.set_jagged_for_attention(din_inputs)
 
     def build_input(self, batch: Batch) -> Dict[str, torch.Tensor]:
         """rank_model.py:114-131."""
@@ -559,34 +578,93 @@ class MultiTaskRank(RankModel):
     multi_task_rank.py:97-142 does.  What the reference honours per tower and this repo does not (sample weights,
     non-BCE losses) is refused at construction instead of silently training with plain mean BCE."""
 
+    # losses a task tower may use: BCE-with-logits on a one-logit head, or the JRC loss on a two-class head (only the
+    # models whose reference towers accept it list jrc_loss)
+    _TOWER_LOSSES = ("binary_cross_entropy",)
+
     def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
         super().__init__(model_config, features, labels, sample_weights, **kwargs)
         self._task_tower_cfgs = list(self._model_config.task_towers)
+        self._jrc = {}                      # tower name -> its jrc_loss config
         for cfg in self._task_tower_cfgs:
             fld = "sample_weight_name"
             if cfg._spec(fld) is not None and cfg.HasField(fld) and getattr(cfg, fld):
                 raise NotImplementedError(f"task tower {cfg.tower_name}: {fld} is outside the hot-path scope")
             for lc in (cfg.losses if cfg._spec("losses") is not None else []):
-                if lc.WhichOneof("loss") not in (None, "binary_cross_entropy"):
-                    raise NotImplementedError(f"task tower {cfg.tower_name}: loss {lc.WhichOneof('loss')} is outside "
-                                              "the hot-path scope (BCE-with-logits only)")
+                kind = lc.WhichOneof("loss")
+                if kind not in (None,) + self._TOWER_LOSSES:
+                    raise NotImplementedError(f"task tower {cfg.tower_name}: loss {kind} is outside the hot-path "
+                                              f"scope ({', '.join(self._TOWER_LOSSES)} only)")
+                if kind == "jrc_loss":
+                    assert cfg.num_class == 2, f"num_class must be 2 when loss type is {kind}"
+                    self._jrc[cfg.tower_name] = lc.jrc_loss
 
     def _multi_task_output_to_prediction(self, tower_outputs: List[torch.Tensor]) -> Dict[str, torch.Tensor]:
-        """multi_task_rank.py:50-65: tower i's output under the suffix `_<tower_name>`."""
+        """multi_task_rank.py:50-65: tower i's output under the suffix `_<tower_name>`; a JRC tower's two-class head as
+        rank_model.py:156-161: logits [B, 2], probs = softmax, probs1 = probs[:, 1]."""
         preds = {}
         for cfg, out in zip(self._task_tower_cfgs, tower_outputs):
-            preds.update(self._output_to_prediction(out, suffix=f"_{cfg.tower_name}"))
+            s = f"_{cfg.tower_name}"
+            if cfg.tower_name in self._jrc:
+                probs = torch.softmax(out, dim=1)
+                preds.update({"logits" + s: out, "probs" + s: probs, "probs1" + s: probs[:, 1]})
+            else:
+                preds.update(self._output_to_prediction(out, suffix=s))
         return preds
 
     def _metric_heads(self):
         """multi_task_rank.py:144-196: per task tower, its metrics and losses on its label, suffixed `_<tower_name>`."""
         return [(list(c.metrics), list(c.losses), c.label_name, f"_{c.tower_name}") for c in self._task_tower_cfgs]
 
+    def update_metric(self, predictions, batch, losses=None) -> None:
+        """A JRC tower's auc reads probs1_<tower> (rank_model.py:289-330)."""
+        if self._jrc:
+            predictions = dict(predictions)
+            for name in self._jrc:
+                predictions[f"probs_{name}"] = predictions[f"probs1_{name}"]
+        super().update_metric(predictions, batch, losses)
+
+    def _session_ids(self, batch: Batch, name: str) -> torch.Tensor:
+        """The first id of feature `name` in the base data group per sample, 0 for an empty row (rank_model.py:247-249
+        `to_padded_dense(1)[:, 0]`), by device work only."""
+        from .features import BASE_DATA_GROUP
+
+        kjt = batch.sparse_features[BASE_DATA_GROUP]
+        f, B = kjt.keys().index(name), kjt.stride()
+        vals = kjt.values()
+        if vals.numel() == 0:
+            return torch.zeros(B, dtype=torch.int64, device=vals.device)
+        start = kjt.offsets()[f * B:(f + 1) * B].to(torch.int64).clamp(max=vals.numel() - 1)
+        lens = kjt.lengths()[f * B:(f + 1) * B]
+        return torch.where(lens > 0, vals[start].to(torch.int64), torch.zeros_like(start))
+
+    def _jrc_loss(self, cfg, predictions, batch) -> torch.Tensor:
+        """rank_model.py:244-261 + multi_task_rank.py:97-142 for a JRC tower: the mean reduction, or, when the tower has
+        `weight` or `task_space_indicator_label` (multi_task_rank.py:67-78), mean(loss * w) with w =
+        div_no_nan(v, mean v) * weight."""
+        jc = self._jrc[cfg.tower_name]
+        label = batch.labels[cfg.label_name].to(torch.float32)
+        sid = self._session_ids(batch, jc.session_name)
+        alpha = proto_float32(jc.alpha)
+        logits = predictions[f"logits_{cfg.tower_name}"]
+        w = None
+        if cfg.HasField("weight") or _task_space_label(cfg):
+            w = torch.ones(1, device=label.device)
+            if _task_space_label(cfg):
+                in_space = (batch.labels[cfg.task_space_indicator_label] > 0).float()
+                w = w * (cfg.in_task_space_weight * in_space + cfg.out_task_space_weight * (1 - in_space))
+            w = torch.nan_to_num(torch.div(w, torch.mean(w)), nan=0.0, posinf=0.0, neginf=0.0) * cfg.weight
+        # the raw ids of the batch, not bounded by the table (the lookup clamps, the grouping must not): all 64 bits
+        return Fn.jrc_loss(logits, label, sid, alpha, w)
+
     def loss(self, predictions, batch):
         from .dense_gemm import bce_with_logits
 
         out = {}
         for cfg in self._task_tower_cfgs:
+            if cfg.tower_name in self._jrc:
+                out[f"jrc_loss_{cfg.tower_name}"] = self._jrc_loss(cfg, predictions, batch)
+                continue
             label = batch.labels[cfg.label_name].to(torch.float32)
             logits = predictions[f"logits_{cfg.tower_name}"]
             if _task_space_label(cfg):
@@ -1184,9 +1262,109 @@ class MaskNet(RankModel):
         return self._output_to_prediction(self.output_linear(hidden))
 
 
+class DBMTL(MultiTaskRank):
+    """tzrec/models/dbmtl.py:28-175: the first feature group through an optional MaskNetModule, bottom MLP and MMoE,
+    then per task tower its MLP, its relation MLP over [own net | relation towers' relation nets] in config order, and
+    `task_outputs.i` (num_class outputs).  Towers take BCE or, on two-class heads, the JRC loss."""
+
+    _TOWER_LOSSES = ("binary_cross_entropy", "jrc_loss")
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        if model_config.use_pareto_loss_weight:
+            raise NotImplementedError("use_pareto_loss_weight is outside the hot-path scope")
+        cfg = self._model_config
+        self.init_input()
+        self.group_name = self.embedding_group.group_names()[0]
+        feature_in = self.embedding_group.group_total_dim(self.group_name)
+        self.mask_net = None
+        if cfg.HasField("mask_net"):
+            self.mask_net = MaskNetModule(feature_in, **config_to_kwargs(cfg.mask_net))
+            feature_in = self.mask_net.output_dim()
+        self.bottom_mlp = None
+        if cfg.HasField("bottom_mlp"):
+            self.bottom_mlp = MLP(feature_in, **config_to_kwargs(cfg.bottom_mlp))
+            feature_in = self.bottom_mlp.output_dim()
+        self.mmoe = None
+        if cfg.HasField("expert_mlp"):
+            self.mmoe = MMoEModule(in_features=feature_in, expert_mlp=config_to_kwargs(cfg.expert_mlp),
+                                   num_expert=cfg.num_expert, num_task=len(self._task_tower_cfgs),
+                                   gate_mlp=config_to_kwargs(cfg.gate_mlp) if cfg.HasField("gate_mlp") else None)
+            feature_in = self.mmoe.output_dim()
+        self.task_mlps = nn.ModuleDict()
+        for tc in self._task_tower_cfgs:
+            if tc.HasField("mlp"):
+                self.task_mlps[tc.tower_name] = MLP(feature_in, **config_to_kwargs(tc.mlp))
+        self.relation_mlps = nn.ModuleDict()
+        for tc in self._task_tower_cfgs:
+            if tc.HasField("relation_mlp"):
+                name = tc.tower_name
+                dim = self.task_mlps[name].output_dim() if name in self.task_mlps else feature_in
+                for rel in tc.relation_tower_names:
+                    # dbmtl.py:98-108: a relation tower counts with its relation MLP, else its task MLP, else the
+                    # tower input (whatever that tower's own output width is)
+                    if rel in self.relation_mlps:
+                        dim += self.relation_mlps[rel].output_dim()
+                    elif rel in self.task_mlps:
+                        dim += self.task_mlps[rel].output_dim()
+                    else:
+                        dim += feature_in
+                self.relation_mlps[name] = MLP(dim, **config_to_kwargs(tc.relation_mlp))
+        self.task_outputs = nn.ModuleList()
+        for tc in self._task_tower_cfgs:
+            name = tc.tower_name
+            if name in self.relation_mlps:
+                dim = self.relation_mlps[name].output_dim()
+            elif name in self.task_mlps:
+                dim = self.task_mlps[name].output_dim()
+            else:
+                dim = feature_in
+            self.task_outputs.append(nn.Linear(dim, tc.num_class))
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        net = self.build_input(batch)[self.group_name]
+        if self.mask_net is not None:
+            net = self.mask_net(net)
+        if self.bottom_mlp is not None:
+            net = self.bottom_mlp(net)
+        task_inputs = self.mmoe(net) if self.mmoe is not None else [net] * len(self._task_tower_cfgs)
+        task_net = {}
+        for i, tc in enumerate(self._task_tower_cfgs):
+            name = tc.tower_name
+            task_net[name] = self.task_mlps[name](task_inputs[i]) if name in self.task_mlps else task_inputs[i]
+        relation_net = {}
+        for tc in self._task_tower_cfgs:
+            name = tc.tower_name
+            if tc.HasField("relation_mlp"):
+                x = torch.cat([task_net[name]] + [relation_net[r] for r in tc.relation_tower_names], dim=1)
+                relation_net[name] = self.relation_mlps[name](x)
+            else:
+                relation_net[name] = task_net[name]
+        return self._multi_task_output_to_prediction(
+            [self.task_outputs[i](relation_net[tc.tower_name]) for i, tc in enumerate(self._task_tower_cfgs)])
+
+
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
                  "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE,
-                 "pepnet": PEPNet}
+                 "pepnet": PEPNet, "dbmtl": DBMTL}
+
+
+class JRCLoss(nn.Module):
+    """tzrec/loss/jrc_loss.py:29-117: forward(logits [B, 2], labels [B], session_ids [B]) -> the [B] per-sample losses
+    (reduction "none") or their mean ("mean", NaN for a batch without a positive or a negative, as the reference).  The
+    mean runs tzk_jrc_loss on CUDA (functional.jrc_loss); "none" and CPU tensors take functional.torch_jrc_loss.  A
+    label outside {0, 1} gives NaN where the reference raises."""
+
+    def __init__(self, alpha: float = 0.5, reduction: str = "mean") -> None:
+        super().__init__()
+        if reduction not in ("mean", "none"):
+            raise ValueError(f"reduction must be mean or none, got {reduction}")
+        self._alpha, self._reduction = alpha, reduction
+
+    def forward(self, logits: torch.Tensor, labels: torch.Tensor, session_ids: torch.Tensor) -> torch.Tensor:
+        if self._reduction == "none":
+            return Fn.torch_jrc_loss(logits, labels, session_ids, self._alpha, "none")
+        return Fn.jrc_loss(logits, labels, session_ids, self._alpha)
 
 
 def create_model(model_config: Message, features: List[BaseFeature], labels: List[str], device=None) -> RankModel:
