@@ -143,7 +143,8 @@ fm_bwd_kernel(const float* __restrict__ x, int64_t ld_x, const float* __restrict
 //    step costs 2 LDS.128 per 16 FMAs; the (bi,bj) decode is a per-CTA lookup table, not per-sample maths;
 //  * results are staged in shared memory and the whole output row [P | D | Ns*D] leaves with coalesced stores.
 // ---------------------------------------------------------------------------------------------------
-constexpr int kIWarps = 8;  // warps (= samples in flight) per CTA
+constexpr int kIWarps = 8;  // most warps (= samples in flight) per CTA; the kernels read the count from blockDim.x
+constexpr size_t kIMaxSmem = 227 * 1024;  // largest dynamic shared memory one CTA may opt into (sm_90)
 
 __device__ __forceinline__ int tri_index(int i, int j, int N) {  // i < j
   return i * N - (i * (i + 1)) / 2 + (j - i - 1);
@@ -203,7 +204,7 @@ dot_interact_fwd_kernel(const float* __restrict__ dense, int64_t ld_dense, const
   const int DS = D + 4;               // row stride
   const int P = N * (N - 1) / 2;
   const int Pp = (P + 3 + 4) & ~3;    // room for p_pad zeros; keeps every warp's slab 16-B aligned
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
   const int nb = Np / 4;
   const int n_blocks = nb * (nb + 1) / 2;
   const int D4 = D / 4;  // D % 4 == 0 enforced by the host wrapper
@@ -247,7 +248,7 @@ dot_interact_fwd_kernel(const float* __restrict__ dense, int64_t ld_dense, const
     }
   }
 
-  for (int64_t b = (int64_t)blockIdx.x * kIWarps + warp; b < B; b += (int64_t)gridDim.x * kIWarps) {
+  for (int64_t b = (int64_t)blockIdx.x * n_warps + warp; b < B; b += (int64_t)gridDim.x * n_warps) {
     stage_x(X, dense, ld_dense, sparse, ld_sparse, b, Ns, N, Np, D4, DS, swm, lane);
     __syncwarp();
     // ---- Gram blocks ------------------------------------------------------------------------------
@@ -391,7 +392,7 @@ dot_interact_bwd_kernel(const float* __restrict__ dense, int64_t ld_dense, const
   const int DS = D + 4;
   const int SS = Np + 8;  // stride of the symmetric grad matrix: the transposed scatter is 4-way, not 32-way
   const int P = N * (N - 1) / 2;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
   const int D4 = D / 4;
   const int swm = swz_mask(D4);
   const int nb = Np / 4;
@@ -413,7 +414,7 @@ dot_interact_bwd_kernel(const float* __restrict__ dense, int64_t ld_dense, const
   for (int i = lane; i < Np * SS; i += 32) S[i] = 0.f;  // diagonal + padding stay zero for the whole kernel
   __syncthreads();
 
-  for (int64_t b = (int64_t)blockIdx.x * kIWarps + warp; b < B; b += (int64_t)gridDim.x * kIWarps) {
+  for (int64_t b = (int64_t)blockIdx.x * n_warps + warp; b < B; b += (int64_t)gridDim.x * n_warps) {
     stage_x(X, dense, ld_dense, sparse, ld_sparse, b, Ns, N, Np, D4, DS, swm, lane);
     const float* go = d_out + b * ld_dout;
     for (int idx0 = lane; idx0 < P; idx0 += 32 * 6) {  // coalesced read of d_out (6 loads in flight), symmetric scatter
@@ -522,6 +523,17 @@ inline int grid_for(int64_t n, int per_block, int max_blocks) {
   if (g < 1) g = 1;
   return (int)(g < max_blocks ? g : max_blocks);
 }
+
+// Warps per CTA of the FFMA interaction kernels: the largest of kIWarps, kIWarps/2, ..., 1 whose shared memory (a
+// CTA-wide table of `table` floats plus one slab of `slab` floats per warp) fits kIMaxSmem, with its size in *smem;
+// 0 when not even one warp fits.  Wide features (e.g. 64 x 64 in the backward) do not fit 8 slabs.
+inline int interact_warps(size_t table, size_t slab, size_t* smem) {
+  for (int w = kIWarps; w >= 1; w >>= 1) {
+    *smem = (table + (size_t)w * slab) * sizeof(float);
+    if (*smem <= kIMaxSmem) return w;
+  }
+  return 0;
+}
 }  // namespace
 
 extern "C" int tzk_col_gather_sum(const float* const* srcs_host, const int64_t* src_ld_host, int32_t n_src,
@@ -620,13 +632,19 @@ extern "C" int tzk_dot_interact_fwd(const float* dense, int64_t ld_dense, const 
   }
   const int aligned = (((P + p_pad) % 4) == 0) && (ld_out % 4 == 0) && ((uintptr_t)out % 16 == 0);
   const int nb = Np / 4, n_blocks = nb * (nb + 1) / 2;
-  size_t smem = ((size_t)((n_blocks + 7) / 8) * 4 + (size_t)kIWarps * (Np * (D + 4) + ((P + 3 + 4) & ~3))) * sizeof(float);
+  size_t smem = 0;
+  const int warps = interact_warps((size_t)((n_blocks + 7) / 8) * 4, (size_t)Np * (D + 4) + ((P + 3 + 4) & ~3), &smem);
+  TZK_REQUIRE(warps > 0, "dot_interact_fwd: N=%d, D=%d needs %zu B of shared memory with one warp, more than %zu", N, D,
+              smem, kIMaxSmem);
 #define TZK_IFWD3(DT_, ONE_, NT_)                                                                              \
   do {                                                                                                       \
-    if (smem > 48 * 1024)                                                                                    \
-      cudaFuncSetAttribute(dot_interact_fwd_kernel<DT_, ONE_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                           (int)smem);                                                                       \
-    dot_interact_fwd_kernel<DT_, ONE_, NT_><<<grid_for(B, kIWarps, kSmCountH100 * 8), kIWarps * 32, smem,     \
+    if (smem > 48 * 1024 &&                                                                                  \
+        cudaFuncSetAttribute(dot_interact_fwd_kernel<DT_, ONE_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                             (int)smem) != cudaSuccess) {                                                    \
+      TZK_REQUIRE(false, "dot_interact_fwd: %zu B of shared memory refused: %s", smem,                       \
+                  cudaGetErrorString(cudaGetLastError()));                                                   \
+    }                                                                                                        \
+    dot_interact_fwd_kernel<DT_, ONE_, NT_><<<grid_for(B, warps, kSmCountH100 * 8), warps * 32, smem,         \
                                               as_stream(stream)>>>(                                          \
         dense, ld_dense, sparse, ld_sparse, B, Ns, D, copy_dense, copy_sparse, p_pad, aligned, out, ld_out); \
   } while (0)
@@ -678,13 +696,19 @@ extern "C" int tzk_dot_interact_bwd(const float* dense, int64_t ld_dense, const 
     return 0;
   }
   const int aligned = (((P + p_pad) % 4) == 0) && (ld_dout % 4 == 0) && ((uintptr_t)d_out % 16 == 0);
-  size_t smem = ((size_t)((P + 7) / 8) * 4 + (size_t)kIWarps * (Np * (D + 4) + Np * (Np + 8))) * sizeof(float);
+  size_t smem = 0;
+  const int warps = interact_warps((size_t)((P + 7) / 8) * 4, (size_t)Np * (D + 4) + (size_t)Np * (Np + 8), &smem);
+  TZK_REQUIRE(warps > 0, "dot_interact_bwd: N=%d, D=%d needs %zu B of shared memory with one warp, more than %zu", N, D,
+              smem, kIMaxSmem);
 #define TZK_IBWD(DT_, NT_)                                                                                    \
   do {                                                                                                       \
-    if (smem > 48 * 1024)                                                                                    \
-      cudaFuncSetAttribute(dot_interact_bwd_kernel<DT_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                           (int)smem);                                                                       \
-    dot_interact_bwd_kernel<DT_, NT_><<<grid_for(B, kIWarps, kSmCountH100 * 8), kIWarps * 32, smem,           \
+    if (smem > 48 * 1024 &&                                                                                  \
+        cudaFuncSetAttribute(dot_interact_bwd_kernel<DT_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                             (int)smem) != cudaSuccess) {                                                    \
+      TZK_REQUIRE(false, "dot_interact_bwd: %zu B of shared memory refused: %s", smem,                       \
+                  cudaGetErrorString(cudaGetLastError()));                                                   \
+    }                                                                                                        \
+    dot_interact_bwd_kernel<DT_, NT_><<<grid_for(B, warps, kSmCountH100 * 8), warps * 32, smem,               \
                                         as_stream(stream)>>>(                                                \
         dense, ld_dense, sparse, ld_sparse, d_out, ld_dout, B, Ns, D, copy_dense, copy_sparse, p_pad, aligned, \
         d_dense, ld_ddense, d_sparse, ld_dsparse);                                                           \

@@ -263,14 +263,35 @@ def _torch_dot_interaction(features: torch.Tensor) -> torch.Tensor:
     return z[:, iu[0], iu[1]]
 
 
+def _interact_rows_ok(t: torch.Tensor) -> bool:
+    return (t.dtype == torch.float32 and t.dim() == 2 and (t.shape[1] <= 1 or t.stride(1) == 1)
+            and (t.shape[0] <= 1 or t.stride(0) % 4 == 0) and t.data_ptr() % 16 == 0)
+
+
+def dot_interact_usable(dense: Optional[torch.Tensor], sparse: torch.Tensor, Ns: int, D: int) -> bool:
+    """True when the dot-interaction kernels (csrc/tzk_dense.cu) cover this call: fp32 [B, Ns*D] sparse and [B, D]
+    dense (or None) with autocast off, 4 <= D <= 128 and D % 4 == 0, at most 64 features in all, every row contiguous
+    and starting on a 16-B boundary, on a device the compute backend runs (CUDA; on the CPU only a test backend that
+    implements the interaction kernels)."""
+    if autocast_dtype(sparse) is not None or not (4 <= D <= 128 and D % 4 == 0) or Ns < 1:
+        return False
+    if Ns + (dense is not None) > 64 or not _interact_rows_ok(sparse) or sparse.shape[1] != Ns * D:
+        return False
+    if dense is not None and not (_interact_rows_ok(dense) and dense.shape[1] == D):
+        return False
+    return sparse.is_cuda or (_backend is not None and hasattr(_backend, "dot_interact_fwd"))
+
+
 def dot_interaction(features: torch.Tensor) -> torch.Tensor:
     """InteractionArch.forward (tzrec/modules/interaction.py:80-91): [B,N,D] -> [B, N(N-1)/2].
 
-    Under autocast this is the reference's torch formulation: bmm is on autocast's lower-precision list."""
-    if autocast_dtype(features) is not None:
-        return _torch_dot_interaction(features)
+    Under autocast, and for shapes outside dot_interact_usable, this is the reference's torch formulation (bmm is on
+    autocast's lower-precision list)."""
     B, N, D = features.shape
-    return _DotInteract.apply(None, features.reshape(B, N * D), N, D, False, False)
+    x = _rows_contig(features.reshape(B, N * D))
+    if not dot_interact_usable(None, x, N, D):
+        return _torch_dot_interaction(features)
+    return _DotInteract.apply(None, x, N, D, False, False)
 
 
 def dlrm_interaction(dense_feat: Optional[torch.Tensor], sparse_feat: torch.Tensor, num_sparse: int, dim: int,
@@ -283,10 +304,14 @@ def dlrm_interaction(dense_feat: Optional[torch.Tensor], sparse_feat: torch.Tens
     that every block and every row starts on a 16-B boundary; `in_map` = [(src_col, dst_col, length), ...] tells the
     consuming Linear where the reference's columns live (dense_gemm.linear pads its weight accordingly).
 
-    Under autocast this is the reference's torch formulation in the reference's layout (with aligned=True the map is
-    None): autocast rounds the bmm to its dtype and the concatenations promote back to fp32, as in dlrm.py.  DLRM-Criteo
-    under bf16 autocast has its own kernel (dense_gemm.InteractBf16Fn)."""
-    if autocast_dtype(sparse_feat) is not None:
+    Under autocast, and for shapes outside dot_interact_usable (e.g. an embedding dim that is not a multiple of 4), this
+    is the reference's torch formulation in the reference's layout (with aligned=True the map is None): autocast rounds
+    the bmm to its dtype and the concatenations promote back to fp32, as in dlrm.py.  DLRM-Criteo under bf16 autocast has
+    its own kernel (dense_gemm.InteractBf16Fn)."""
+    if dense_feat is not None:
+        dense_feat = _rows_contig(dense_feat)
+    sparse_feat = _rows_contig(sparse_feat)
+    if not dot_interact_usable(dense_feat, sparse_feat, num_sparse, dim):
         B = sparse_feat.shape[0]
         feat = sparse_feat.reshape(-1, num_sparse, dim)
         if dense_feat is not None:
