@@ -6,11 +6,12 @@
 //                            work items)
 //
 // The GEMM parts compute what tzk_gemm3x.cu computes (TMA SWIZZLE_128B boxes through mbarrier-guarded stages, the 3xTF32
-// split, every k-step's three products in a fresh accumulator, added in round-to-nearest in k order).  The forward and
-// the weight gradient issue each k-step as m64n64k8 warpgroup MMAs (tzk_wgmma.cuh) with B straight from shared memory:
-// one wgmma k8 gives the bits of the mma.sync m16n8k8 it replaces (tests/test_wgmma_bits_gpu.py).  The input gradient
-// stays on mma.sync.  The per-sample interaction is tzk_interact_tc.cuh's.  The same source runs on the CPU under
-// tests/native/cuda_cpu_shim.h, sm90_cpu_emu.h and sm90_wgmma_emu.h (tests/test_interact_wide_fused.py,
+// split, every k-step's three products in a fresh accumulator, added in round-to-nearest in k order).  All three issue
+// each k-step as warpgroup MMAs (tzk_wgmma.cuh) with B straight from shared memory, m64n64k8 in the forward and the
+// weight gradient, m64n32k8 in the input gradient: one wgmma k8 gives the bits of the mma.sync m16n8k8 it replaces
+// (tests/test_wgmma_bits_gpu.py, tests/test_wgmma_n32_bits_gpu.py).  The per-sample interaction is
+// tzk_interact_tc.cuh's.  The same source runs on the CPU under tests/native/cuda_cpu_shim.h, sm90_cpu_emu.h and
+// sm90_wgmma_emu.h (tests/test_interact_wide_fused.py, tests/test_interact_wide_bwd_ring.py,
 // tests/test_interact_wide_fwd_fused.py).
 #include <stdint.h>
 #include <stdio.h>
@@ -21,6 +22,8 @@
 #include "sm90_cpu_emu.h"
 #include "sm90_wgmma_emu.h"
 typedef void* tzk_stream_t;
+// sm90_cpu_emu.h's arrive: expect_tx with no bytes is a plain arrival
+inline void mbar_arrive(uint64_t* bar) { mbar_expect_tx(bar, 0); }
 #define TZK_REQUIRE(cond, ...) do { if (!(cond)) return 1; } while (0)
 #define TZK_CHECK_LAUNCH(name) do {} while (0)
 #else
@@ -54,32 +57,63 @@ __device__ __forceinline__ float4 load_l2(const float* p) {
 
 // ======================================================================================================================
 // Input gradient of the wide layer fused with the backward of the DLRM interaction that produced its input (DLRM-Criteo:
-// X = [351 pairs | 0 | dense 16 | sparse 416], 784 columns).  Per CTA of FB_M samples:
-//   1. dX[FB_M x 784] = dZ W, in chunks of 32 columns: dZ's fragments are split once and stay in registers (K = 64), W^T
-//      hi / lo chunks arrive by TMA through the stage ring; mma.sync m16n8k8 (m64n8k8 wgmma per warpgroup was slower,
-//      DESIGN §8).  The pass-through columns (352 ..) are stored straight into d_dense / d_sparse; the pair columns
-//      (0 .. 351) go to a shared-memory tile.  They run second so that the tile is complete when the ring drains.
-//   2. per sample, one warp: S from the pair columns, dE = S E + pass-through (tzk_itc::bwd_sample), the pass-through
-//      read back from d_dense / d_sparse (written by this CTA in step 1, so an L2 hit).
-// dX never reaches global memory.  The MMA order and the per-k-step accumulation are gemm3x_kernel's, so dX and with it
-// dE are bit for bit what gemm3x_kernel (dgrad) followed by dot_interact27_bwd_tc_kernel computes.
-constexpr int FB_M = 64;                      // samples per CTA
-constexpr int FB_THREADS = 512;               // 16 warps: 4 along the samples x 4 along a 32-column chunk
+// X = [351 pairs | 0 | dense 16 | sparse 416], 784 columns).  Persistent: min(tiles, SMs) CTAs of four warpgroups, CTA
+// b takes the 64-sample tiles b, b + gridDim.x, ..  Per tile:
+//   1. dZ [64 x 64] arrives by TMA and every warpgroup reads all of it into its A fragments in registers (K = 64).
+//   2. dX [64 x 784] = dZ W in 25 chunks of 32 columns, chunk c on warpgroup (26 t + 1 + c) % 4 (t: the CTA's tile
+//      count), each k-step as three m64n32k8 wgmma with A = dZ split into hi / lo and B = the W^T hi / lo SWIZZLE_128B
+//      boxes.  The pass-through columns (352 ..) are stored straight into d_dense / d_sparse; the pair columns
+//      (0 .. 351) go to a shared-memory tile P.
+//   3. per sample, one warp: S from the pair columns, dE = S E + pass-through (tzk_itc::bwd_sample), the pass-through
+//      read back from d_dense / d_sparse (written by this CTA in step 2, so an L2 hit).
+// Steps 1 and 2 read a ring of FB_STAGES stages that carries, per tile, the dZ tile and then the 25 W^T chunks, 26
+// items in all, item i in stage i % FB_STAGES: the ring runs on into the CTA's next tile, so that tile's dZ and first
+// chunks load while this tile's step 3 runs.  A stage is two halves (k 0 .. 31, k 32 .. 63), each with a full barrier
+// (the TMA's bytes) and an empty barrier (four arrivals, one per warp of the reader).  Chunk item i is read by
+// warpgroup i % 4 = stage i % 4: each of its warps arrives on a half's empty barrier once its wgmma on that half are
+// complete, and the warpgroup's first thread, when all four have, refills the half with item i + FB_STAGES, so the
+// next chunk's first half loads while this chunk's second half is computed.  The dZ item is read by the whole CTA:
+// warps 0 .. 3 arrive for it after the barrier that follows the split, and thread 0 refills it.  The only CTA-wide
+// barriers are two per tile: P complete before step 3, and P read (and dZ split) before the next step 2.
+// dX never reaches global memory.  The products and the per-k-step accumulation are gemm3x_kernel's (one k8 wgmma
+// gives the bits of the mma.sync m16n8k8 it replaces), so dX and with it dE are bit for bit what gemm3x_kernel (dgrad)
+// followed by dot_interact27_bwd_tc_kernel computes.
+constexpr int FB_M = 64;                      // samples per tile
+constexpr int FB_THREADS = 512;               // 4 warpgroups
 constexpr int FB_WARPS = FB_THREADS / 32;
 constexpr int FB_CHUNKS = (tzk_itc::kRow + 31) / 32;   // 25: the last one reads W^T rows 784 .. 799 as zeros
 constexpr int FB_PAIR_CHUNKS = tzk_itc::kInter / 32;   // 11: columns 0 .. 351
+constexpr int FB_ITEMS = 1 + FB_CHUNKS;       // ring items per tile: dZ, then the chunks
 constexpr int FB_BOX = 32 * 128;              // one W^T box: 32 dX columns x 32 k = 4 KB
-constexpr int FB_STAGE = 4 * FB_BOX;          // hi k 0..31 | hi k 32..63 | lo k 0..31 | lo k 32..63
-constexpr int FB_STAGES = 3;
+constexpr int FB_HALF = 2 * FB_BOX;           // half a stage, k 0..31 or 32..63: W^T hi | lo, or dZ; a barrier each
+constexpr int FB_STAGE = 2 * FB_HALF;
+constexpr int FB_STAGES = 4;
 constexpr int FB_LDP = 360;                   // row stride of the pair tile: 8 mod 32 words -> conflict-free float2 stores
 constexpr int FB_P_OFF = FB_STAGES * FB_STAGE;
 constexpr int FB_S_OFF = FB_P_OFF + FB_M * FB_LDP * 4;
 constexpr int FB_IJ_OFF = FB_S_OFF + FB_WARPS * 32 * tzk_itc::kSS * 4;
 constexpr int FB_BAR_OFF = FB_IJ_OFF + tzk_itc::kInter * 2;
-constexpr int FB_SMEM = FB_BAR_OFF + FB_STAGES * 8;    // 215 768 B: one CTA per SM
+constexpr int FB_SMEM = FB_BAR_OFF + 4 * FB_STAGES * 8;    // 232 256 B: one CTA per SM
+static_assert(FB_HALF == FB_M * 128, "a dZ box [64 x 32 floats] fills half a stage");
+static_assert(FB_STAGES == 4, "stage i % 4 is read by warpgroup i % 4");
+static_assert(FB_SMEM <= 227 * 1024, "over the opt-in shared memory of one CTA");
+
+#ifdef TZK_FB_TIMING
+// scripts/phase_split_interact_wide.py builds with this on: %globaltimer at four points of every tile, [tile][4]
+__device__ unsigned long long* fb_timing;
+__device__ __forceinline__ unsigned long long fb_now() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define FB_STAMP(tile, slot) do { if (threadIdx.x == 0) fb_timing[4 * (tile) + (slot)] = fb_now(); } while (0)
+#define FB_STAMP_LAST(tile, slot) do { if ((threadIdx.x & 31) == 0) atomicMax(fb_timing + 4 * (tile) + (slot), fb_now()); } while (0)
+#else
+#define FB_STAMP(tile, slot) do {} while (0)
+#define FB_STAMP_LAST(tile, slot) do {} while (0)
+#endif
 
 struct FbParams {
-  const float* dz; int64_t ld_dz;
   const float* dense; int64_t ld_dense;
   const float* sparse; int64_t ld_sparse;
   float* d_dense; int64_t ld_ddense;
@@ -88,16 +122,21 @@ struct FbParams {
 };
 
 __global__ void __launch_bounds__(FB_THREADS, 1)
-interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
-                         FbParams p) {
+interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_constant__ CUtensorMap map_whi,
+                         const __grid_constant__ CUtensorMap map_wlo, FbParams p) {
   TZK_DYN_SMEM(uint8_t, smem);
   float* P = reinterpret_cast<float*>(smem + FB_P_OFF);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + FB_BAR_OFF);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + FB_BAR_OFF);   // [stage][half]
+  uint64_t* empty = full + 2 * FB_STAGES;                             // [stage][half]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int64_t m0 = (int64_t)blockIdx.x * FB_M;
+  const int wg = warp >> 2, r = (warp & 3) * 16 + g;   // warpgroup; this lane's A / D rows r and r + 8
+  const int64_t tiles = (p.M + FB_M - 1) / FB_M;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < FB_STAGES; ++s) mbar_init(full + s, 1);
+    for (int s = 0; s < 2 * FB_STAGES; ++s) {
+      mbar_init(full + s, 1);
+      mbar_init(empty + s, 4);
+    }
     fence_mbarrier_init();
   }
   float* S = reinterpret_cast<float*>(smem + FB_S_OFF) + warp * (32 * tzk_itc::kSS);
@@ -105,92 +144,135 @@ interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_whi, const __gr
   tzk_itc::init_pair_ij(pair_ij);
   for (int i = lane; i < 32 * tzk_itc::kSS; i += 32) S[i] = 0.f;   // diagonal and padding stay zero
   __syncthreads();
-  // chunk c covers dX columns 32 col_chunk(c) ..: the pass-through chunks first, then the pair chunks
-  auto col_chunk = [](int c) { return (c + FB_PAIR_CHUNKS) % FB_CHUNKS; };
-  auto load = [&](int c) {                        // thread 0 only
-    uint8_t* sb = smem + (c % FB_STAGES) * FB_STAGE;
-    uint64_t* bar = full + c % FB_STAGES;
-    const int n0 = col_chunk(c) * 32;
-    mbar_expect_tx(bar, FB_STAGE);
-    tma_load_2d(sb, &map_whi, bar, 0, n0);
-    tma_load_2d(sb + FB_BOX, &map_whi, bar, 32, n0);
-    tma_load_2d(sb + 2 * FB_BOX, &map_wlo, bar, 0, n0);
-    tma_load_2d(sb + 3 * FB_BOX, &map_wlo, bar, 32, n0);
+  // half h (k 32 h ..) of an item, once the half's previous item is released; items past the CTA's last tile are not
+  // loaded.  One thread.
+  auto load = [&](int64_t item, int h) {
+    const int64_t tile = blockIdx.x + item / FB_ITEMS * gridDim.x;
+    if (tile >= tiles) return;
+    if (item >= FB_STAGES) mbar_wait(empty + 2 * (item % FB_STAGES) + h, (uint32_t)(item / FB_STAGES - 1) & 1u);
+    const int j = (int)(item % FB_ITEMS);
+    uint8_t* hb = smem + (item % FB_STAGES) * FB_STAGE + h * FB_HALF;
+    uint64_t* bar = full + 2 * (item % FB_STAGES) + h;
+    mbar_expect_tx(bar, FB_HALF);
+    if (j == 0) {
+      tma_load_2d(hb, &map_dz, bar, 32 * h, (int)(tile * FB_M));
+    } else {
+      tma_load_2d(hb, &map_whi, bar, 32 * h, (j - 1) * 32);
+      tma_load_2d(hb + FB_BOX, &map_wlo, bar, 32 * h, (j - 1) * 32);
+    }
   };
   if (threadIdx.x == 0)
-    for (int c = 0; c < FB_STAGES; ++c) load(c);
+    for (int i = 0; i < FB_STAGES; ++i) {
+      load(i, 0);
+      load(i, 1);
+    }
 
-  // A = dZ rows r, r + 8 of this warp's 16, all 64 columns, split once (rows past M are zeros)
-  const int wm = warp & 3, wn = warp >> 2;
-  const int r = wm * 16 + g;
-  uint32_t ah[8][4], al[8][4];
+  int64_t item0 = 0;                              // the tile's dZ item
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x, item0 += FB_ITEMS) {
+    const int64_t m0 = tile * FB_M;
+    FB_STAMP(tile, 0);
+    // 1. A = dZ rows r, r + 8, all 64 columns (rows past M are zeros from the TMA), split per k-step in step 2: hi / lo
+    // of all of it would take 64 registers and leave too few for the accumulators
+    float a[8][4];
+    {
+      const int s = (int)(item0 % FB_STAGES);
+      mbar_wait(full + 2 * s, (uint32_t)(item0 / FB_STAGES) & 1u);
+      mbar_wait(full + 2 * s + 1, (uint32_t)(item0 / FB_STAGES) & 1u);
+      const float* zs = reinterpret_cast<const float*>(smem + s * FB_STAGE);
 #pragma unroll
-  for (int kk = 0; kk < 8; ++kk) {
-    const int k0 = kk * 8 + t, k1 = k0 + 4;
-    const int64_t ra = m0 + r, rb = ra + 8;
-    const float a[4] = {ra < p.M ? __ldg(p.dz + ra * p.ld_dz + k0) : 0.f, rb < p.M ? __ldg(p.dz + rb * p.ld_dz + k0) : 0.f,
-                        ra < p.M ? __ldg(p.dz + ra * p.ld_dz + k1) : 0.f, rb < p.M ? __ldg(p.dz + rb * p.ld_dz + k1) : 0.f};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      ah[kk][i] = tf32_bits(a[i]);
-      al[kk][i] = tf32_bits(a[i] - __uint_as_float(ah[kk][i]));
-    }
-  }
-  const int n = wn * 8 + g;                       // this lane's B column (W^T row) within the chunk
-  for (int c = 0; c < FB_CHUNKS; ++c) {
-    const int s = c % FB_STAGES;
-    mbar_wait(full + s, (uint32_t)(c / FB_STAGES) & 1u);
-    const uint32_t* whi = reinterpret_cast<const uint32_t*>(smem + s * FB_STAGE);
-    const uint32_t* wlo = whi + 2 * FB_BOX / 4;
-    float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      const uint32_t* bh_box = whi + (kk >> 2) * (FB_BOX / 4);
-      const uint32_t* bl_box = wlo + (kk >> 2) * (FB_BOX / 4);
-      const int k0 = (kk & 3) * 8 + t, k1 = k0 + 4;
-      const uint32_t bh[2] = {bh_box[swz(n, k0)], bh_box[swz(n, k1)]};
-      const uint32_t bl[2] = {bl_box[swz(n, k0)], bl_box[swz(n, k1)]};
-      float part[4] = {0.f, 0.f, 0.f, 0.f};
-      mma_tf32(part, al[kk], bh);                 // small terms first
-      mma_tf32(part, ah[kk], bl);
-      mma_tf32(part, ah[kk], bh);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) acc[q] += part[q];
-    }
-    // c0/c1: row r, columns col, col + 1; c2/c3: row r + 8
-    const int col = col_chunk(c) * 32 + wn * 8 + 2 * t;
-    if (col < tzk_itc::kInter) {
-      *reinterpret_cast<float2*>(P + r * FB_LDP + col) = make_float2(acc[0], acc[1]);
-      *reinterpret_cast<float2*>(P + (r + 8) * FB_LDP + col) = make_float2(acc[2], acc[3]);
-    } else if (col < tzk_itc::kRow) {
-      const int e = col - tzk_itc::kInter;        // column of [dense 16 | sparse 416]
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t row = m0 + r + 8 * h;
-        if (row >= p.M) continue;
-        float* dst = e < tzk_itc::kD ? p.d_dense + row * p.ld_ddense + e : p.d_sparse + row * p.ld_dsparse + (e - tzk_itc::kD);
-        *reinterpret_cast<float2*>(dst) = make_float2(acc[2 * h], acc[2 * h + 1]);
+      for (int kk = 0; kk < 8; ++kk) {
+        const float* box = zs + (kk >> 2) * (FB_HALF / 4);
+        const int k0 = (kk & 3) * 8 + t, k1 = k0 + 4;
+        a[kk][0] = box[swz(r, k0)];
+        a[kk][1] = box[swz(r + 8, k0)];
+        a[kk][2] = box[swz(r, k1)];
+        a[kk][3] = box[swz(r + 8, k1)];
       }
     }
-    __syncthreads();                              // every warp is done with stage s; at the end: P and the stores
-    if (threadIdx.x == 0 && c + FB_STAGES < FB_CHUNKS) load(c + FB_STAGES);
-  }
-
-  for (int i = warp; i < FB_M; i += FB_WARPS) {
-    const int64_t b = m0 + i;
-    if (b >= p.M) break;
-    float* dd = p.d_dense + b * p.ld_ddense;
-    float* ds = p.d_sparse + b * p.ld_dsparse;
-    float4 pass[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int row = g + 8 * q;
-      pass[q] = row == 0 ? load_l2(dd + 4 * t)
-              : row < tzk_itc::kN ? load_l2(ds + (row - 1) * tzk_itc::kD + 4 * t)
-              : make_float4(0.f, 0.f, 0.f, 0.f);
+    __syncthreads();                              // dZ read by every warp; the previous tile's P read
+    if (warp < 4 && lane == 0) {
+      mbar_arrive(empty + 2 * (item0 % FB_STAGES));
+      mbar_arrive(empty + 2 * (item0 % FB_STAGES) + 1);
     }
-    tzk_itc::bwd_sample(P + i * FB_LDP, p.dense + b * p.ld_dense, p.sparse + b * p.ld_sparse, pass, pair_ij, S, dd, ds,
-                        lane);
+    if (threadIdx.x == 0) {
+      load(item0 + FB_STAGES, 0);
+      load(item0 + FB_STAGES, 1);
+    }
+    FB_STAMP(tile, 1);
+
+    // 2. this warpgroup's chunks: items item0 + 1 + c with (item0 + 1 + c) % 4 == wg
+    for (int c = (int)((wg - item0 - 1) & 3); c < FB_CHUNKS; c += 4) {
+      const int64_t item = item0 + 1 + c;
+      float acc[16], part[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const int h = kk >> 2;
+        const uint8_t* whi = smem + wg * FB_STAGE + h * FB_HALF;   // stage wg, half h: W^T hi | lo
+        if ((kk & 3) == 0) mbar_wait(full + 2 * wg + h, (uint32_t)(item / FB_STAGES) & 1u);
+        uint32_t ah[4], al[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          ah[i] = tf32_bits(a[kk][i]);
+          al[i] = tf32_bits(a[kk][i] - __uint_as_float(ah[i]));
+        }
+        wgmma_fence();
+        wgmma_3xtf32<32>(part, ah, al, wgmma_desc(whi, kk & 3), wgmma_desc(whi + FB_BOX, kk & 3));
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          wgmma_reg_fence(part[i]);
+          acc[i] += part[i];
+        }
+        // this warp's wgmma are done with the half: its next chunk's half loads during the rest of this one
+        if ((kk & 3) == 3) {
+          __syncwarp();                           // every lane of the warp is past its wait
+          if (lane == 0) mbar_arrive(empty + 2 * wg + h);
+          if ((threadIdx.x & 127) == 0) load(item + FB_STAGES, h);
+        }
+      }
+      // acc[4 i + q]: row r + 8 (q / 2), column 32 c + 8 i + 2 t + q % 2
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int col = c * 32 + i * 8 + 2 * t;
+        if (col < tzk_itc::kInter) {
+          *reinterpret_cast<float2*>(P + r * FB_LDP + col) = make_float2(acc[4 * i], acc[4 * i + 1]);
+          *reinterpret_cast<float2*>(P + (r + 8) * FB_LDP + col) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        } else if (col < tzk_itc::kRow) {
+          const int e = col - tzk_itc::kInter;    // column of [dense 16 | sparse 416]
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int64_t row = m0 + r + 8 * h;
+            if (row >= p.M) continue;
+            float* dst = e < tzk_itc::kD ? p.d_dense + row * p.ld_ddense + e : p.d_sparse + row * p.ld_dsparse + (e - tzk_itc::kD);
+            *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          }
+        }
+      }
+    }
+    __syncthreads();                              // P and the pass-through stores complete
+    FB_STAMP(tile, 2);
+
+    // 3. warp w: samples m0 + w, m0 + w + 16, ..
+    for (int i = warp; i < FB_M; i += FB_WARPS) {
+      const int64_t b = m0 + i;
+      if (b >= p.M) break;
+      float* dd = p.d_dense + b * p.ld_ddense;
+      float* ds = p.d_sparse + b * p.ld_dsparse;
+      float4 pass[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int row = g + 8 * q;
+        pass[q] = row == 0 ? load_l2(dd + 4 * t)
+                : row < tzk_itc::kN ? load_l2(ds + (row - 1) * tzk_itc::kD + 4 * t)
+                : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      tzk_itc::bwd_sample(P + i * FB_LDP, p.dense + b * p.ld_dense, p.sparse + b * p.ld_sparse, pass, pair_ij, S, dd, ds,
+                          lane);
+    }
+    FB_STAMP_LAST(tile, 3);
   }
 }
 
@@ -499,6 +581,12 @@ __global__ void split_wt_kernel(const float* __restrict__ w, int64_t ld_w, int K
 
 }  // namespace
 
+#ifdef TZK_FB_TIMING
+extern "C" int tzk_interact_wide_bwd_timing(unsigned long long* buf) {
+  return cudaMemcpyToSymbol(fb_timing, &buf, sizeof(buf)) == cudaSuccess ? 0 : 1;
+}
+#endif
+
 extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_t ld_w, const float* dense,
                                      int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
                                      int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
@@ -510,13 +598,21 @@ extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float
   const void* ptrs[] = {dz, w, dense, sparse, d_dense, d_sparse, wt_hi, wt_lo};
   for (const void* q : ptrs)
     TZK_REQUIRE(q && reinterpret_cast<uintptr_t>(q) % 16 == 0, "interact_wide_bwd: NULL or not 16-B aligned pointer");
+  int dev = 0, sms = 0;
+  TZK_REQUIRE(cudaGetDevice(&dev) == cudaSuccess &&
+              cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0,
+              "interact_wide_bwd: no device");
+#ifdef TZK_CPU_SHIM
+  // tests/test_interact_wide_bwd_ring.py: a small emulated grid, so that a few tiles already wrap the ring across tiles
+  if (const char* e = getenv("TZK_EMU_SMS")) sms = atoi(e);
+#endif
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   TZK_LAUNCH((split_wt_kernel), (tzk_itc::kRow * 64 + 255) / 256, 256, 0, st, w, ld_w, tzk_itc::kRow, wt_hi, wt_lo);
-  CUtensorMap mh, ml;
-  TZK_REQUIRE(!make_map(&mh, wt_hi, tzk_itc::kRow, 64, 64, 32) && !make_map(&ml, wt_lo, tzk_itc::kRow, 64, 64, 32),
-              "interact_wide_bwd: tensor-map encoding failed");
+  CUtensorMap mz, mh, ml;
+  TZK_REQUIRE(!make_map(&mz, dz, M, 64, ld_dz, FB_M) && !make_map(&mh, wt_hi, tzk_itc::kRow, 64, 64, 32) &&
+              !make_map(&ml, wt_lo, tzk_itc::kRow, 64, 64, 32), "interact_wide_bwd: tensor-map encoding failed");
   FbParams p;
-  p.dz = dz; p.ld_dz = ld_dz; p.dense = dense; p.ld_dense = ld_dense; p.sparse = sparse; p.ld_sparse = ld_sparse;
+  p.dense = dense; p.ld_dense = ld_dense; p.sparse = sparse; p.ld_sparse = ld_sparse;
   p.d_dense = d_dense; p.ld_ddense = ld_ddense; p.d_sparse = d_sparse; p.ld_dsparse = ld_dsparse; p.M = M;
 #ifndef TZK_CPU_SHIM
   static bool configured = false;     // once: nothing but the launches happens inside a stream capture
@@ -525,7 +621,8 @@ extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float
     configured = true;
   }
 #endif
-  TZK_LAUNCH((interact_wide_bwd_kernel), (unsigned)((M + FB_M - 1) / FB_M), FB_THREADS, FB_SMEM, st, mh, ml, p);
+  const int64_t tiles = (M + FB_M - 1) / FB_M;
+  TZK_LAUNCH((interact_wide_bwd_kernel), (unsigned)(tiles < sms ? tiles : sms), FB_THREADS, FB_SMEM, st, mz, mh, ml, p);
   TZK_CHECK_LAUNCH("interact_wide_bwd_kernel");
   return 0;
 }
