@@ -711,6 +711,54 @@ int tzk_jrc_loss(const float* logits, int64_t ld, const float* labels, const int
                  const float* weights, int64_t B, float alpha, int32_t key_bits, float* loss, float* dlogits,
                  void* workspace, size_t workspace_bytes, tzk_stream_t stream);
 
+/* ---- RocketLaunching's booster / light head (tzrec/models/rocket_launching.py: the output Linears, the softmax,
+ * the softmax cross-entropy of each head, the hint MSE and the feature-based similarity losses), forward and backward.
+ * head[0] is the light head, head[1] the booster head (has_booster = 0: light only).  Head e: hidden h [B, H] (rows
+ * contiguous), weight w [C, H], bias b [C]; 2 <= C <= 8, 4 <= H <= 1024 with H % 4 == 0.  labels [B] fp32 class
+ * indices and losses, or both NULL (no losses: logits and probs only; pairs need labels).  Pair k: light [B, d] and booster [B, d] hidden layers.
+ *   head_fwd: logits / probs [B, C] of every head; with labels, losses[3 + n_pairs] =
+ *             [0] CE_light, [1] CE_booster, [2] hint = mean (logits_light - logits_booster)^2 over B C,
+ *             [3 + k] sim_k: COSINE -0.1 mean_b <normalize(booster), normalize(light)>, EUCLID sqrt(sum (b - l)^2),
+ *             CE = the mean over the batch of -sum_c q_c log p_c, q = (1 - eps) onehot(label) + eps / C.
+ *             The per-sample terms are summed per CTA and the CTA rows folded in CTA order (partials: grid rows of
+ *             3 + n_pairs floats).  pair_stats [n_pairs][B][2] (COSINE) keeps what the backward needs.
+ *   head_bwd: dlosses [3 + n_pairs] (device) -> dh of every head, dlight of every pair, dparams = dW_light | db_light
+ *             | dW_booster | db_booster as per-CTA partials (grid rows) reduced in CTA order.  No float atomics.
+ * The description travels by value as a kernel parameter: graph-capturable. */
+#define TZK_ROCKET_MAX_PAIRS 8
+#define TZK_ROCKET_MAX_CLASSES 8
+#define TZK_ROCKET_COSINE 0
+#define TZK_ROCKET_EUCLID 1
+typedef struct tzk_rocket_head {
+  const float* h;
+  const float* w;
+  const float* b;
+  float* logits;
+  float* probs;
+  float* dh; /* head_bwd only */
+  int32_t H, pad_;
+} tzk_rocket_head;
+typedef struct tzk_rocket_pair {
+  const float* light;
+  const float* booster;
+  float* dlight; /* head_bwd only */
+  int32_t d, pad_;
+} tzk_rocket_pair;
+typedef struct tzk_rocket_args {
+  int64_t B;
+  int32_t C, has_booster, n_pairs, sim;
+  float eps;
+  int32_t pad_;
+  const float* labels;
+  float* pair_stats;
+  tzk_rocket_head head[2];
+  tzk_rocket_pair pair[TZK_ROCKET_MAX_PAIRS];
+} tzk_rocket_args;
+int tzk_rocket_head_fwd(const tzk_rocket_args* args_host, int32_t grid, float* partials, float* losses,
+                        tzk_stream_t stream);
+int tzk_rocket_head_bwd(const tzk_rocket_args* args_host, const float* dlosses, const float* losses, int32_t grid,
+                        float* partials, float* dparams, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -54,6 +54,30 @@ class TzkPepnetGateArgs(ctypes.Structure):
     _fields_ = [("B", c_int64), ("n_segs", c_int32), ("pad_", c_int32), ("seg", TzkPepnetSeg * PEPNET_MAX_SEGS)]
 
 
+ROCKET_MAX_PAIRS, ROCKET_MAX_CLASSES, ROCKET_COSINE, ROCKET_EUCLID = 8, 8, 0, 1
+
+
+class TzkRocketHead(ctypes.Structure):
+    """struct tzk_rocket_head (include/tzk.h): one output head of RocketLaunching (hidden, Linear, logits, probs)."""
+
+    _fields_ = [("h", c_void_p), ("w", c_void_p), ("b", c_void_p), ("logits", c_void_p), ("probs", c_void_p),
+                ("dh", c_void_p), ("H", c_int32), ("pad_", c_int32)]
+
+
+class TzkRocketPair(ctypes.Structure):
+    """struct tzk_rocket_pair (include/tzk.h): one light / booster hidden-layer pair of the similarity losses."""
+
+    _fields_ = [("light", c_void_p), ("booster", c_void_p), ("dlight", c_void_p), ("d", c_int32), ("pad_", c_int32)]
+
+
+class TzkRocketArgs(ctypes.Structure):
+    """struct tzk_rocket_args (include/tzk.h): the light head, optionally the booster head and up to 8 pairs."""
+
+    _fields_ = [("B", c_int64), ("C", c_int32), ("has_booster", c_int32), ("n_pairs", c_int32), ("sim", c_int32),
+                ("eps", c_float), ("pad_", c_int32), ("labels", c_void_p), ("pair_stats", c_void_p),
+                ("head", TzkRocketHead * 2), ("pair", TzkRocketPair * ROCKET_MAX_PAIRS)]
+
+
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
 SIGNATURES = {
     "tzk_abi_version": (c_int32, []),
@@ -218,6 +242,9 @@ SIGNATURES = {
     # JRC loss: session sort, per-session sums, loss and d loss / d logits in one call
     "tzk_jrc_loss_workspace_bytes": (c_size_t, [c_int64]),
     "tzk_jrc_loss": (c_int32, [P, c_int64, P, P, P, c_int64, c_float, c_int32, P, P, P, c_size_t, P]),
+    # RocketLaunching: both output heads, their softmax and every distillation loss (TzkRocketArgs), each direction
+    "tzk_rocket_head_fwd": (c_int32, [P, c_int32, P, P, P]),
+    "tzk_rocket_head_bwd": (c_int32, [P, P, P, c_int32, P, P, P]),
 }
 
 _lib = None

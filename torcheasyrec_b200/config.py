@@ -131,7 +131,7 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
                   "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE",
-                  "pepnet": "PEPNet", "dbmtl": "DBMTL"}.get(k, "Generic"))
+                  "pepnet": "PEPNet", "dbmtl": "DBMTL", "rocket_launching": "RocketLaunching"}.get(k, "Generic"))
            for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
@@ -168,9 +168,13 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
                   "out_task_space_weight": _f(F, 1.0)},
     "DBMTL": {"mask_net": _f("MaskNetModule"), "bottom_mlp": _f("MLP"), "expert_mlp": _f("MLP"), "gate_mlp": _f("MLP"),
               "num_expert": _f(I, 3), "task_towers": _f("BayesTaskTower", rep=True)},
-    "LossConfig": {"binary_cross_entropy": _f("Generic"), "softmax_cross_entropy": _f("Generic"),
+    # feature_distillation_function: a Similarity (simi.proto: COSINE, INNER_PRODUCT, EUCLID)
+    "RocketLaunching": {"share_mlp": _f("MLP"), "booster_mlp": _f("MLP"), "light_mlp": _f("MLP"),
+                        "feature_based_distillation": _f(B, False), "feature_distillation_function": _f(E, "COSINE")},
+    "LossConfig": {"binary_cross_entropy": _f("Generic"), "softmax_cross_entropy": _f("SoftmaxCrossEntropy"),
                    "l2_loss": _f("Generic"), "jrc_loss": _f("JRCLoss"), "binary_focal_loss": _f("Generic")},
     "JRCLoss": {"session_name": _f(S), "alpha": _f(F, 0.5)},
+    "SoftmaxCrossEntropy": {"label_smoothing": _f(F, 0.0)},
     "SeqEncoderConfig": {"din_encoder": _f("DINEncoder"), "simple_attention": _f("Generic"),
                          "pooling_encoder": _f("Generic"), "multi_window_din_encoder": _f("Generic"),
                          "self_attention_encoder": _f("Generic")},

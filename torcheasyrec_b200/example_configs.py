@@ -1,6 +1,6 @@
 """Generators for the pipeline configs BASELINE.json names (text format, same message tree as the reference's
 examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo,ple_taobao,
-pepnet_taobao}.config).
+pepnet_taobao,rocket_launching_criteo}.config).
 
 The package does not depend on the reference's files, so the configs are re-derived here from their defining facts
 (SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table list and price boundaries, and the model
@@ -310,10 +310,27 @@ def dbmtl_taobao_seq() -> str:
             + _dbmtl_towers(10000, "binary_cross_entropy {}") + "    }\n}\n")
 
 
+def rocket_launching_criteo() -> str:
+    """examples/rocket_launching_criteo.config: dlrm_criteo's features in one DEEP group `deep` (13 raw + 26 id(D=16),
+    429 wide); rocket_launching{booster 256-128-64-32, light 96-64-32, feature_based_distillation}; a two-class head
+    with softmax cross-entropy."""
+    ints = [f"int_{i}" for i in range(13)]
+    cats = [f"cat_{i}" for i in range(26)]
+    return (_header("criteo_terabyte_train_hashed_v1", "criteo_terabyte_val_test_hashed_v1", "rocket_launch_criteo",
+                    "FG_DAG", ["label"], 100)
+            + _criteo_features(True)
+            + "model_config {\n" + _group("deep", ints + cats, "DEEP")
+            + "    rocket_launching {\n" + _mlp("booster_mlp", [256, 128, 64, 32], "        ")
+            + _mlp("light_mlp", [96, 64, 32], "        ") + "        feature_based_distillation: true\n    }\n"
+            "    num_class: 2\n"
+            "    metrics {\n        auc {}\n    }\n    losses {\n        softmax_cross_entropy {}\n    }\n}\n")
+
+
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
               "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo,
               "ple_taobao": ple_taobao, "pepnet_taobao": pepnet_taobao, "dbmtl_taobao": dbmtl_taobao,
-              "dbmtl_taobao_jrc": dbmtl_taobao_jrc, "dbmtl_taobao_seq": dbmtl_taobao_seq}
+              "dbmtl_taobao_jrc": dbmtl_taobao_jrc, "dbmtl_taobao_seq": dbmtl_taobao_seq,
+              "rocket_launching_criteo": rocket_launching_criteo}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
 EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}

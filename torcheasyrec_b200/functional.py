@@ -966,3 +966,116 @@ def jrc_loss(logits: torch.Tensor, labels: torch.Tensor, session_ids: torch.Tens
     if weights is None:
         return torch_jrc_loss(logits, labels, session_ids, alpha, "mean")
     return torch.mean(torch_jrc_loss(logits, labels, session_ids, alpha, "none") * weights)
+
+
+# --------------------------------------------------------------------------------------------------------
+# RocketLaunching head (tzrec/models/rocket_launching.py; csrc/tzk_rocket.cuh)
+# --------------------------------------------------------------------------------------------------------
+ROCKET_MAX_CLASSES = 8        # csrc/tzk_rocket.cuh: the logits of a sample stay in registers
+ROCKET_MAX_PAIRS = 8          # similarity pairs in one launch
+ROCKET_MAX_WIDTH = 1024       # hidden and pair widths
+ROCKET_COSINE, ROCKET_EUCLID = 0, 1
+
+
+def rocket_head_usable(hiddens: Sequence[torch.Tensor], num_class: int, pair_widths: Sequence[int]) -> bool:
+    """True when tzk_rocket_head covers the heads over `hiddens` (light first) with `num_class` outputs and similarity
+    pairs of `pair_widths`: fp32 2-D hidden layers, autocast and TF32 off, 2 <= num_class <= 8, every hidden and pair
+    width a multiple of 4 from 4 to 1024, at most 8 pairs; on CUDA (on the CPU only a test backend that implements the
+    kernels)."""
+    t = hiddens[0]
+    if autocast_dtype(t) is not None or not 2 <= num_class <= ROCKET_MAX_CLASSES or len(pair_widths) > ROCKET_MAX_PAIRS:
+        return False
+    if any(h.dtype != torch.float32 or h.dim() != 2 or h.device != t.device for h in hiddens):
+        return False
+    if not all(4 <= w <= ROCKET_MAX_WIDTH and w % 4 == 0 for w in [h.shape[1] for h in hiddens] + list(pair_widths)):
+        return False
+    if t.is_cuda:
+        return _backend is None and not torch.backends.cuda.matmul.allow_tf32
+    return _backend is not None and hasattr(_backend, "rocket_head_fwd")
+
+
+class _RocketHead(torch.autograd.Function):
+    """Both heads' Linear + softmax and every loss of RocketLaunching in one tzk_rocket_head_fwd call, their gradients
+    in one tzk_rocket_head_bwd call.  Outputs: logits and probs of every head (not differentiable), then the loss
+    vector [CE light, CE booster, hint, sim_0, ...] (empty without labels)."""
+
+    @staticmethod
+    def forward(ctx, spec, labels, *tensors):
+        n_heads, n_pairs, eps, sim = spec
+        heads = [tuple(tensors[3 * e:3 * e + 3]) for e in range(n_heads)]
+        rest = tensors[3 * n_heads:]
+        pairs = [(rest[2 * k], rest[2 * k + 1]) for k in range(n_pairs)]
+        logits, probs, losses, stats = backend().rocket_head_fwd(heads, labels, eps, pairs, sim)
+        if losses is None:
+            losses = logits[0].new_empty(0)
+        ctx.mark_non_differentiable(*logits, *probs)
+        ctx.save_for_backward(labels, stats, losses, *logits, *probs, *tensors)
+        ctx.spec = spec
+        return (*logits, *probs, losses)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        n_heads, n_pairs, eps, sim = ctx.spec
+        labels, stats, losses, *rest = ctx.saved_tensors
+        logits, probs, tensors = rest[:n_heads], rest[n_heads:2 * n_heads], rest[2 * n_heads:]
+        heads = [tuple(tensors[3 * e:3 * e + 3]) for e in range(n_heads)]
+        pr = tensors[3 * n_heads:]
+        pairs = [(pr[2 * k], pr[2 * k + 1]) for k in range(n_pairs)]
+        dlosses = grads[-1].to(torch.float32).contiguous()
+        dhs, dlights, dparams = backend().rocket_head_bwd(heads, logits, probs, labels, eps, pairs, sim, stats, losses,
+                                                          dlosses)
+        out = [None, None]
+        for dh, (dw, db) in zip(dhs, dparams):
+            out += [dh, dw, db]
+        for dl in dlights:
+            out += [dl, None]
+        return tuple(out)
+
+
+def rocket_head(heads, labels: Optional[torch.Tensor], eps: float = 0.0, pairs=(), sim: int = ROCKET_COSINE):
+    """heads [(h [B, H], weight [C, H], bias [C])]: the light head, then optionally the booster head; labels [B] (class
+    indices) or None; pairs [(light [B, d], booster [B, d])], the booster side taken as detached.  -> (logits per head,
+    probs per head, losses [CE light, CE booster, hint, sim_0, ...] or None without labels), from one fused call each
+    way.  The caller checks rocket_head_usable first."""
+    y = None if labels is None else labels.to(torch.float32).contiguous()
+    flat = [t.contiguous() for h in heads for t in h]
+    for light, booster in pairs:
+        flat += [light.contiguous(), booster.detach().contiguous()]
+    out = _RocketHead.apply((len(heads), len(pairs), float(eps), int(sim)), y, *flat)
+    n = len(heads)
+    losses = out[2 * n]
+    return list(out[:n]), list(out[n:2 * n]), (list(losses.unbind(0)) if labels is not None else None)
+
+
+def feature_based_sim(light: torch.Tensor, booster: torch.Tensor, sim: int) -> torch.Tensor:
+    """rocket_launching.py:125-155 without sample weights: COSINE -0.1 mean_b <normalize(b), normalize(l)> with the
+    booster detached; any other value the EUCLID branch sqrt(sum (b - l)^2) over the whole batch."""
+    import torch.nn.functional as F
+
+    b = booster.detach()
+    if sim == ROCKET_COSINE:
+        return -0.1 * torch.mean(torch.sum(torch.mul(F.normalize(b, p=2, dim=1), F.normalize(light, p=2, dim=1)), dim=1))
+    return torch.sqrt(torch.sum(torch.square(b - light)))
+
+
+def torch_rocket_head(heads, labels: Optional[torch.Tensor], eps: float = 0.0, pairs=(), sim: int = ROCKET_COSINE):
+    """rocket_head in torch ops, as the reference computes it (the fallback on CPU tensors, under autocast, with TF32 on
+    and outside the kernels' cover).  heads [(h, linear module)]."""
+    logits = [lin(h) for h, lin in heads]
+    probs = [torch.softmax(z, dim=1) for z in logits]
+    return logits, probs, None if labels is None else torch_rocket_losses(logits, labels, eps, pairs, sim)
+
+
+def torch_rocket_losses(logits: Sequence[torch.Tensor], labels: torch.Tensor, eps: float = 0.0, pairs=(),
+                        sim: int = ROCKET_COSINE) -> List[Optional[torch.Tensor]]:
+    """[CE light, CE booster, hint, sim_0, ...] of rocket_launching.py:182-245 from the heads' logits (light first;
+    None where the booster head is absent): CrossEntropyLoss(mean, label_smoothing) on the label as a class index,
+    MSELoss(mean)(logits_light, logits_booster.detach()) and feature_based_sim per pair."""
+    import torch.nn.functional as F
+
+    target = labels.to(torch.int64)
+    ce = [F.cross_entropy(z, target, reduction="mean", label_smoothing=eps) for z in logits]
+    losses = [ce[0], ce[1] if len(ce) > 1 else None,
+              F.mse_loss(logits[0], logits[1].detach()) if len(logits) > 1 else None]
+    losses += [feature_based_sim(light, booster, sim) for light, booster in pairs]
+    return losses

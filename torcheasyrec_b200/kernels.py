@@ -1364,6 +1364,81 @@ class CudaKernels:
         self.launches += 6 if B > 0 else 1            # iota, pass 1-3 and two carries; B = 0: one carry (CUB's sort not counted)
         return loss, dlogits
 
+    # ------------------------------------------------------------------ RocketLaunching head (csrc/tzk_rocket.cuh)
+    # Resident CTAs per SM: ptxas register counts at 256 threads (head_fwd 80 -> 3, head_bwd 48 -> 5).  The grid fixes
+    # the order of the loss and parameter sums and depends only on the batch size and the device.
+    def _rocket_args(self, heads, logits, probs, labels, eps: float, pairs, sim: int, pair_stats, dhs=None,
+                     dlights=None):
+        from ._lib import ROCKET_MAX_PAIRS, TzkRocketArgs
+
+        if not 1 <= len(heads) <= 2 or len(pairs) > ROCKET_MAX_PAIRS:
+            raise TzkError(f"rocket head: 1 or 2 heads and at most {ROCKET_MAX_PAIRS} pairs")
+        a = TzkRocketArgs()
+        B, C = heads[0][0].shape[0], heads[0][1].shape[0]
+        a.B, a.C, a.has_booster, a.n_pairs, a.sim, a.eps = B, C, len(heads) - 1, len(pairs), int(sim), float(eps)
+        if labels is not None:
+            a.labels = _need(labels, torch.float32, "labels").data_ptr()
+            if labels.numel() != B:
+                raise TzkError("rocket head: need one label per sample")
+        a.pair_stats = _ptr(pair_stats)
+        for e, (h, w, b) in enumerate(heads):
+            for t, nm in ((h, "h"), (w, "w"), (b, "b"), (logits[e], "logits"), (probs[e], "probs")):
+                _need(t, torch.float32, f"head[{e}].{nm}")
+            if h.shape[0] != B or tuple(w.shape) != (C, h.shape[1]) or b.numel() != C:
+                raise TzkError("rocket head: need h [B, H], w [C, H] and b [C] with one B and one C")
+            g = a.head[e]
+            g.h, g.w, g.b, g.logits, g.probs, g.H = h.data_ptr(), w.data_ptr(), b.data_ptr(), logits[e].data_ptr(), \
+                probs[e].data_ptr(), h.shape[1]
+            if dhs is not None:
+                g.dh = dhs[e].data_ptr()
+        for k, (l, o) in enumerate(pairs):
+            _need(l, torch.float32, f"pair[{k}].light")
+            _need(o, torch.float32, f"pair[{k}].booster")
+            if l.shape != o.shape or l.shape[0] != B:
+                raise TzkError("rocket head: the light and booster layers of a pair must have one [B, d] shape")
+            p = a.pair[k]
+            p.light, p.booster, p.d = l.data_ptr(), o.data_ptr(), l.shape[1]
+            if dlights is not None:
+                p.dlight = dlights[k].data_ptr()
+        return a
+
+    def rocket_head_fwd(self, heads, labels, eps: float, pairs, sim: int):
+        """heads [(h [B, H], w [C, H], b [C])]: the light head, then optionally the booster head; labels [B] fp32 class
+        indices or None; pairs [(light [B, d], booster [B, d])] -> (logits per head, probs per head, losses
+        [3 + n_pairs] or None, pair_stats or None)."""
+        dev = heads[0][0].device
+        B, C = heads[0][0].shape[0], heads[0][1].shape[0]
+        logits = [torch.empty((B, C), dtype=torch.float32, device=dev) for _ in heads]
+        probs = [torch.empty((B, C), dtype=torch.float32, device=dev) for _ in heads]
+        pair_stats = torch.empty((len(pairs), B, 2), dtype=torch.float32, device=dev) if pairs else None
+        losses = partials = None
+        grid = self._grid(-(-int(B) // 8), 3)
+        if labels is not None:
+            losses = torch.empty(3 + len(pairs), dtype=torch.float32, device=dev)
+            partials = self._workspace("rocket_fwd", grid * losses.numel() * 4, dev)
+        a = self._rocket_args(heads, logits, probs, labels, eps, pairs, sim, pair_stats)
+        check(self._lib.tzk_rocket_head_fwd(ctypes.byref(a), grid, _ptr(partials), _ptr(losses), _stream()),
+              "tzk_rocket_head_fwd")
+        self.launches += int(B > 0) + int(labels is not None)
+        return logits, probs, losses, pair_stats
+
+    def rocket_head_bwd(self, heads, logits, probs, labels, eps: float, pairs, sim: int, pair_stats, losses, dlosses):
+        """dlosses [3 + n_pairs] (device) -> (dh per head, dlight per pair, [(dW [C, H], db [C])] per head)."""
+        _need(losses, torch.float32, "losses")
+        _need(dlosses, torch.float32, "dlosses")
+        dev = heads[0][0].device
+        B, C = heads[0][0].shape[0], heads[0][1].shape[0]
+        dhs = [torch.empty_like(h) for h, _, _ in heads]
+        dlights = [torch.empty_like(l) for l, _ in pairs]
+        a = self._rocket_args(heads, logits, probs, labels, eps, pairs, sim, pair_stats, dhs, dlights)
+        grid = self._grid(-(-int(B) // 32), 5)
+        shapes = [s for h, _, _ in heads for s in ((C, h.shape[1]), (C,))]
+        partials, dparams, views = self._batch_sums("rocket_bwd", grid, shapes, dev)
+        check(self._lib.tzk_rocket_head_bwd(ctypes.byref(a), _ptr(dlosses), _ptr(losses), grid, _ptr(partials),
+                                            _ptr(dparams), _stream()), "tzk_rocket_head_bwd")
+        self.launches += 1 + int(B > 0)
+        return dhs, dlights, list(zip(views[0::2], views[1::2]))
+
 
 @dataclass
 class ColPlan:

@@ -76,9 +76,10 @@ class Perceptron(nn.Module):
 class MLP(nn.Module):
     def __init__(self, in_features: int, hidden_units: List[int], bias: bool = True,
                  activation: Optional[str] = "nn.ReLU", use_bn: bool = False, dropout_ratio=None,
-                 use_ln: bool = False, dim: int = 2, **_: Any) -> None:
+                 use_ln: bool = False, dim: int = 2, return_hidden_layer_feature: bool = False, **_: Any) -> None:
         super().__init__()
         self.hidden_units = list(hidden_units)
+        self.return_hidden_layer_feature = return_hidden_layer_feature
         n = len(self.hidden_units)
         if dropout_ratio is None or (isinstance(dropout_ratio, list) and len(dropout_ratio) == 0):
             dropout_ratio = [0.0] * n
@@ -95,10 +96,18 @@ class MLP(nn.Module):
     def output_dim(self) -> int:
         return self.hidden_units[-1]
 
-    def forward(self, x: torch.Tensor, in_map=None) -> torch.Tensor:
-        """`in_map`: column map of a zero-padded input (see dense_gemm.linear), consumed by the first layer."""
+    def forward(self, x: torch.Tensor, in_map=None):
+        """`in_map`: column map of a zero-padded input (see dense_gemm.linear), consumed by the first layer.  With
+        return_hidden_layer_feature: {"hidden_layer<i>": output of layer i, "hidden_layer_end": the last} instead of
+        the last layer's output (mlp.py:161-177)."""
+        hidden = {}
         for i, layer in enumerate(self.mlp):
             x = layer(x, in_map) if (i == 0 and in_map is not None) else layer(x)
+            if self.return_hidden_layer_feature:
+                hidden[f"hidden_layer{i}"] = x
+        if self.return_hidden_layer_feature:
+            hidden["hidden_layer_end"] = x
+            return hidden
         return x
 
 
@@ -229,7 +238,8 @@ def _create_seq_encoder(seq_encoder_config: Message, group_total_dim: Dict[str, 
 # models
 # --------------------------------------------------------------------------------------------------------
 class RankModel(nn.Module):
-    """tzrec/models/rank_model.py:40-287 reduced to: init_input / build_input / prediction dict / BCE loss."""
+    """tzrec/models/rank_model.py:40-287 reduced to: init_input / build_input / prediction dict / the BCE loss of a
+    one-logit head or the softmax cross-entropy of a num_class > 1 head."""
 
     def __init__(self, model_config: Message, features: List[BaseFeature], labels: List[str],
                  sample_weights: Optional[List[str]] = None, device=None, **kwargs: Any) -> None:
@@ -246,10 +256,15 @@ class RankModel(nn.Module):
                                       "are outside the hot-path scope")
         self._device = device
         self.embedding_group: Optional[EmbeddingGroup] = None
+        # label_smoothing of the softmax_cross_entropy loss (None: a BCE head)
+        self._ce_smoothing: Optional[float] = None
         for lc in model_config.losses:
             kind = lc.WhichOneof("loss")
-            if kind not in (None, "binary_cross_entropy"):
-                raise NotImplementedError(f"loss {kind} is outside the hot-path scope (BCE-with-logits only)")
+            if kind not in (None, "binary_cross_entropy", "softmax_cross_entropy"):
+                raise NotImplementedError(f"loss {kind} is outside the hot-path scope (BCE-with-logits and softmax "
+                                          "cross-entropy only)")
+            if kind == "softmax_cross_entropy":
+                self._ce_smoothing = proto_float32(lc.softmax_cross_entropy.label_smoothing)
 
     def init_input(self) -> None:
         """rank_model.py:83-112."""
@@ -271,17 +286,32 @@ class RankModel(nn.Module):
         return self.embedding_group(batch)
 
     def _output_to_prediction(self, output: torch.Tensor, suffix: str = "") -> Dict[str, torch.Tensor]:
-        """rank_model.py:133-179 for num_class == 1 binary heads."""
+        """rank_model.py:133-179: a one-logit BCE head (logits [B], probs = sigmoid), or a softmax cross-entropy head
+        (logits [B, C], probs = softmax, and probs1 = probs[:, 1] when C == 2)."""
+        if self._ce_smoothing is not None:
+            assert self._num_class > 1, "num_class must be greater than 1 when loss type is softmax_cross_entropy"
+            probs = torch.softmax(output, dim=1)
+            preds = {"logits" + suffix: output, "probs" + suffix: probs}
+            if self._num_class == 2:
+                preds["probs1" + suffix] = probs[:, 1]
+            return preds
         assert self._num_class == 1, "only binary heads (num_class=1) are in scope"
         logits = torch.squeeze(output, dim=1)
         return {"logits" + suffix: logits, "probs" + suffix: torch.sigmoid(logits)}
 
+    def _softmax_ce(self, logits: torch.Tensor, batch: Batch) -> torch.Tensor:
+        """nn.CrossEntropyLoss(mean, label_smoothing) on the first label as a class index (rank_model.py:222-224)."""
+        label = batch.labels[self._label_name].to(torch.int64)
+        return F.cross_entropy(logits, label, reduction="mean", label_smoothing=self._ce_smoothing)
+
     def loss(self, predictions: Dict[str, torch.Tensor], batch: Batch) -> Dict[str, torch.Tensor]:
-        """rank_model.py:181-287: BCEWithLogitsLoss(mean) on the first label."""
+        """rank_model.py:181-287: BCEWithLogitsLoss(mean) or CrossEntropyLoss(mean) on the first label."""
         tail = getattr(self, "_tail_loss", None)
         if tail is not None:                 # computed together with the tower's tail (DLRM._fused_tail)
             self._tail_loss = None
             return {"binary_cross_entropy": tail}
+        if self._ce_smoothing is not None:
+            return {"softmax_cross_entropy": self._softmax_ce(predictions["logits"], batch)}
         label = batch.labels[self._label_name].to(torch.float32)
         from .dense_gemm import bce_with_logits
 
@@ -291,6 +321,10 @@ class RankModel(nn.Module):
     def _metric_heads(self):
         """[(metric configs, loss configs, label name, name suffix)]: the model's own for single-task models."""
         return [(list(self._base_model_config.metrics), list(self._base_model_config.losses), self._label_name, "")]
+
+    def _updated_metric_heads(self):
+        """The heads update_metric adds a batch to: all of them."""
+        return self._metric_heads()
 
     def init_metric(self, device=None, process_group=None, distributed: bool = False) -> None:
         """One metric state per configured metric and loss, named as the reference names them.  `distributed`:
@@ -306,6 +340,9 @@ class RankModel(nn.Module):
                 kind = mc.WhichOneof("metric")
                 if kind != "auc":
                     raise NotImplementedError(f"metric {kind}{suffix}: only auc and the loss metrics are implemented")
+                if self._ce_smoothing is not None and self._num_class > 2:
+                    raise ValueError(f"auc{suffix}: num_class must be at most 2 when metric type is auc "
+                                     f"(got {self._num_class})")
                 mods[kind + suffix] = BinnedAUC(mc.auc.thresholds, device)
             for lc in losses:
                 mods[lc.WhichOneof("loss") + suffix] = MeanLoss(device)
@@ -316,10 +353,11 @@ class RankModel(nn.Module):
                       losses: Optional[Dict[str, torch.Tensor]] = None) -> None:
         """Adds one batch to every metric state (device work only, capturable)."""
         mods = self._metric_modules
-        for metrics, loss_cfgs, label_name, suffix in self._metric_heads():
+        probs = "probs1" if self._ce_smoothing is not None else "probs"      # a two-class head's auc reads probs1
+        for metrics, loss_cfgs, label_name, suffix in self._updated_metric_heads():
             label = batch.labels[label_name]
             for mc in metrics:
-                mods[mc.WhichOneof("metric") + suffix].update(predictions["probs" + suffix], label)
+                mods[mc.WhichOneof("metric") + suffix].update(predictions[probs + suffix], label)
             if losses is not None:
                 for lc in loss_cfgs:
                     name = lc.WhichOneof("loss") + suffix
@@ -584,6 +622,11 @@ class MultiTaskRank(RankModel):
 
     def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
         super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        for lc in model_config.losses:          # a model-level loss: only BCE, which the towers' predictions assume
+            kind = lc.WhichOneof("loss")
+            if kind not in (None, "binary_cross_entropy"):
+                raise NotImplementedError(f"loss {kind} is outside the hot-path scope of multi-task models "
+                                          "(model-level BCE-with-logits only)")
         self._task_tower_cfgs = list(self._model_config.task_towers)
         self._jrc = {}                      # tower name -> its jrc_loss config
         for cfg in self._task_tower_cfgs:
@@ -1344,9 +1387,134 @@ class DBMTL(MultiTaskRank):
             [self.task_outputs[i](relation_net[tc.tower_name]) for i, tc in enumerate(self._task_tower_cfgs)])
 
 
+class RocketLaunching(RankModel):
+    """tzrec/models/rocket_launching.py:28-323: a booster MLP and a light MLP on the first feature group (after an
+    optional share_mlp), each with its own output Linear.  The light net reads the shared input detached and is the one
+    served; training adds the booster's loss, the hint MSE between the two heads' logits and, with
+    feature_based_distillation, a similarity loss for every light hidden layer whose width matches a booster layer.
+
+    Everything after the two MLPs (both Linears, the softmaxes and every loss) runs as one fused call each way when
+    Fn.rocket_head_usable holds (csrc/tzk_rocket.cuh); predict stashes the losses for loss().  Otherwise the heads and
+    losses are the reference's torch ops.  softmax_cross_entropy heads only; sample weights are refused."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        cfg = self._model_config
+        kinds = [lc.WhichOneof("loss") for lc in model_config.losses]
+        if not kinds or any(k != "softmax_cross_entropy" for k in kinds):
+            raise NotImplementedError(f"RocketLaunching: losses {kinds} are outside the hot-path scope "
+                                      "(softmax_cross_entropy only)")
+        self.return_hidden_layer_feature = bool(cfg.feature_based_distillation)
+        self.init_input()
+        self.group_name = self.embedding_group.group_names()[0]
+        feature_in = self.embedding_group.group_total_dim(self.group_name)
+        self.share_mlp = None
+        if cfg.HasField("share_mlp"):
+            self.share_mlp = MLP(feature_in, **config_to_kwargs(cfg.share_mlp))
+        in_dim = self.share_mlp.output_dim() if self.share_mlp else feature_in
+        self.booster_mlp = MLP(in_dim, return_hidden_layer_feature=self.return_hidden_layer_feature,
+                               **config_to_kwargs(cfg.booster_mlp))
+        self.booster_linear = nn.Linear(self.booster_mlp.output_dim(), self._num_class)
+        self.light_mlp = MLP(in_dim, return_hidden_layer_feature=self.return_hidden_layer_feature,
+                             **config_to_kwargs(cfg.light_mlp))
+        self.light_linear = nn.Linear(self.light_mlp.output_dim(), self._num_class)
+        self.hint_loss_name = "hint_l2_loss"
+        self.mlp_index_dict = self._get_distillation_mlp_index()
+        sim = cfg.feature_distillation_function
+        # any value but COSINE takes the reference's EUCLID branch (INNER_PRODUCT included)
+        self._sim = Fn.ROCKET_COSINE if sim in ("COSINE", 0, "") else Fn.ROCKET_EUCLID
+        self._head_losses = None
+
+    def _get_distillation_mlp_index(self) -> Dict[int, int]:
+        """light layer i -> the FIRST booster layer of the same width (several light layers may share one)."""
+        booster = list(self._model_config.booster_mlp.hidden_units)
+        out = {}
+        for i, unit_i in enumerate(self._model_config.light_mlp.hidden_units):
+            for j, unit_j in enumerate(booster):
+                if unit_i == unit_j:
+                    out[i] = j
+                    break
+        return out
+
+    def _head_prediction(self, logits: torch.Tensor, probs: torch.Tensor, suffix: str) -> Dict[str, torch.Tensor]:
+        preds = {"logits" + suffix: logits, "probs" + suffix: probs}
+        if self._num_class == 2:
+            preds["probs1" + suffix] = probs[:, 1]
+        return preds
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        assert self._num_class > 1, "num_class must be greater than 1 when loss type is softmax_cross_entropy"
+        net = self.build_input(batch)[self.group_name]
+        share_net = self.share_mlp(net) if self.share_mlp is not None else net
+        light_net = self.light_mlp(share_net.detach())
+        light_h = light_net["hidden_layer_end"] if self.return_hidden_layer_feature else light_net
+        booster_net = booster_h = None
+        pairs = []
+        if self.training:
+            booster_net = self.booster_mlp(share_net)
+            booster_h = booster_net["hidden_layer_end"] if self.return_hidden_layer_feature else booster_net
+            if self.mlp_index_dict and not self.return_hidden_layer_feature:
+                # the reference indexes the plain MLP outputs by layer name here and fails the same way
+                raise TypeError("RocketLaunching: light and booster layers of equal width need "
+                                "feature_based_distillation to expose their hidden layers")
+            pairs = [(light_net[f"hidden_layer{i}"], booster_net[f"hidden_layer{j}"])
+                     for i, j in self.mlp_index_dict.items()]
+        hiddens = [light_h] + ([booster_h] if self.training else [])
+        linears = [self.light_linear] + ([self.booster_linear] if self.training else [])
+        fused_pairs = pairs if self.return_hidden_layer_feature else []
+        self._head_losses = None
+        if Fn.rocket_head_usable(hiddens, self._num_class, [l.shape[1] for l, _ in fused_pairs]):
+            label = batch.labels.get(self._label_name) if self._label_name else None
+            logits, probs, self._head_losses = Fn.rocket_head(
+                [(h, m.weight, m.bias) for h, m in zip(hiddens, linears)], label, self._ce_smoothing, fused_pairs,
+                self._sim)
+        else:
+            logits, probs, _ = Fn.torch_rocket_head(list(zip(hiddens, linears)), None)
+        preds = self._head_prediction(logits[0], probs[0], "_light")
+        if self.training:
+            preds.update(self._head_prediction(logits[1], probs[1], "_booster"))
+            for (i, j), (light, booster) in zip(self.mlp_index_dict.items(), pairs):
+                preds[f"light_{i}"] = light
+                preds[f"booster_{j}"] = booster
+        return preds
+
+    def loss(self, predictions: Dict[str, torch.Tensor], batch: Batch) -> Dict[str, torch.Tensor]:
+        """rocket_launching.py:182-245: softmax_cross_entropy_booster (training), softmax_cross_entropy_light, then in
+        training similarity_<i>_<j> per pair (feature_based_distillation) and hint_l2_loss."""
+        losses, self._head_losses = self._head_losses, None
+        distill = self.training and self.return_hidden_layer_feature
+        if losses is None:
+            logits = [predictions["logits_light"]] + ([predictions["logits_booster"]] if self.training else [])
+            pairs = [(predictions[f"light_{i}"], predictions[f"booster_{j}"])
+                     for i, j in self.mlp_index_dict.items()] if distill else []
+            losses = Fn.torch_rocket_losses(logits, batch.labels[self._label_name], self._ce_smoothing, pairs,
+                                            self._sim)
+        ce_light, ce_booster, hint, *sims = losses
+        out = {}
+        if self.training:
+            out["softmax_cross_entropy_booster"] = ce_booster
+        out["softmax_cross_entropy_light"] = ce_light
+        if self.training:
+            if distill:
+                for (i, j), s in zip(self.mlp_index_dict.items(), sims):
+                    out[f"similarity_{i}_{j}"] = s
+            out[self.hint_loss_name] = hint
+        return out
+
+    def _metric_heads(self):
+        """rocket_launching.py:169-180: every metric and loss mean once per head, booster first."""
+        m, l = list(self._base_model_config.metrics), list(self._base_model_config.losses)
+        return [(m, l, self._label_name, "_booster"), (m, l, self._label_name, "_light")]
+
+    def _updated_metric_heads(self):
+        """rocket_launching.py:247-294: the booster head only in training; evaluation updates the light head alone."""
+        heads = self._metric_heads()
+        return heads if self.training else heads[1:]
+
+
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
                  "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE,
-                 "pepnet": PEPNet, "dbmtl": DBMTL}
+                 "pepnet": PEPNet, "dbmtl": DBMTL, "rocket_launching": RocketLaunching}
 
 
 class JRCLoss(nn.Module):
