@@ -322,6 +322,12 @@ int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_
                           int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
                           int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
                           tzk_stream_t stream);
+/* The same with dz read as dz * dz_scale[0] (a device scalar, e.g. the gradient reaching the loss), multiplied in
+ * before the TF32 split: the bits of tzk_interact_wide_bwd on that product.  dz_scale NULL: no scaling. */
+int tzk_interact_wide_bwd_scaled(const float* dz, int64_t ld_dz, const float* dz_scale, const float* w, int64_t ld_w,
+                                 const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M,
+                                 float* d_dense, int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi,
+                                 float* wt_lo, tzk_stream_t stream);
 /* The forward of the same pair of layers: y [M,64] = relu(X w^T + bias) with X = [351 pairs | 0 | dense | sparse] the
  * interaction's output, and pairs [M,352] = X's first 352 columns (column 351 zero), which the weight gradient needs.
  * X itself is never written.  w [64, ld_w] in the interaction's column layout (ld_w >= 784), bias nullable; w_hi / w_lo:
@@ -336,6 +342,11 @@ int tzk_interact_wide_fwd(const float* dense, int64_t ld_dense, const float* spa
 int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const float* pairs, int64_t ld_pairs, const float* dense,
                             int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, int32_t slabs,
                             float* partial, float* dw, int64_t ld_dw, tzk_stream_t stream);
+/* The same with dz read as dz * dz_scale[0], as tzk_interact_wide_bwd_scaled. */
+int tzk_interact_wide_wgrad_scaled(const float* dz, int64_t ld_dz, const float* dz_scale, const float* pairs,
+                                   int64_t ld_pairs, const float* dense, int64_t ld_dense, const float* sparse,
+                                   int64_t ld_sparse, int64_t M, int32_t slabs, float* partial, float* dw,
+                                   int64_t ld_dw, tzk_stream_t stream);
 
 /* ---- dense-tower helpers (callers of the path: tzrec/modules/mlp.py:20-84, Perceptron = Linear -> ReLU) ----
  * The tower GEMMs stay library calls; these fuse the element-wise passes around them.
@@ -371,11 +382,13 @@ size_t tzk_bce_logits_workspace_bytes(int64_t M);
  * tzrec/modules/mlp.py:20-84), output Linear(N, 1) and mean BCE-with-logits on the label (tzrec/models/rank_model.py:
  * 133-179, 181-262).  h = relu(y1 @ w1^T + b1); logits = h @ w2^T + b2; loss as tzk_bce_logits; and d loss / d ... :
  * dy1 [M, K] and out = [dW1 (N x K, row-major) | db1 (N) | dw2 (N) | db2 (1) | loss (1)].  K, N <= 64; b1, b2 nullable.
- * Deterministic (fixed-order folds).  Replaces 18 launches of the unfused chain on DLRM-Criteo (64 -> 32 -> 1). */
+ * Deterministic (fixed-order folds).  Replaces 18 launches of the unfused chain on DLRM-Criteo (64 -> 32 -> 1).
+ * colsum nullable.  Given (y1 the output of a ReLU layer), dy1 receives dz = dy1 * (y1 > 0) instead, the gradient of
+ * that layer's pre-activation, and colsum [K] its column sums (at K = 64 the bits of tzk_act_bwd_colsum on dy1, y1). */
 size_t tzk_tower_tail_bce_workspace_bytes(int64_t M, int32_t K, int32_t N);
 int tzk_tower_tail_bce(const float* y1, int64_t ld_y, const float* w1, const float* b1, const float* w2, const float* b2,
                        const float* labels, int64_t M, int32_t K, int32_t N, float* logits, float* dy1, int64_t ld_dy,
-                       float* out, void* workspace, size_t workspace_bytes, tzk_stream_t stream);
+                       float* colsum, float* out, void* workspace, size_t workspace_bytes, tzk_stream_t stream);
 int tzk_bce_logits_fwd_bwd(const float* logits, const float* labels, int64_t M, float* loss, float* dlogits,
                            void* workspace, size_t workspace_bytes, tzk_stream_t stream);
 

@@ -165,12 +165,17 @@ SIGNATURES = {
     ),
     "tzk_interact_wide_bwd": (
         c_int32, [P, c_int64, P, c_int64, P, c_int64, P, c_int64, c_int64, P, c_int64, P, c_int64, P, P, P]),
+    "tzk_interact_wide_bwd_scaled": (
+        c_int32, [P, c_int64, P, P, c_int64, P, c_int64, P, c_int64, c_int64, P, c_int64, P, c_int64, P, P, P]),
     "tzk_interact_wide_fwd": (
         c_int32, [P, c_int64, P, c_int64, P, c_int64, P, c_int64, P, c_int64, P, c_int64, P, P, P]),
     "tzk_interact_wide_wgrad": (
         c_int32, [P, c_int64, P, c_int64, P, c_int64, P, c_int64, c_int64, c_int32, P, P, c_int64, P]),
+    "tzk_interact_wide_wgrad_scaled": (
+        c_int32, [P, c_int64, P, P, c_int64, P, c_int64, P, c_int64, c_int64, c_int32, P, P, c_int64, P]),
     "tzk_tower_tail_bce_workspace_bytes": (c_size_t, [c_int64, c_int32, c_int32]),
-    "tzk_tower_tail_bce": (c_int32, [P, c_int64, P, P, P, P, P, c_int64, c_int32, c_int32, P, P, c_int64, P, P, c_size_t, P]),
+    "tzk_tower_tail_bce": (
+        c_int32, [P, c_int64, P, P, P, P, P, c_int64, c_int32, c_int32, P, P, c_int64, P, P, P, c_size_t, P]),
     "tzk_din_attn_input_fwd": (c_int32, [P, c_int64, c_int32, P, P, c_int32, c_int32, c_int64, P, P]),
     "tzk_din_attn_input_bwd": (c_int32, [P, P, c_int64, c_int32, P, P, c_int32, c_int32, c_int64, P, P, P]),
     "tzk_jagged_softmax_wsum_fwd": (c_int32, [P, P, P, c_int32, c_int32, c_int32, c_int64, P, P, P]),

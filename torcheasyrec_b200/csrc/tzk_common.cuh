@@ -11,6 +11,9 @@
 namespace tzk {
 
 void set_error(const char* fmt, ...);
+// colsum[c] = sum over b (ascending) of partial[b][c], b < n_blocks, c < N: act_bwd_colsum's fold of its per-slab
+// column sums (tzk_dense.cu), shared with the tower tail's masked mode (tzk_tower.cu)
+void colsum_final(const float* partial, int64_t n_blocks, int N, float* colsum, cudaStream_t st);
 
 inline cudaStream_t as_stream(tzk_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 

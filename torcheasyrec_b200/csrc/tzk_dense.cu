@@ -823,6 +823,10 @@ colsum_final_kernel(const float* __restrict__ partial, int64_t n_blocks, int N, 
 }
 }  // namespace
 
+void tzk::colsum_final(const float* partial, int64_t n_blocks, int N, float* colsum, cudaStream_t st) {
+  colsum_final_kernel<<<(N + 31) / 32, 256, 0, st>>>(partial, n_blocks, N, colsum);
+}
+
 extern "C" int tzk_bias_act(float* y, int64_t ld_y, const float* bias, int64_t M, int32_t N, int32_t relu,
                             tzk_stream_t stream) {
   TZK_REQUIRE(M >= 0 && N >= 1, "bias_act: bad sizes");
@@ -857,7 +861,7 @@ extern "C" int tzk_act_bwd_colsum(const float* dy, int64_t ld_dy, const float* y
   act_bwd_colsum_kernel<<<(unsigned)nb, kThreads, 0, as_stream(stream)>>>(dy, ld_dy, y, ld_y, M, N, relu, dz, ld_dz,
                                                                           partial);
   TZK_CHECK_LAUNCH("act_bwd_colsum_kernel");
-  colsum_final_kernel<<<(N + 31) / 32, 256, 0, as_stream(stream)>>>(partial, nb, N, colsum);
+  colsum_final(partial, nb, N, colsum, as_stream(stream));
   TZK_CHECK_LAUNCH("colsum_final_kernel");
   return 0;
 }

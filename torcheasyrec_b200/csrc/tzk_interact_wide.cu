@@ -119,6 +119,7 @@ struct FbParams {
   float* d_dense; int64_t ld_ddense;
   float* d_sparse; int64_t ld_dsparse;
   int64_t M;
+  const float* dz_scale;   // nullable: dZ is read times *dz_scale
 };
 
 __global__ void __launch_bounds__(FB_THREADS, 1)
@@ -175,6 +176,7 @@ interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     // of all of it would take 64 registers and leave too few for the accumulators
     float a[8][4];
     {
+      const float zk = p.dz_scale ? __ldg(p.dz_scale) : 1.f;   // x * 1 is x: no scale, the same bits
       const int s = (int)(item0 % FB_STAGES);
       mbar_wait(full + 2 * s, (uint32_t)(item0 / FB_STAGES) & 1u);
       mbar_wait(full + 2 * s + 1, (uint32_t)(item0 / FB_STAGES) & 1u);
@@ -183,10 +185,10 @@ interact_wide_bwd_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
       for (int kk = 0; kk < 8; ++kk) {
         const float* box = zs + (kk >> 2) * (FB_HALF / 4);
         const int k0 = (kk & 3) * 8 + t, k1 = k0 + 4;
-        a[kk][0] = box[swz(r, k0)];
-        a[kk][1] = box[swz(r + 8, k0)];
-        a[kk][2] = box[swz(r, k1)];
-        a[kk][3] = box[swz(r + 8, k1)];
+        a[kk][0] = box[swz(r, k0)] * zk;
+        a[kk][1] = box[swz(r + 8, k0)] * zk;
+        a[kk][2] = box[swz(r, k1)] * zk;
+        a[kk][3] = box[swz(r + 8, k1)] * zk;
       }
     }
     __syncthreads();                              // dZ read by every warp; the previous tile's P read
@@ -516,13 +518,14 @@ interact_wide_wgrad_kernel(const __grid_constant__ CUtensorMap map_x0, const __g
     const float* zs = reinterpret_cast<const float*>(smem + s * WG_STAGE + WG_A);
     auto at = [](const float* base, int m, int col) { return base[(col >> 5) * (WG_BOX / 4) + swz(m, col & 31)]; };
     // dZ^T (n, m) at swz(n, m): 16-B stores, the 8 lanes of a quarter-warp on the 8 chunks of a swizzle row group
+    const float zk = p.dz_scale ? __ldg(p.dz_scale) : 1.f;  // x * 1 is x: no scale, the same bits
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int m = 4 * tq + 16 * h;
       float hi[4], lo[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float v = at(zs, m + j, tn);
+        const float v = at(zs, m + j, tn) * zk;
         hi[j] = tf32_rna(v);
         lo[j] = tf32_rna(v - hi[j]);
       }
@@ -587,10 +590,11 @@ extern "C" int tzk_interact_wide_bwd_timing(unsigned long long* buf) {
 }
 #endif
 
-extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_t ld_w, const float* dense,
-                                     int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
-                                     int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
-                                     tzk_stream_t stream) {
+extern "C" int tzk_interact_wide_bwd_scaled(const float* dz, int64_t ld_dz, const float* dz_scale, const float* w,
+                                            int64_t ld_w, const float* dense, int64_t ld_dense, const float* sparse,
+                                            int64_t ld_sparse, int64_t M, float* d_dense, int64_t ld_ddense,
+                                            float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
+                                            tzk_stream_t stream) {
   TZK_REQUIRE(M > 0, "interact_wide_bwd: M must be positive");
   TZK_REQUIRE(ld_w >= tzk_itc::kRow, "interact_wide_bwd: w needs %d columns", tzk_itc::kRow);
   const int64_t lds[] = {ld_dz, ld_w, ld_dense, ld_sparse, ld_ddense, ld_dsparse};
@@ -614,6 +618,7 @@ extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float
   FbParams p;
   p.dense = dense; p.ld_dense = ld_dense; p.sparse = sparse; p.ld_sparse = ld_sparse;
   p.d_dense = d_dense; p.ld_ddense = ld_ddense; p.d_sparse = d_sparse; p.ld_dsparse = ld_dsparse; p.M = M;
+  p.dz_scale = dz_scale;
 #ifndef TZK_CPU_SHIM
   static bool configured = false;     // once: nothing but the launches happens inside a stream capture
   if (!configured) {
@@ -625,6 +630,14 @@ extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float
   TZK_LAUNCH((interact_wide_bwd_kernel), (unsigned)(tiles < sms ? tiles : sms), FB_THREADS, FB_SMEM, st, mz, mh, ml, p);
   TZK_CHECK_LAUNCH("interact_wide_bwd_kernel");
   return 0;
+}
+
+extern "C" int tzk_interact_wide_bwd(const float* dz, int64_t ld_dz, const float* w, int64_t ld_w, const float* dense,
+                                     int64_t ld_dense, const float* sparse, int64_t ld_sparse, int64_t M, float* d_dense,
+                                     int64_t ld_ddense, float* d_sparse, int64_t ld_dsparse, float* wt_hi, float* wt_lo,
+                                     tzk_stream_t stream) {
+  return tzk_interact_wide_bwd_scaled(dz, ld_dz, nullptr, w, ld_w, dense, ld_dense, sparse, ld_sparse, M, d_dense,
+                                      ld_ddense, d_sparse, ld_dsparse, wt_hi, wt_lo, stream);
 }
 
 extern "C" int tzk_interact_wide_fwd(const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse,
@@ -661,10 +674,10 @@ extern "C" int tzk_interact_wide_fwd(const float* dense, int64_t ld_dense, const
   return 0;
 }
 
-extern "C" int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const float* pairs, int64_t ld_pairs,
-                                       const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse,
-                                       int64_t M, int32_t slabs, float* partial, float* dw, int64_t ld_dw,
-                                       tzk_stream_t stream) {
+extern "C" int tzk_interact_wide_wgrad_scaled(const float* dz, int64_t ld_dz, const float* dz_scale,
+                                              const float* pairs, int64_t ld_pairs, const float* dense, int64_t ld_dense,
+                                              const float* sparse, int64_t ld_sparse, int64_t M, int32_t slabs,
+                                              float* partial, float* dw, int64_t ld_dw, tzk_stream_t stream) {
   TZK_REQUIRE(M > 0 && slabs > 0, "interact_wide_wgrad: M and slabs must be positive");
   TZK_REQUIRE(ld_dw >= tzk_itc::kRow, "interact_wide_wgrad: dw needs %d columns", tzk_itc::kRow);
   const int64_t lds[] = {ld_dz, ld_pairs, ld_dense, ld_sparse};
@@ -682,7 +695,16 @@ extern "C" int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const flo
   const WgSources src = {{0, FB_PAIR_CHUNKS, FB_CHUNKS - 1, FB_CHUNKS}, {0, 0, 0}, {0, FF_SPARSE0, tzk_itc::kInter},
                          {tzk_itc::kInter, tzk_itc::kRow - FF_SPARSE0, tzk_itc::kD}};
   TZK_REQUIRE(wgrad3x_launch<interact_wide_wgrad_kernel>(mx, mz, src, M, slabs, partial, dw, ld_dw,
-                                                         reinterpret_cast<cudaStream_t>(stream), 2 * WW_ZT) == 0,
+                                                         reinterpret_cast<cudaStream_t>(stream), 2 * WW_ZT,
+                                                         dz_scale) == 0,
               "interact_wide_wgrad: launch failed");
   return 0;
+}
+
+extern "C" int tzk_interact_wide_wgrad(const float* dz, int64_t ld_dz, const float* pairs, int64_t ld_pairs,
+                                       const float* dense, int64_t ld_dense, const float* sparse, int64_t ld_sparse,
+                                       int64_t M, int32_t slabs, float* partial, float* dw, int64_t ld_dw,
+                                       tzk_stream_t stream) {
+  return tzk_interact_wide_wgrad_scaled(dz, ld_dz, nullptr, pairs, ld_pairs, dense, ld_dense, sparse, ld_sparse, M,
+                                        slabs, partial, dw, ld_dw, stream);
 }

@@ -477,8 +477,8 @@ extern "C" size_t tzk_tower_tail_bce_workspace_bytes(int64_t M, int32_t K, int32
 
 extern "C" int tzk_tower_tail_bce(const float* y1, int64_t ld_y, const float* w1, const float* b1, const float* w2,
                                   const float* b2, const float* labels, int64_t M, int32_t K, int32_t N, float* logits,
-                                  float* dy1, int64_t ld_dy, float* out, void* workspace, size_t workspace_bytes,
-                                  tzk_stream_t stream) {
+                                  float* dy1, int64_t ld_dy, float* colsum, float* out, void* workspace,
+                                  size_t workspace_bytes, tzk_stream_t stream) {
   TZK_REQUIRE(M >= 1, "tower_tail_bce: empty batch");
   TZK_REQUIRE(tzk_tail::supported(K, N), "tower_tail_bce: K=%d, N=%d must be in [1, 64]", K, N);
   TZK_REQUIRE(y1 && w1 && w2 && labels && logits && dy1 && out, "tower_tail_bce: NULL argument");
@@ -486,7 +486,12 @@ extern "C" int tzk_tower_tail_bce(const float* y1, int64_t ld_y, const float* w1
   TZK_REQUIRE(workspace && workspace_bytes >= tzk_tower_tail_bce_workspace_bytes(M, K, N),
               "tower_tail_bce: workspace too small");
   const int rc = tzk_tail::run(y1, ld_y, w1, b1, w2, b2, labels, M, K, N, logits, dy1, ld_dy, out, workspace,
-                               workspace_bytes, as_stream(stream));
+                               workspace_bytes, as_stream(stream), colsum != nullptr);
   TZK_REQUIRE(rc == 0, "tower_tail_bce: tzk_tail::run failed with code %d", rc);
+  if (colsum) {
+    colsum_final(static_cast<const float*>(workspace) + tzk_tail::colsum_offset(M, K, N), tzk_tail::tiles(M), K, colsum,
+                 as_stream(stream));
+    TZK_CHECK_LAUNCH("colsum_final_kernel");
+  }
   return 0;
 }

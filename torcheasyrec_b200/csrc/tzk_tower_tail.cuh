@@ -16,6 +16,11 @@
 // The per-CTA sums leave as one vector [N K | N | N | 1 | 1] = dW1, db1, dw2, db2, loss; tower_tail_reduce_kernel folds
 // the CTAs in CTA order: deterministic.
 //
+// Masked mode (kMask; y1 the output of a ReLU layer): the kernel stores dZ = dy1 * [y1 > 0], the gradient of that
+// layer's pre-activation, in place of dy1, and per 128-row tile the K column sums of dZ, in act_bwd_colsum_kernel's
+// order at 64 columns (tzk_dense.cu): its 128-row slabs are these tiles, so colsum_final_kernel folds them into the
+// layer's bias gradient with act_bwd_colsum's bits.  The separate ReLU-backward pass over [M, K] is not needed.
+//
 // Plain CUDA (no PTX): the includer provides TZK_DYN_SMEM / TZK_LAUNCH (nvcc: tzk_tower.cu; g++ +
 // tests/native/cuda_cpu_shim.h: tests/test_tower_tail_cpu.py runs this source on the host against float64).
 #pragma once
@@ -32,18 +37,26 @@ inline int grid_for(int64_t M) {
   const int64_t t = (M + kRows - 1) / kRows;
   return (int)(t < 1 ? 1 : (t < kMaxCtas ? t : kMaxCtas));
 }
-inline size_t workspace_bytes(int64_t M, int K, int N) { return (size_t)grid_for(M) * out_len(K, N) * sizeof(float); }
+inline int64_t tiles(int64_t M) { return (M + kRows - 1) / kRows; }
+// workspace: the per-CTA sums [grid][out_len], then (masked mode) the per-tile column sums of dZ [tiles][K]
+inline size_t colsum_offset(int64_t M, int K, int N) { return (size_t)grid_for(M) * out_len(K, N); }
+inline size_t workspace_bytes(int64_t M, int K, int N) {
+  return (colsum_offset(M, K, N) + (size_t)tiles(M) * K) * sizeof(float);
+}
 // shared memory: W1 [NP][KP] | b1 [NP] | w2 [NP] | y1 tile [R][KP + 4] | dh tile [R][NP] | dz*h tile [R][NP] | dz [R] | l [R]
-inline size_t smem_bytes(int KP, int NP) {
-  return ((size_t)NP * KP + 2 * NP + (size_t)kRows * (KP + 4) + 2 * (size_t)kRows * NP + 2 * kRows) * sizeof(float);
+// | masked mode: dZ tile [R][KP + 4]
+inline size_t smem_bytes(int KP, int NP, bool mask) {
+  return ((size_t)NP * KP + 2 * NP + (size_t)(mask ? 2 : 1) * kRows * (KP + 4) + 2 * (size_t)kRows * NP + 2 * kRows) *
+         sizeof(float);
 }
 
-template <int KP, int NP>
+template <int KP, int NP, bool kMask>
 __global__ void __launch_bounds__(kRows)
 tower_tail_bce_kernel(const float* __restrict__ y1, int64_t ld_y, const float* __restrict__ w1,
                       const float* __restrict__ b1, const float* __restrict__ w2, const float* __restrict__ b2,
                       const float* __restrict__ labels, int64_t M, int K, int N, float inv_m, int rows_per_cta,
-                      float* __restrict__ logits, float* __restrict__ dy1, int64_t ld_dy, float* __restrict__ partial) {
+                      float* __restrict__ logits, float* __restrict__ dy1, int64_t ld_dy, float* __restrict__ partial,
+                      float* __restrict__ zsum) {
   constexpr int R = kRows, KC = KP / 4, NC = NP / 4, XS = KP + 4;
   constexpr int NB = (KC * NC + R - 1) / R;          // 4 x 4 blocks of dW1 per thread
   TZK_DYN_SMEM(float, sm);
@@ -55,6 +68,7 @@ tower_tail_bce_kernel(const float* __restrict__ y1, int64_t ld_y, const float* _
   float* Hg = Dh + R * NP;               // [R][NP]
   float* Dz = Hg + R * NP;               // [R]
   float* Ls = Dz + R;                    // [R]
+  float* Zs = Ls + R;                    // [R][XS], masked mode
   const int tid = threadIdx.x;
   for (int i = tid; i < NP * KP; i += R) {
     const int n = i / KP, k = i - n * KP;
@@ -147,6 +161,14 @@ tower_tail_bce_kernel(const float* __restrict__ y1, int64_t ld_y, const float* _
         a.z = fmaf(h[n], w4.z, a.z);
         a.w = fmaf(h[n], w4.w, a.w);
       }
+      if constexpr (kMask) {                      // act_bwd_colsum's predicate: !(y1 > 0), NaN included, gives +0
+        const float4 y4 = *reinterpret_cast<const float4*>(xr + 4 * c);
+        a.x = y4.x > 0.f ? a.x : 0.f;
+        a.y = y4.y > 0.f ? a.y : 0.f;
+        a.z = y4.z > 0.f ? a.z : 0.f;
+        a.w = y4.w > 0.f ? a.w : 0.f;
+        *reinterpret_cast<float4*>(Zs + tid * XS + 4 * c) = a;     // dead rows and columns past K: y1 = 0, so +0
+      }
       if (live && 4 * c < K) {
         float* p = dy1 + row * ld_dy + 4 * c;
         if (vout) {
@@ -190,6 +212,23 @@ tower_tail_bce_kernel(const float* __restrict__ y1, int64_t ld_y, const float* _
       for (int r = 0; r < R; ++r) {
         accz += Dz[r];
         accl += Ls[r];
+      }
+    }
+    if constexpr (kMask) {
+      // column c on thread R - KP + c (past the db1 / dw2 threads, NP <= 64 <= R - KP + c): act_bwd_colsum_kernel's
+      // sums at 64 columns, rows r0, r0 + 4, .. for r0 = 0 .. 3 from +0, then the four in r0 order.  Its slab stops at
+      // M; the dead rows here add +0, which changes no sum (a sum that starts at +0 is never -0).
+      const int c = tid - (R - KP);
+      if (c >= 0 && c < K) {
+        float s[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+        for (int r = 0; r < R; r += 4)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) s[j] += Zs[(r + j) * XS + c];
+        float v = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) v += s[j];
+        zsum[t0 / R * K + c] = v;
       }
     }
     __syncthreads();
@@ -239,11 +278,12 @@ tower_tail_reduce_kernel(const float* __restrict__ partial, int n_parts, int len
 
 inline bool supported(int K, int N) { return K >= 1 && N >= 1 && K <= 64 && N <= 64; }
 
-// out: [N K + 2 N + 2] = dW1 (row-major [N][K]), db1, dw2, db2, loss.  Returns 0, or 1 bad argument / 2 workspace too
+// out: [N K + 2 N + 2] = dW1 (row-major [N][K]), db1, dw2, db2, loss.  mask: masked mode, dy1 receives dZ and the
+// workspace at colsum_offset() the per-tile column sums [tiles(M)][K].  Returns 0, or 1 bad argument / 2 workspace too
 // small / 3 launch failure.
 inline int run(const float* y1, int64_t ld_y, const float* w1, const float* b1, const float* w2, const float* b2,
                const float* labels, int64_t M, int32_t K, int32_t N, float* logits, float* dy1, int64_t ld_dy,
-               float* out, void* workspace, size_t workspace_bytes_, cudaStream_t st) {
+               float* out, void* workspace, size_t workspace_bytes_, cudaStream_t st, bool mask = false) {
   if (M < 1 || !supported(K, N) || !y1 || !w1 || !w2 || !labels || !logits || !dy1 || !out || ld_y < K || ld_dy < K) return 1;
   if (workspace_bytes_ < workspace_bytes(M, K, N)) return 2;
   const int KP = K <= 16 ? 16 : (K <= 32 ? 32 : 64);
@@ -252,30 +292,37 @@ inline int run(const float* y1, int64_t ld_y, const float* w1, const float* b1, 
   int rows_per_cta = (int)((M + grid - 1) / grid);
   rows_per_cta = (rows_per_cta + kRows - 1) / kRows * kRows;        // whole tiles: every CTA but the last is full
   const float inv_m = 1.0f / (float)M;
-  const size_t smem = smem_bytes(KP, NP);
+  const size_t smem = smem_bytes(KP, NP, mask);
   float* partial = static_cast<float*>(workspace);
+  float* zsum = partial + colsum_offset(M, K, N);
 #ifdef TZK_CPU_SHIM
-#define TZK_TAIL_ATTR(KP_, NP_)
+#define TZK_TAIL_ATTR(KP_, NP_, MASK_)
 #else
-#define TZK_TAIL_ATTR(KP_, NP_)                                                                                       \
+#define TZK_TAIL_ATTR(KP_, NP_, MASK_)                                                                                \
   if (smem > 48 * 1024)                                                                                               \
-    cudaFuncSetAttribute(tower_tail_bce_kernel<KP_, NP_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(tower_tail_bce_kernel<KP_, NP_, MASK_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 #endif
-#define TZK_TAIL(KP_, NP_)                                                                                            \
+#define TZK_TAIL(KP_, NP_, MASK_)                                                                                     \
   do {                                                                                                                \
-    TZK_TAIL_ATTR(KP_, NP_)                                                                                           \
-    TZK_LAUNCH((tower_tail_bce_kernel<KP_, NP_>), grid, kRows, smem, st, y1, ld_y, w1, b1, w2, b2, labels, M, K, N,   \
-               inv_m, rows_per_cta, logits, dy1, ld_dy, partial);                                                     \
+    TZK_TAIL_ATTR(KP_, NP_, MASK_)                                                                                    \
+    TZK_LAUNCH((tower_tail_bce_kernel<KP_, NP_, MASK_>), grid, kRows, smem, st, y1, ld_y, w1, b1, w2, b2, labels, M,  \
+               K, N, inv_m, rows_per_cta, logits, dy1, ld_dy, partial, zsum);                                         \
   } while (0)
-#define TZK_TAIL_N(KP_)                                                                                               \
+#define TZK_TAIL_N(KP_, MASK_)                                                                                        \
   do {                                                                                                                \
-    if (NP == 16) TZK_TAIL(KP_, 16);                                                                                  \
-    else if (NP == 32) TZK_TAIL(KP_, 32);                                                                             \
-    else TZK_TAIL(KP_, 64);                                                                                           \
+    if (NP == 16) TZK_TAIL(KP_, 16, MASK_);                                                                           \
+    else if (NP == 32) TZK_TAIL(KP_, 32, MASK_);                                                                      \
+    else TZK_TAIL(KP_, 64, MASK_);                                                                                    \
   } while (0)
-  if (KP == 16) TZK_TAIL_N(16);
-  else if (KP == 32) TZK_TAIL_N(32);
-  else TZK_TAIL_N(64);
+#define TZK_TAIL_K(MASK_)                                                                                             \
+  do {                                                                                                                \
+    if (KP == 16) TZK_TAIL_N(16, MASK_);                                                                              \
+    else if (KP == 32) TZK_TAIL_N(32, MASK_);                                                                         \
+    else TZK_TAIL_N(64, MASK_);                                                                                       \
+  } while (0)
+  if (mask) TZK_TAIL_K(true);
+  else TZK_TAIL_K(false);
+#undef TZK_TAIL_K
 #undef TZK_TAIL_N
 #undef TZK_TAIL
 #undef TZK_TAIL_ATTR

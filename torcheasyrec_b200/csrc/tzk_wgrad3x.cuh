@@ -38,6 +38,7 @@ struct WgParams {
   int64_t slab_rows;   // multiple of 32
   int k_tiles;         // ceil(boxes / 4)
   WgSources src;
+  const float* dz_scale;   // nullable: dZ is read times *dz_scale (interact_wide_wgrad_kernel; wgrad3x_kernel: null)
 };
 
 __device__ __forceinline__ int wg_source(const WgSources& s, int box) {
@@ -168,9 +169,10 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int slabs
 template <auto Kernel = wgrad3x_kernel>
 inline int wgrad3x_launch(const CUtensorMap (&mx)[WG_SRC], const CUtensorMap& mz, const WgSources& src, int64_t M,
                           int32_t slabs, float* partial, float* dw, int64_t ld_dw, cudaStream_t st,
-                          size_t extra_smem = 0) {
+                          size_t extra_smem = 0, const float* dz_scale = nullptr) {
   WgParams p;
   p.partial = partial;
+  p.dz_scale = dz_scale;
   p.M = M;
   p.k_tiles = (src.first[WG_SRC] + 3) / 4;
   p.slab_rows = ((M + slabs - 1) / slabs + WG_ROWS - 1) / WG_ROWS * WG_ROWS;

@@ -320,9 +320,7 @@ class InteractWideFn(torch.autograd.Function):
         from .kernels import default_kernels
 
         dense, sparse = _rows_contig(dense), _rows_contig(sparse)
-        w = torch.zeros((weight.shape[0], 784), dtype=weight.dtype, device=weight.device)
-        for (src, dst, n) in in_map:
-            w[:, dst:dst + n].copy_(weight[:, src:src + n])
+        w = _interact_wide_weight(weight, in_map)
         y, pairs = default_kernels().interact_wide_fwd(dense, sparse, w, bias)
         ctx.in_map, ctx.has_bias = in_map, bias is not None
         ctx.save_for_backward(dense, sparse, pairs, w, y)
@@ -343,6 +341,57 @@ class InteractWideFn(torch.autograd.Function):
         db = colsum if (ctx.has_bias and ctx.needs_input_grad[4]) else None
         return (None, d_dense if ctx.needs_input_grad[1] else None, d_sparse if ctx.needs_input_grad[2] else None, dw, db,
                 None)
+
+
+def _interact_wide_weight(weight: torch.Tensor, in_map) -> torch.Tensor:
+    """[64, 783] -> [64, 784] in the interaction's column layout (column 351 zero)."""
+    w = torch.zeros((weight.shape[0], 784), dtype=weight.dtype, device=weight.device)
+    for (src, dst, n) in in_map:
+        w[:, dst:dst + n].copy_(weight[:, src:src + n])
+    return w
+
+
+class InteractWideTailFn(torch.autograd.Function):
+    """(loss, logits) of InteractWideFn followed by _TowerTailFn, as one autograd node: DLRM-Criteo's interaction, a final
+    MLP of the wide layer and one more Perceptron, the output layer and mean BCE.  The tail kernel stores the wide layer's
+    pre-activation gradient dZ = dy1 * [y1 > 0] and its column sums (the bias gradient) in place of dy1, so dy1 is never
+    scaled by the loss gradient or read back with y1 by act_bwd_colsum; the backward hands the loss gradient to the wide
+    layer's kernels, which scale dZ as they read it.  For loss.backward() the bits of the two nodes; for a loss gradient g,
+    the gradients from dZ are those of dZ * g, and the bias gradient is colsum * g rather than the column sums of dZ * g.
+    d_dense / d_sparse come first, as in InteractWideFn: the sparse update waits on them."""
+
+    @staticmethod
+    def forward(ctx, dense, sparse, weight, bias, in_map, w1, b1, w2, b2, labels):
+        from .functional import _rows_contig
+        from .kernels import default_kernels
+
+        K = default_kernels()
+        dense, sparse = _rows_contig(dense), _rows_contig(sparse)
+        w = _interact_wide_weight(weight, in_map)
+        y1, pairs = K.interact_wide_fwd(dense, sparse, w, bias)
+        loss, logits, dz, dw1, db1, dw2, db2, colsum = K.tower_tail_bce(y1, w1, b1, w2, b2, labels, relu_dz=True)
+        ctx.save_for_backward(dense, sparse, pairs, w, dz, colsum, dw1, db1, dw2, db2)
+        ctx.in_map, ctx.has = in_map, (bias is not None, b1 is not None, b2 is not None)
+        ctx.mark_non_differentiable(logits)
+        return loss, logits
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_logits):
+        from .kernels import default_kernels
+
+        K = default_kernels()
+        dense, sparse, pairs, w, dz, colsum, dw1, db1, dw2, db2 = ctx.saved_tensors
+        g = g_loss.reshape(1)
+        need = ctx.needs_input_grad
+        d_dense = d_sparse = dw = None
+        if need[0] or need[1]:
+            d_dense, d_sparse = K.interact_wide_bwd(dz, w, dense, sparse, scale=g)
+        if need[2]:
+            full = K.interact_wide_wgrad(dz, pairs, dense, sparse, SLABS, scale=g)
+            dw = torch.cat([full[:, dst:dst + n] for (_, dst, n) in ctx.in_map], dim=1)
+        return (d_dense if need[0] else None, d_sparse if need[1] else None, dw,
+                (colsum * g_loss) if (ctx.has[0] and need[3]) else None, None, dw1 * g_loss,
+                (db1 * g_loss) if ctx.has[1] else None, dw2 * g_loss, (db2 * g_loss) if ctx.has[2] else None, None)
 
 
 class InteractBf16Fn(torch.autograd.Function):
@@ -443,7 +492,7 @@ class _TowerTailFn(torch.autograd.Function):
     def forward(ctx, y1, w1, b1, w2, b2, labels):
         from .kernels import default_kernels
 
-        loss, logits, dy1, dw1, db1, dw2, db2 = default_kernels().tower_tail_bce(y1, w1, b1, w2, b2, labels)
+        loss, logits, dy1, dw1, db1, dw2, db2, _ = default_kernels().tower_tail_bce(y1, w1, b1, w2, b2, labels)
         ctx.save_for_backward(dy1, dw1, db1, dw2, db2)
         ctx.has = (b1 is not None, b2 is not None)
         ctx.mark_non_differentiable(logits)
@@ -460,9 +509,19 @@ class _TowerTailFn(torch.autograd.Function):
 def tower_tail_usable(y1: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, labels: torch.Tensor) -> bool:
     """The fused tail covers fp32 CUDA towers ending K -> N (ReLU) -> 1 with K, N <= 64 and a float label per row, with
     autocast off."""
-    return (autocast_dtype(y1) is None and y1.is_cuda and y1.dim() == 2 and y1.dtype == torch.float32 and w1.dtype == torch.float32
-            and w1.shape[1] == y1.shape[1] <= 64 and w1.shape[0] <= 64 and tuple(w2.shape) == (1, w1.shape[0])
-            and labels.dtype == torch.float32 and labels.numel() == y1.shape[0] >= 1 and y1.stride(1) == 1)
+    return (autocast_dtype(y1) is None and y1.is_cuda and y1.dim() == 2 and y1.dtype == torch.float32
+            and y1.stride(1) == 1 and _tail_layers_usable(y1.shape[0], y1.shape[1], w1, w2, labels))
+
+
+def _tail_layers_usable(M: int, K: int, w1: torch.Tensor, w2: torch.Tensor, labels: torch.Tensor) -> bool:
+    return (w1.dtype == torch.float32 and w1.shape[1] == K <= 64 and w1.shape[0] <= 64
+            and tuple(w2.shape) == (1, w1.shape[0]) and labels.dtype == torch.float32 and labels.numel() == M >= 1)
+
+
+def interact_wide_tail_usable(sparse: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, labels: torch.Tensor) -> bool:
+    """Whether InteractWideTailFn covers a wide layer that interact_wide_usable() accepts followed by the fused tail: its
+    output [B, 64] is an fp32 CUDA tensor with contiguous rows, so only the tail's layers and labels are left to check."""
+    return _tail_layers_usable(sparse.shape[0], 64, w1, w2, labels)
 
 
 def tower_tail_bce(y1, w1, b1, w2, b2, labels):

@@ -908,8 +908,9 @@ class CudaKernels:
         return y, pairs
 
     def interact_wide_wgrad(self, dz: torch.Tensor, pairs: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor,
-                            slabs: int) -> torch.Tensor:
-        """dW [64, 784] = dz^T X in the interaction's column layout, X = [pairs | dense | sparse] read in place."""
+                            slabs: int, scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """dW [64, 784] = dz^T X in the interaction's column layout, X = [pairs | dense | sparse] read in place.  `scale`:
+        a one-element fp32 tensor on the device; dz is read times it (the bits of passing dz * scale)."""
         dz, ld_z = _rows2d(dz, "dz")
         pairs, ld_p = _rows2d(pairs, "pairs")
         dense, ld_d = _rows2d(dense, "dense")
@@ -917,14 +918,19 @@ class CudaKernels:
         B = dz.shape[0]
         dw = torch.empty((64, 784), dtype=torch.float32, device=dz.device)
         part = torch.empty(slabs * 896 * 64, dtype=torch.float32, device=dz.device)
-        check(self._lib.tzk_interact_wide_wgrad(_ptr(dz), ld_z, _ptr(pairs), ld_p, _ptr(dense), ld_d, _ptr(sparse), ld_s,
-                                                B, slabs, _ptr(part), _ptr(dw), 784, _stream()), "tzk_interact_wide_wgrad")
+        if scale is not None and _need(scale, torch.float32, "scale").numel() != 1:
+            raise TzkError("scale: expected one element")
+        check(self._lib.tzk_interact_wide_wgrad_scaled(_ptr(dz), ld_z, _ptr(scale), _ptr(pairs), ld_p, _ptr(dense), ld_d,
+                                                       _ptr(sparse), ld_s, B, slabs, _ptr(part), _ptr(dw), 784,
+                                                       _stream()), "tzk_interact_wide_wgrad_scaled")
         self.launches += 2
         return dw
 
-    def interact_wide_bwd(self, dz: torch.Tensor, w: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor):
+    def interact_wide_bwd(self, dz: torch.Tensor, w: torch.Tensor, dense: torch.Tensor, sparse: torch.Tensor,
+                          scale: Optional[torch.Tensor] = None):
         """(d_dense [B, 16], d_sparse [B, 416]) of DLRM-Criteo's interaction followed by a 784 -> 64 layer with weight
-        w [64, 784] (the interaction's column layout), from dz [B, 64], the gradient of the layer's pre-activation."""
+        w [64, 784] (the interaction's column layout), from dz [B, 64], the gradient of the layer's pre-activation.
+        `scale`: as in interact_wide_wgrad."""
         dz, ld_z = _rows2d(dz, "dz")
         w, ld_w = _rows2d(w, "w")
         dense, ld_d = _rows2d(dense, "dense")
@@ -933,9 +939,12 @@ class CudaKernels:
         d_dense = torch.empty((B, 16), dtype=torch.float32, device=dz.device)
         d_sparse = torch.empty((B, 416), dtype=torch.float32, device=dz.device)
         wt = torch.empty((2, 784, 64), dtype=torch.float32, device=dz.device)
-        check(self._lib.tzk_interact_wide_bwd(_ptr(dz), ld_z, _ptr(w), ld_w, _ptr(dense), ld_d, _ptr(sparse), ld_s, B,
-                                              _ptr(d_dense), 16, _ptr(d_sparse), 416, _ptr(wt[0]), _ptr(wt[1]),
-                                              _stream()), "tzk_interact_wide_bwd")
+        if scale is not None and _need(scale, torch.float32, "scale").numel() != 1:
+            raise TzkError("scale: expected one element")
+        check(self._lib.tzk_interact_wide_bwd_scaled(_ptr(dz), ld_z, _ptr(scale), _ptr(w), ld_w, _ptr(dense), ld_d,
+                                                     _ptr(sparse), ld_s, B, _ptr(d_dense), 16, _ptr(d_sparse), 416,
+                                                     _ptr(wt[0]), _ptr(wt[1]), _stream()),
+              "tzk_interact_wide_bwd_scaled")
         self.launches += 2
         return d_dense, d_sparse
 
@@ -1022,9 +1031,10 @@ class CudaKernels:
         return loss, dz
 
     def tower_tail_bce(self, y1: torch.Tensor, w1: torch.Tensor, b1: Optional[torch.Tensor], w2: torch.Tensor,
-                       b2: Optional[torch.Tensor], labels: torch.Tensor):
+                       b2: Optional[torch.Tensor], labels: torch.Tensor, relu_dz: bool = False):
         """Last Perceptron (K -> N, ReLU) + Linear(N, 1) + mean BCE, forward and backward in one pass
-        (csrc/tzk_tower_tail.cuh).  -> (loss [scalar], logits [M], dy1 [M, K], dW1 [N, K], db1 [N], dw2 [1, N], db2 [1])."""
+        (csrc/tzk_tower_tail.cuh).  -> (loss [scalar], logits [M], dy1 [M, K], dW1 [N, K], db1 [N], dw2 [1, N], db2 [1],
+        None).  relu_dz (y1 a ReLU output): dz = dy1 * (y1 > 0) in place of dy1, and its column sums [K] last."""
         y1, ld = _rows2d(y1, "y1")
         _need(w1, torch.float32, "w1")
         _need(w2, torch.float32, "w2")
@@ -1037,15 +1047,16 @@ class CudaKernels:
         logits = torch.empty(M, dtype=torch.float32, device=dev)
         dy1 = torch.empty((M, K), dtype=torch.float32, device=dev)
         out = torch.empty(N * K + 2 * N + 2, dtype=torch.float32, device=dev)
+        colsum = torch.empty(K, dtype=torch.float32, device=dev) if relu_dz else None
         nb = self._lib.tzk_tower_tail_bce_workspace_bytes(M, K, N)
         ws = self._workspace("tail", nb, dev)
         check(self._lib.tzk_tower_tail_bce(_ptr(y1), ld, _ptr(w1), _ptr(b1), _ptr(w2), _ptr(b2), _ptr(labels), M, K, N,
-                                           _ptr(logits), _ptr(dy1), K, _ptr(out), _ptr(ws), ws.numel(), _stream()),
-              "tzk_tower_tail_bce")
-        self.launches += 2
+                                           _ptr(logits), _ptr(dy1), K, _ptr(colsum), _ptr(out), _ptr(ws), ws.numel(),
+                                           _stream()), "tzk_tower_tail_bce")
+        self.launches += 3 if relu_dz else 2
         o = N * K
         return (out[o + 2 * N + 1], logits, dy1, out[:o].view(N, K), out[o:o + N], out[o + N:o + 2 * N].view(1, N),
-                out[o + 2 * N:o + 2 * N + 1])
+                out[o + 2 * N:o + 2 * N + 1], colsum)
 
     def binned_auc_update(self, preds: torch.Tensor, labels: torch.Tensor, thresholds: torch.Tensor,
                           counts: torch.Tensor, invalid: torch.Tensor) -> None:

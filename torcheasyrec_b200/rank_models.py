@@ -445,6 +445,9 @@ class DLRM(RankModel):
         sparse = grouped[self._sparse_group_name]
         if self.dense_mlp and dense_feat is None:
             dense_feat = self.dense_mlp(grouped[self._dense_group_name])
+        fused = self._interact_wide_tail(batch, dense_feat, sparse)
+        if fused is not None:
+            return fused
         x = self._interact_wide(dense_feat, sparse)
         if x is not None:           # the interaction and the first final-MLP layer in one autograd node
             in_map, start = None, 1
@@ -473,14 +476,38 @@ class DLRM(RankModel):
     def _interact_wide(self, dense_feat: Optional[torch.Tensor], sparse: torch.Tensor) -> Optional[torch.Tensor]:
         """Output of the first final-MLP layer computed together with the interaction (dense_gemm.InteractWideFn) when
         the model has DLRM-Criteo's shape and that layer is Linear(783 -> 64) + ReLU; None otherwise."""
-        from .dense_gemm import InteractWideFn, _gemm3x_lib, interact_wide_usable
+        from .dense_gemm import InteractWideFn, _gemm3x_lib
+
+        if not self._interact_wide_ok(dense_feat, sparse):
+            return None
+        first = self.final_mlp.mlp[0].perceptron
+        return InteractWideFn.apply(_gemm3x_lib(), dense_feat, sparse, first[0].weight, first[0].bias, self._WIDE_IN_MAP)
+
+    _WIDE_IN_MAP = ((0, 0, 351), (351, 352, 432))
+
+    def _interact_wide_ok(self, dense_feat: Optional[torch.Tensor], sparse: torch.Tensor) -> bool:
+        from .dense_gemm import interact_wide_usable
 
         first = self.final_mlp.mlp[0].perceptron
-        if not (self._model_config.arch_with_sparse and len(first) == 2 and isinstance(first[1], nn.ReLU)
-                and interact_wide_usable(dense_feat, sparse, first[0].weight, self._sparse_num, self._per_sparse_dim)):
+        return bool(self._model_config.arch_with_sparse and len(first) == 2 and isinstance(first[1], nn.ReLU)
+                    and interact_wide_usable(dense_feat, sparse, first[0].weight, self._sparse_num, self._per_sparse_dim))
+
+    def _interact_wide_tail(self, batch: Batch, dense_feat: Optional[torch.Tensor], sparse: torch.Tensor):
+        """Training steps where the final MLP is the wide layer of _interact_wide and the fused tail's layer (DLRM-Criteo:
+        783 -> 64 -> 32): the interaction, both layers, the output layer and the loss as one autograd node
+        (dense_gemm.InteractWideTailFn), whose tail kernel also does the wide layer's ReLU backward and bias gradient.
+        None when _interact_wide and _fused_tail do not both apply."""
+        from .dense_gemm import InteractWideTailFn, interact_wide_tail_usable
+
+        if len(self.final_mlp.mlp) != 2 or not self._interact_wide_ok(dense_feat, sparse):
             return None
-        in_map = ((0, 0, 351), (351, 352, 432))
-        return InteractWideFn.apply(_gemm3x_lib(), dense_feat, sparse, first[0].weight, first[0].bias, in_map)
+        tail = self._tail_inputs(batch, sparse)
+        if tail is None or not interact_wide_tail_usable(sparse, tail[0], tail[2], tail[4]):
+            return None
+        first = self.final_mlp.mlp[0].perceptron[0]
+        loss, logits = InteractWideTailFn.apply(dense_feat, sparse, first.weight, first.bias, self._WIDE_IN_MAP, *tail)
+        self._tail_loss = loss
+        return {"logits": logits, "probs": torch.sigmoid(logits)}
 
     def _interact_bf16_ok(self, dense_feat: Optional[torch.Tensor], sparse: torch.Tensor) -> bool:
         """DLRM-Criteo's glue under bf16 autocast (dense_gemm.InteractBf16Fn); every other shape or dtype takes the torch
@@ -499,15 +526,10 @@ class DLRM(RankModel):
 
         self._tail_loss = None
         layers = list(self.final_mlp.mlp)
-        if (not self.training or Fn.autocast_dtype(all_feat) is not None or not torch.is_grad_enabled() or not all_feat.is_cuda or self._num_class != 1
-                or not layers or self._label_name not in batch.labels or os.environ.get("TZK_FUSED_TAIL", "1") == "0"):
+        tail = self._tail_inputs(batch, all_feat)
+        if tail is None:
             return None
-        last = layers[-1].perceptron
-        if not (len(last) == 2 and isinstance(last[1], nn.ReLU)):     # Linear -> ReLU only (no BN / LN / dropout)
-            return None
-        label = batch.labels[self._label_name].to(torch.float32)
-        w1, b1 = last[0].weight, last[0].bias
-        w2, b2 = self.output_mlp.weight, self.output_mlp.bias
+        w1, b1, w2, b2, label = tail
         if start >= len(layers):
             return None
         x = all_feat
@@ -521,6 +543,19 @@ class DLRM(RankModel):
         self._tail_loss = loss
         return {"logits": logits, "probs": torch.sigmoid(logits)}
 
+
+    def _tail_inputs(self, batch: Batch, feat: torch.Tensor):
+        """(w1, b1, w2, b2, fp32 label) of the fused tail when this step can take it: a CUDA fp32 training step with
+        gradients, one class, the label in the batch, and a final MLP ending in Linear -> ReLU; None otherwise."""
+        layers = list(self.final_mlp.mlp)
+        if (not self.training or Fn.autocast_dtype(feat) is not None or not torch.is_grad_enabled() or not feat.is_cuda or self._num_class != 1
+                or not layers or self._label_name not in batch.labels or os.environ.get("TZK_FUSED_TAIL", "1") == "0"):
+            return None
+        last = layers[-1].perceptron
+        if not (len(last) == 2 and isinstance(last[1], nn.ReLU)):     # Linear -> ReLU only (no BN / LN / dropout)
+            return None
+        return (last[0].weight, last[0].bias, self.output_mlp.weight, self.output_mlp.bias,
+                batch.labels[self._label_name].to(torch.float32))
 
     def _dense_group_input(self, batch: Batch) -> Optional[torch.Tensor]:
         """[B, 13]-style input of the `dense` group when it consists of raw dense features only (the usual DLRM
