@@ -772,6 +772,48 @@ int tzk_rocket_head_fwd(const tzk_rocket_args* args_host, int32_t grid, float* p
 int tzk_rocket_head_bwd(const tzk_rocket_args* args_host, const float* dlosses, const float* losses, int32_t grid,
                         float* partials, float* dparams, tzk_stream_t stream);
 
+/* ---- TDM's multi-window DIN attention (tzrec/modules/sequence.py MultiWindowDINEncoder.forward, called from
+ * tzrec/models/tdm.py TDM.predict: `self.multiwindow_din(grouped_feature)`), forward and backward over jagged rows.
+ * Sample b owns rows offsets[b] .. offsets[b + 1] of seq [N, C] (offsets [B + 1] int64, offsets[0] = 0,
+ * offsets[B] = N); query [B, Dq], Dq <= C, zero-padded to C.  Per row at position p < S = sum windows:
+ * x = [k, q k, q], h = act(W_l h + b_l) over n_layers attention layers (w[l] [H_l, K_l], K_0 = 3C; act ReLU, or PReLU
+ * with one slope per layer), z = lin_w . h + lin_b, a = PReLU(z; act_w).
+ *   tdm_fwd: out [B, (L + 1) C] = [window_0 .. window_{L-1}, q], window_w = sum_{p in window w} a_p k_p /
+ *            max(min(len - cum_w, W_w), 1); z [N] saved (0 on rows p >= S, which never contribute).
+ *   tdm_bwd: d_out [B, (L + 1) C] -> d_seq [N, C], d_query [B, Dq] and dparams = per layer dW [H][K] | db [H] |
+ *            dslope [PReLU only], then d lin_w [H_last] | d lin_b | d act_w, as per-CTA partials (grid rows; CTA g owns
+ *            samples [B g / grid, B (g + 1) / grid)) reduced in CTA order.  No float atomics.
+ * tdm_smem_bytes: the dynamic shared memory of one CTA (backward != 0: of tdm_bwd) for the description's shapes, or
+ * 0 outside the cover.  The description travels by value as a kernel parameter: graph-capturable. */
+#define TZK_TDM_MAX_LAYERS 3
+#define TZK_TDM_MAX_WINDOWS 32
+#define TZK_TDM_RELU 0
+#define TZK_TDM_PRELU 1
+typedef struct tzk_tdm_args {
+  int64_t B, N;
+  int32_t C, Dq, L, n_layers, act, pad_;
+  int32_t windows[TZK_TDM_MAX_WINDOWS];
+  int32_t hidden[TZK_TDM_MAX_LAYERS];
+  int32_t pad2_;
+  const float* seq;
+  const int64_t* offsets;
+  const float* query;
+  const float* w[TZK_TDM_MAX_LAYERS];
+  const float* b[TZK_TDM_MAX_LAYERS];
+  const float* slope[TZK_TDM_MAX_LAYERS];
+  const float* lin_w;
+  const float* lin_b;
+  const float* act_w;
+  float* out;           /* tdm_fwd */
+  float* z;             /* written by tdm_fwd, read by tdm_bwd */
+  const float* d_out;   /* tdm_bwd only */
+  float* d_seq;         /* tdm_bwd only */
+  float* d_query;       /* tdm_bwd only */
+} tzk_tdm_args;
+int64_t tzk_tdm_smem_bytes(const tzk_tdm_args* args_host, int32_t backward);
+int tzk_tdm_fwd(const tzk_tdm_args* args_host, int32_t grid, tzk_stream_t stream);
+int tzk_tdm_bwd(const tzk_tdm_args* args_host, int32_t grid, float* partials, float* dparams, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

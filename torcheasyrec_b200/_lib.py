@@ -78,6 +78,20 @@ class TzkRocketArgs(ctypes.Structure):
                 ("head", TzkRocketHead * 2), ("pair", TzkRocketPair * ROCKET_MAX_PAIRS)]
 
 
+TDM_MAX_LAYERS, TDM_MAX_WINDOWS, TDM_RELU, TDM_PRELU = 3, 32, 0, 1
+
+
+class TzkTdmArgs(ctypes.Structure):
+    """struct tzk_tdm_args (include/tzk.h): TDM's multi-window DIN attention over jagged rows."""
+
+    _fields_ = [("B", c_int64), ("N", c_int64), ("C", c_int32), ("Dq", c_int32), ("L", c_int32), ("n_layers", c_int32),
+                ("act", c_int32), ("pad_", c_int32), ("windows", c_int32 * TDM_MAX_WINDOWS),
+                ("hidden", c_int32 * TDM_MAX_LAYERS), ("pad2_", c_int32), ("seq", c_void_p), ("offsets", c_void_p),
+                ("query", c_void_p), ("w", c_void_p * TDM_MAX_LAYERS), ("b", c_void_p * TDM_MAX_LAYERS),
+                ("slope", c_void_p * TDM_MAX_LAYERS), ("lin_w", c_void_p), ("lin_b", c_void_p), ("act_w", c_void_p),
+                ("out", c_void_p), ("z", c_void_p), ("d_out", c_void_p), ("d_seq", c_void_p), ("d_query", c_void_p)]
+
+
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
 SIGNATURES = {
     "tzk_abi_version": (c_int32, []),
@@ -250,6 +264,10 @@ SIGNATURES = {
     # RocketLaunching: both output heads, their softmax and every distillation loss (TzkRocketArgs), each direction
     "tzk_rocket_head_fwd": (c_int32, [P, c_int32, P, P, P]),
     "tzk_rocket_head_bwd": (c_int32, [P, P, P, c_int32, P, P, P]),
+    # TDM: the multi-window DIN attention over jagged rows (TzkTdmArgs), each direction
+    "tzk_tdm_smem_bytes": (c_int64, [P, c_int32]),
+    "tzk_tdm_fwd": (c_int32, [P, c_int32, P]),
+    "tzk_tdm_bwd": (c_int32, [P, c_int32, P, P, P]),
 }
 
 _lib = None

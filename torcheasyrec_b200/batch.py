@@ -76,6 +76,18 @@ def _draw_ids(rng: np.random.Generator, rows: int, n: int, dist: str) -> np.ndar
     raise ValueError(dist)
 
 
+def _behaviour_list(name: str, feats: Sequence[BaseFeature]) -> str:
+    """The behaviour list a top-level sequence feature belongs to: `<list>__<field>` names (the reference's naming of a
+    sequence group's fields, e.g. click_50_seq__adgroup_id) share `<list>` with every other top-level sequence feature
+    of that prefix in the data group, so all of them get one length per sample; any other name is a list of its own."""
+    head, sep, _ = name.partition("__")
+    if not sep:
+        return name
+    peers = [f for f in feats
+             if f.is_sparse and f.is_sequence and not f.sequence_name and f.name.startswith(head + "__")]
+    return head + "__" if len(peers) > 1 else name
+
+
 def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Sequence[str], seed: int = 0,
                     id_dist: str = "uniform", seq_len_mix: bool = True,
                     label_cardinality: Optional[Dict[str, int]] = None) -> Batch:
@@ -83,8 +95,8 @@ def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Se
 
     Non-sequence id features get exactly one id per sample (Criteo / Taobao, L=1); grouped sequence features
     draw a length per sample from the mixture {0, 1, U[2,max], max} the reference's mock data uses
-    (tzrec/tests/utils.py:157-182).  Labels are {0, 1} (1 with probability 0.25), except a label named in
-    `label_cardinality`, which is drawn uniformly over [0, cardinality) (e.g. PEPNet's domain label)."""
+    (tzrec/tests/utils.py:157-182), one draw per behaviour list (_behaviour_list).  Labels are {0, 1} (1 with
+    probability 0.25), except a label named in `label_cardinality`, which is drawn uniformly over [0, cardinality) (e.g. PEPNet's domain label)."""
     rng = np.random.default_rng(seed)
     B = batch_size
     by_group: Dict[str, List[BaseFeature]] = {}
@@ -99,7 +111,7 @@ def synthetic_batch(features: Sequence[BaseFeature], batch_size: int, labels: Se
         for f in feats:
             if f.is_sparse:
                 if f.is_sequence:
-                    sname = f.sequence_name or f.name
+                    sname = f.sequence_name or _behaviour_list(f.name, feats)
                     if sname not in seq_lengths:
                         mx = int(f.sequence_length or 50)
                         if seq_len_mix:

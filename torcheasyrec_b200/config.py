@@ -131,7 +131,8 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
          "use_pareto_loss_weight": _f(B, False)},
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
                   "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE",
-                  "pepnet": "PEPNet", "dbmtl": "DBMTL", "rocket_launching": "RocketLaunching"}.get(k, "Generic"))
+                  "pepnet": "PEPNet", "dbmtl": "DBMTL", "rocket_launching": "RocketLaunching",
+                  "tdm": "TDM"}.get(k, "Generic"))
            for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
@@ -171,6 +172,8 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     # feature_distillation_function: a Similarity (simi.proto: COSINE, INNER_PRODUCT, EUCLID)
     "RocketLaunching": {"share_mlp": _f("MLP"), "booster_mlp": _f("MLP"), "light_mlp": _f("MLP"),
                         "feature_based_distillation": _f(B, False), "feature_distillation_function": _f(E, "COSINE")},
+    "TDM": {"multiwindow_din": _f("MultiWindowDINTower"), "final": _f("MLP")},
+    "MultiWindowDINTower": {"windows_len": _f(I, rep=True), "attn_mlp": _f("MLP")},
     "LossConfig": {"binary_cross_entropy": _f("Generic"), "softmax_cross_entropy": _f("SoftmaxCrossEntropy"),
                    "l2_loss": _f("Generic"), "jrc_loss": _f("JRCLoss"), "binary_focal_loss": _f("Generic")},
     "JRCLoss": {"session_name": _f(S), "alpha": _f(F, 0.5)},

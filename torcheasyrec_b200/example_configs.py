@@ -1,6 +1,6 @@
 """Generators for the pipeline configs BASELINE.json names (text format, same message tree as the reference's
 examples/{dlrm_criteo,deepfm_criteo,mmoe_taobao,multi_tower_din_taobao,masknet_criteo,ple_taobao,
-pepnet_taobao,rocket_launching_criteo}.config).
+pepnet_taobao,rocket_launching_criteo,tdm_taobao}.config).
 
 The package does not depend on the reference's files, so the configs are re-derived here from their defining facts
 (SURVEY.md §8 / Appendix D): the Criteo hash sizes, the Taobao table list and price boundaries, and the model
@@ -326,11 +326,68 @@ def rocket_launching_criteo() -> str:
             "    metrics {\n        auc {}\n    }\n    losses {\n        softmax_cross_entropy {}\n    }\n}\n")
 
 
+def tdm_taobao() -> str:
+    """examples/tdm_taobao.config: the Taobao user and item id features (D=16) with the item tables shared by name
+    (item_emb, cate_emb, brand_emb) and the three click_50_seq__{adgroup_id,cate_id,brand} sequence id features (up to
+    50) of one behaviour list; a SEQUENCE group `seq` (the three sequences, queried by adgroup_id, cate_id, brand),
+    DEEP groups `user` and `item`; tdm{multiwindow_din{windows 1,1,1,2,2,2,5,6,10,20, attn_mlp 36 PReLU}, final
+    256-128-64-32 with BN}; a two-class softmax cross-entropy head with auc.  data_config.tdm_sampler configures the
+    reference's tree sampler (data pipeline, not the model)."""
+    adam = "        adam_optimizer {\n            lr: 0.001\n        }\n        constant_learning_rate {\n        }\n"
+    layers = [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 17, 23, 30, 34, 82, 200]
+    attrs = "".join(f'        attr_fields: "{a}"\n' for a in ["cate_id", "campaign_id", "customer", "brand", "price"])
+    head = ('train_input_path: "data/taobao_data_recall_train_transformed/*.parquet"\n'
+            'eval_input_path: "data/taobao_data_recall_eval_transformed/*.parquet"\n'
+            'model_dir: "experiments/tdm_taobao"\n'
+            "train_config {\n    sparse_optimizer {\n" + adam + "    }\n    dense_optimizer {\n" + adam + "    }\n"
+            "    num_epochs: 2\n    log_step_count_steps: 1\n    save_checkpoints_steps: 100000\n}\n"
+            "eval_config {\n}\n"
+            "data_config {\n    batch_size: 32\n    dataset_type: ParquetDataset\n    fg_mode: FG_NONE\n"
+            '    label_fields: "clk"\n    num_workers: 10\n    tdm_sampler {\n'
+            "        item_input_path: 'data/init_tree/node_table.txt'\n"
+            "        edge_input_path: 'data/init_tree/edge_table.txt'\n"
+            "        predict_edge_input_path: 'data/init_tree/predict_edge_table.txt'\n" + attrs +
+            '        item_id_field: "adgroup_id"\n'
+            f"        layer_num_sample: [{', '.join(str(n) for n in layers)}]\n"
+            "        attr_delimiter: ','\n    }\n}\n")
+    user = [(n, r) for n, r in TAOBAO_USER]
+
+    def named(name, side, rows, emb=None):
+        f = _id_feature(name, side, rows)
+        return f if emb is None else f.replace("        embedding_dim: 16\n",
+                                               f'        embedding_dim: 16\n        embedding_name: "{emb}"\n')
+
+    seqs = "".join(
+        "feature_configs {\n    sequence_id_feature {\n"
+        f'        feature_name: "click_50_seq__{n}"\n        sequence_length: 50\n        sequence_delim: ";"\n'
+        f'        expression: "user:click_50_seq__{n}"\n        embedding_dim: 16\n        num_buckets: {r}\n'
+        f'        embedding_name: "{e}"\n    }}\n}}\n'
+        for n, r, e in [("adgroup_id", 1895387, "item_emb"), ("cate_id", 12961, "cate_emb"),
+                        ("brand", 461498, "brand_emb")])
+    feats = ("".join(named(n, "user", r) for n, r in user) + seqs
+             + named("adgroup_id", "item", 1895387, "item_emb") + named("cate_id", "item", 12961, "cate_emb")
+             + named("campaign_id", "item", 423438) + named("customer", "item", 255877)
+             + named("brand", "item", 461498, "brand_emb") + named("price", "item", 100)
+             + _id_feature("pid", "context", 20, field="hash_bucket_size"))
+    seq_names = ["click_50_seq__adgroup_id", "click_50_seq__cate_id", "click_50_seq__brand", "adgroup_id", "cate_id",
+                 "brand"]
+    return (head + feats + "model_config {\n" + _group("seq", seq_names, "SEQUENCE")
+            + _group("user", [n for n, _ in user] + ["pid"], "DEEP")
+            + _group("item", ["campaign_id", "customer", "price"], "DEEP")
+            + "    tdm {\n        multiwindow_din {\n            windows_len: [1, 1, 1, 2, 2, 2, 5, 6, 10, 20]\n"
+            + _mlp("attn_mlp", [36], "            ").replace("hidden_units: [36]\n",
+                                                             "hidden_units: [36]\n                activation: 'nn.PReLU'\n")
+            + "        }\n" + _mlp("final", [256, 128, 64, 32], "        ").replace(
+                "hidden_units: [256, 128, 64, 32]\n", "hidden_units: [256, 128, 64, 32]\n            use_bn: true\n")
+            + "    }\n    num_class: 2\n"
+            "    metrics {\n        auc {}\n    }\n    losses {\n        softmax_cross_entropy {}\n    }\n}\n")
+
+
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
               "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo,
               "ple_taobao": ple_taobao, "pepnet_taobao": pepnet_taobao, "dbmtl_taobao": dbmtl_taobao,
               "dbmtl_taobao_jrc": dbmtl_taobao_jrc, "dbmtl_taobao_seq": dbmtl_taobao_seq,
-              "rocket_launching_criteo": rocket_launching_criteo}
+              "rocket_launching_criteo": rocket_launching_criteo, "tdm_taobao": tdm_taobao}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
 EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}

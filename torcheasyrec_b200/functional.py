@@ -7,6 +7,7 @@ tensors.
 """
 
 import contextlib
+import ctypes
 from typing import List, Optional, Sequence
 
 import torch
@@ -1079,3 +1080,134 @@ def torch_rocket_losses(logits: Sequence[torch.Tensor], labels: torch.Tensor, ep
               F.mse_loss(logits[0], logits[1].detach()) if len(logits) > 1 else None]
     losses += [feature_based_sim(light, booster, sim) for light, booster in pairs]
     return losses
+
+
+# --------------------------------------------------------------------------------------------------------
+# TDM multi-window DIN attention (tzrec/modules/sequence.py MultiWindowDINEncoder; csrc/tzk_tdm.cuh)
+# --------------------------------------------------------------------------------------------------------
+TDM_MAX_C = 128               # csrc/tzk_tdm.cuh: sequence width, a multiple of 4
+TDM_MAX_HIDDEN = 64           # units of one attention layer (two per lane)
+TDM_MAX_LAYERS = 3
+TDM_MAX_WINDOWS = 32
+TDM_MAX_SPAN = 256            # sum of the window lengths
+
+
+def _attn_layers(mlp):
+    """[(linear, activation)] of an attention MLP whose every Perceptron is exactly Linear(bias) + ReLU / one-slope
+    PReLU, with one activation kind throughout; else None."""
+    out = []
+    for p in mlp.mlp:
+        seq = p.perceptron
+        if len(seq) != 2 or seq[0].bias is None:
+            return None
+        act = seq[1]
+        if not (type(act) is torch.nn.ReLU or (type(act) is torch.nn.PReLU and act.weight.numel() == 1)):
+            return None
+        out.append((seq[0], act))
+    if not out or len({type(a) for _, a in out}) != 1:
+        return None
+    return out
+
+
+def multiwindow_din_usable(query: torch.Tensor, seq: torch.Tensor, mlp, windows: Sequence[int]) -> bool:
+    """True when tzk_tdm_fwd / _bwd cover the encoder: fp32 query and rows, autocast and TF32 off, 4 <= C <= 128 with
+    C % 4 == 0, Dq <= C, 1..3 attention layers of at most 64 units with bias and ReLU or one-slope PReLU (no BN, LN or
+    dropout), 1..32 windows of total length <= 256, shared memory within the H100's 227 KB; on CUDA (on the CPU only a
+    test backend that implements the kernels)."""
+    if autocast_dtype(seq) is not None or query.dtype != torch.float32 or seq.dtype != torch.float32:
+        return False
+    C, Dq = seq.shape[1], query.shape[1]
+    if not (4 <= C <= TDM_MAX_C and C % 4 == 0 and Dq <= C):
+        return False
+    layers = _attn_layers(mlp)
+    if layers is None or len(layers) > TDM_MAX_LAYERS or any(l.out_features > TDM_MAX_HIDDEN for l, _ in layers):
+        return False
+    if not 1 <= len(windows) <= TDM_MAX_WINDOWS or min(windows) < 1 or sum(windows) > TDM_MAX_SPAN:
+        return False
+    if seq.is_cuda:
+        if _backend is not None or torch.backends.cuda.matmul.allow_tf32:
+            return False
+        from ._lib import TDM_PRELU, TDM_RELU, TzkTdmArgs, lib
+
+        a = TzkTdmArgs()
+        a.C, a.Dq, a.L, a.n_layers = C, Dq, len(windows), len(layers)
+        a.act = TDM_PRELU if type(layers[0][1]) is torch.nn.PReLU else TDM_RELU
+        for w, n in enumerate(windows):
+            a.windows[w] = int(n)
+        for l, (lin, _) in enumerate(layers):
+            a.hidden[l] = lin.out_features
+        return lib().tzk_tdm_smem_bytes(ctypes.byref(a), 1) > 0
+    return _backend is not None and hasattr(_backend, "tdm_fwd")
+
+
+class _MultiWindowDin(torch.autograd.Function):
+    """MultiWindowDINEncoder's attention, pooling and query block in one tzk_tdm_fwd call; every gradient in one
+    tzk_tdm_bwd call.  params: per layer w, b (and the slope with PReLU), then lin_w, lin_b, act_w."""
+
+    @staticmethod
+    def forward(ctx, spec, query, seq, offsets, *params):
+        windows, prelu, n_layers = spec
+        layers, lin = _tdm_unflatten(params, prelu, n_layers)
+        out, z = backend().tdm_fwd(query, seq, offsets, layers, *lin, windows, prelu)
+        ctx.save_for_backward(query, seq, offsets, z, *params)
+        ctx.spec = spec
+        return out
+
+    @staticmethod
+    def backward(ctx, d_out):
+        windows, prelu, n_layers = ctx.spec
+        query, seq, offsets, z, *params = ctx.saved_tensors
+        layers, lin = _tdm_unflatten(params, prelu, n_layers)
+        d_q, d_seq, grads, d_lw, d_lb, d_aw = backend().tdm_bwd(query, seq, offsets, layers, *lin, windows, prelu, z,
+                                                                d_out.contiguous())
+        out = [None, d_q, d_seq, None]
+        for dw, db, ds in grads:
+            out += [dw, db] + ([ds] if prelu else [])
+        return tuple(out + [d_lw, d_lb, d_aw])
+
+
+def _tdm_unflatten(params, prelu: bool, n_layers: int):
+    per = 3 if prelu else 2
+    layers = [(params[per * l], params[per * l + 1], params[per * l + 2] if prelu else None) for l in range(n_layers)]
+    return layers, params[per * n_layers:]
+
+
+def multiwindow_din(query: torch.Tensor, seq: torch.Tensor, offsets: torch.Tensor, mlp, linear, active,
+                    windows: Sequence[int]) -> torch.Tensor:
+    """[B, (L + 1) C] of MultiWindowDINEncoder over jagged rows seq [N, C] (sample b: rows offsets[b] ..
+    offsets[b + 1]) from one fused call each way.  The caller checks multiwindow_din_usable first."""
+    layers = _attn_layers(mlp)
+    prelu = type(layers[0][1]) is torch.nn.PReLU
+    flat = []
+    for lin, act in layers:
+        flat += [lin.weight, lin.bias] + ([act.weight] if prelu else [])
+    flat += [linear.weight, linear.bias, active.weight]
+    return _MultiWindowDin.apply((tuple(int(w) for w in windows), prelu, len(layers)), query.contiguous(),
+                                 seq.contiguous(), offsets, *[t.contiguous() for t in flat])
+
+
+def torch_multiwindow_din(query: torch.Tensor, seq: torch.Tensor, offsets: torch.Tensor, mlp, linear, active,
+                          windows: Sequence[int]) -> torch.Tensor:
+    """multiwindow_din in torch ops over the same jagged rows (library GEMMs; the path under autocast, on CPU tensors
+    and outside the kernels' cover).  The reference's padded rows give exact zeros and its rows past S are cropped, so
+    over the real rows this is the reference up to the order of the sums."""
+    N, C = seq.shape
+    B = offsets.numel() - 1
+    L, S = len(windows), int(sum(windows))
+    seg = _segments(offsets, N)
+    pos = torch.arange(N, device=seq.device) - offsets[:-1][seg]
+    q = torch.nn.functional.pad(query, (0, C - query.shape[1])) if query.shape[1] < C else query
+    qr = q[seg]
+    a = active(linear(mlp(torch.cat([seq, qr * seq, qr], dim=-1))))           # [N, 1]
+    keep = pos < S
+    win_of = torch.repeat_interleave(torch.arange(L, device=seq.device),
+                                     torch.tensor(list(windows), device=seq.device), output_size=S)
+    idx = seg * L + win_of[pos.clamp(max=S - 1)]
+    att = a * keep.unsqueeze(1) * seq
+    pooled = torch.zeros((B * L, C), dtype=att.dtype, device=seq.device).index_add(0, idx, att)
+    w = torch.tensor(list(windows), device=seq.device)
+    cum = torch.cumsum(w, 0) - w
+    lens = offsets[1:] - offsets[:-1]
+    cnt = torch.clamp(torch.minimum(lens.unsqueeze(1) - cum.unsqueeze(0), w.unsqueeze(0)), min=1)
+    res = pooled.view(B, L, C) / cnt.unsqueeze(2)
+    return torch.cat([res, q.unsqueeze(1).to(res.dtype)], dim=1).reshape(B, -1)

@@ -1451,6 +1451,85 @@ class CudaKernels:
         return dhs, dlights, list(zip(views[0::2], views[1::2]))
 
 
+    # ------------------------------------------------------------------ TDM multi-window DIN (csrc/tzk_tdm.cuh)
+    # Resident CTAs per SM: ptxas register counts (fwd 61 at 256 threads -> 4, bwd 126 at 128 threads -> 4), fewer when
+    # the shapes' shared memory (tzk_tdm_smem_bytes) allows fewer.  The backward grid fixes the order of the parameter
+    # sums and depends only on the batch size, the shapes and the device.
+    def _tdm_args(self, query, seq, offsets, layers, lin_w, lin_b, act_w, windows, prelu: bool):
+        from ._lib import TDM_MAX_LAYERS, TDM_MAX_WINDOWS, TDM_PRELU, TDM_RELU, TzkTdmArgs
+
+        _need(query, torch.float32, "query")
+        _need(seq, torch.float32, "seq")
+        _need(offsets, torch.int64, "offsets")
+        if not 1 <= len(layers) <= TDM_MAX_LAYERS or not 1 <= len(windows) <= TDM_MAX_WINDOWS:
+            raise TzkError(f"tdm: 1..{TDM_MAX_LAYERS} attention layers and 1..{TDM_MAX_WINDOWS} windows")
+        a = TzkTdmArgs()
+        a.B, a.Dq = query.shape
+        a.N, a.C = seq.shape
+        if offsets.numel() != a.B + 1:
+            raise TzkError("tdm: need offsets [B + 1] for query [B, Dq]")
+        a.L, a.n_layers, a.act = len(windows), len(layers), TDM_PRELU if prelu else TDM_RELU
+        for w, n in enumerate(windows):
+            a.windows[w] = int(n)
+        a.seq, a.offsets, a.query = seq.data_ptr(), offsets.data_ptr(), query.data_ptr()
+        K = 3 * a.C
+        for l, (W, b, slope) in enumerate(layers):
+            _need(W, torch.float32, f"w[{l}]")
+            _need(b, torch.float32, f"b[{l}]")
+            if W.dim() != 2 or W.shape[1] != K or b.numel() != W.shape[0]:
+                raise TzkError(f"tdm: layer {l} needs w [H, {K}] and b [H]")
+            a.hidden[l], a.w[l], a.b[l] = W.shape[0], W.data_ptr(), b.data_ptr()
+            if prelu:
+                a.slope[l] = _need(slope, torch.float32, f"slope[{l}]").data_ptr()
+            K = W.shape[0]
+        for t, nm in ((lin_w, "lin_w"), (lin_b, "lin_b"), (act_w, "act_w")):
+            _need(t, torch.float32, nm)
+        if lin_w.numel() != K or lin_b.numel() != 1 or act_w.numel() != 1:
+            raise TzkError("tdm: need lin_w [1, H_last], lin_b [1] and act_w [1]")
+        a.lin_w, a.lin_b, a.act_w = lin_w.data_ptr(), lin_b.data_ptr(), act_w.data_ptr()
+        return a
+
+    def _tdm_grid(self, a, B: int, backward: int) -> int:
+        smem = int(self._lib.tzk_tdm_smem_bytes(ctypes.byref(a), backward))
+        if smem == 0:
+            raise TzkError("tdm: shapes outside the kernels' cover (Fn.multiwindow_din_usable)")
+        per_sm = max(1, min(4, (227 * 1024) // (smem + 1024)))
+        return self._grid(-(-int(B) // 8) if not backward else int(B), per_sm)
+
+    def tdm_fwd(self, query, seq, offsets, layers, lin_w, lin_b, act_w, windows, prelu: bool):
+        """query [B, Dq], seq [N, C] jagged rows, offsets [B + 1] int64, layers [(w [H, K], b [H], slope [1] or
+        None)], lin_w [1, H_last], lin_b [1], act_w [1] -> (out [B, (L + 1) C], z [N])."""
+        a = self._tdm_args(query, seq, offsets, layers, lin_w, lin_b, act_w, windows, prelu)
+        out = torch.empty((a.B, (a.L + 1) * a.C), dtype=torch.float32, device=seq.device)
+        z = torch.empty(a.N, dtype=torch.float32, device=seq.device)
+        a.out, a.z = out.data_ptr(), z.data_ptr()
+        check(self._lib.tzk_tdm_fwd(ctypes.byref(a), self._tdm_grid(a, a.B, 0), _stream()), "tzk_tdm_fwd")
+        self.launches += int(a.B > 0)
+        return out, z
+
+    def tdm_bwd(self, query, seq, offsets, layers, lin_w, lin_b, act_w, windows, prelu: bool, z, d_out):
+        """-> (d_query [B, Dq], d_seq [N, C], [(dw, db, dslope or None)] per layer, d lin_w, d lin_b, d act_w)."""
+        _need(z, torch.float32, "z")
+        _need(d_out, torch.float32, "d_out")
+        a = self._tdm_args(query, seq, offsets, layers, lin_w, lin_b, act_w, windows, prelu)
+        if z.numel() != a.N or tuple(d_out.shape) != (a.B, (a.L + 1) * a.C):
+            raise TzkError("tdm_bwd: need z [N] and d_out [B, (L + 1) C]")
+        d_query, d_seq = torch.empty_like(query), torch.empty_like(seq)
+        a.z, a.d_out, a.d_seq, a.d_query = z.data_ptr(), d_out.data_ptr(), d_seq.data_ptr(), d_query.data_ptr()
+        grid = self._tdm_grid(a, a.B, 1)
+        shapes = []
+        for W, _, _ in layers:
+            shapes += [tuple(W.shape), (W.shape[0],)] + ([(1,)] if prelu else [])
+        shapes += [tuple(lin_w.shape), (1,), (1,)]
+        partials, dparams, views = self._batch_sums("tdm_bwd", grid, shapes, seq.device)
+        check(self._lib.tzk_tdm_bwd(ctypes.byref(a), grid, _ptr(partials), _ptr(dparams), _stream()), "tzk_tdm_bwd")
+        self.launches += 1 + int(a.B > 0)
+        per, grads, o = 3 if prelu else 2, [], 0
+        for _ in layers:
+            grads.append((views[o], views[o + 1], views[o + 2] if prelu else None))
+            o += per
+        return d_query, d_seq, grads, views[o], views[o + 1], views[o + 2]
+
 @dataclass
 class ColPlan:
     """CSR description of a column gather-sum (K6): column c of the destination sums

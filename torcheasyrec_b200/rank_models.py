@@ -12,6 +12,7 @@ import contextlib
 import os
 import struct
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -219,6 +220,56 @@ class DINEncoder(nn.Module):
         padding = torch.ones_like(attn) * (-(2 ** 31) + 1)
         scores = F.softmax(torch.where(mask.unsqueeze(1), attn, padding), dim=-1)
         return torch.matmul(scores, sequence).squeeze(1)
+
+
+class MultiWindowDINEncoder(nn.Module):
+    """tzrec/modules/sequence.py:288-367: target attention ([k, q k, q] through attn_mlp, a Linear and a PReLU) pooled
+    per time window: window w sums a_t k_t over its positions [cum_w, cum_w + W_w) and divides by
+    max(min(len - cum_w, W_w), 1); the output is [window_0 .. window_{L-1}, q zero-padded to C].
+
+    Jagged rows (`<input>.sequence_offsets` present, as TDM asks its group for): one fused call each way when
+    Fn.multiwindow_din_usable holds (csrc/tzk_tdm.cuh), else Fn.torch_multiwindow_din over the same rows.  The padded
+    [B, T, C] form is the reference's formulation."""
+
+    def __init__(self, sequence_dim: int, query_dim: int, input: str, windows_len: List[int],
+                 attn_mlp: Dict[str, Any], **_: Any) -> None:
+        super().__init__()
+        self._query_dim, self._sequence_dim = query_dim, sequence_dim
+        self._windows_len = [int(w) for w in windows_len]
+        if query_dim > sequence_dim:
+            raise ValueError("query_dim > sequence_dim not supported yet.")
+        self.register_buffer("windows_len", torch.tensor(self._windows_len))
+        self.register_buffer("cumsum_windows_len", torch.tensor(np.cumsum([0] + self._windows_len[:-1])))
+        self._sum_windows_len = sum(self._windows_len)
+        self.mlp = MLP(in_features=sequence_dim * 3, dim=3, **attn_mlp)
+        self.linear = nn.Linear(self.mlp.hidden_units[-1], 1)
+        self.active = nn.PReLU()
+        self._q, self._s, self._l = f"{input}.query", f"{input}.sequence", f"{input}.sequence_length"
+
+    def output_dim(self) -> int:
+        return self._sequence_dim * (len(self._windows_len) + 1)
+
+    def forward(self, emb: Dict[str, torch.Tensor]) -> torch.Tensor:
+        query, sequence, seq_len = emb[self._q], emb[self._s], emb[self._l]
+        offsets = emb.get(self._s + "_offsets")
+        if offsets is not None:
+            if Fn.multiwindow_din_usable(query, sequence, self.mlp, self._windows_len):
+                return Fn.multiwindow_din(query, sequence, offsets, self.mlp, self.linear, self.active,
+                                          self._windows_len)
+            return Fn.torch_multiwindow_din(query, sequence, offsets, self.mlp, self.linear, self.active,
+                                            self._windows_len)
+        T = sequence.size(1)
+        mask = torch.arange(T, device=seq_len.device).unsqueeze(0) < seq_len.unsqueeze(1)
+        if self._query_dim < self._sequence_dim:
+            query = F.pad(query, (0, self._sequence_dim - self._query_dim))
+        queries = query.unsqueeze(1).expand(-1, T, -1)
+        attn = self.active(self.linear(self.mlp(torch.cat([sequence, queries * sequence, queries], dim=-1))))
+        att_sequences = attn * mask.unsqueeze(2) * sequence
+        pad = F.pad(att_sequences, (0, 0, 0, self._sum_windows_len - T)).transpose(0, 1)
+        result = torch.segment_reduce(pad, reduce="sum", lengths=self.windows_len, axis=0).transpose(0, 1)
+        segment_length = torch.min(seq_len.unsqueeze(1) - self.cumsum_windows_len.unsqueeze(0), self.windows_len)
+        result = result / torch.max(segment_length, torch.ones_like(segment_length)).unsqueeze(2)
+        return torch.cat([result, query.unsqueeze(1)], dim=1).reshape(result.shape[0], -1)
 
 
 def _create_seq_encoder(seq_encoder_config: Message, group_total_dim: Dict[str, int]) -> nn.Module:
@@ -1547,9 +1598,44 @@ class RocketLaunching(RankModel):
         return heads if self.training else heads[1:]
 
 
+class TDM(RankModel):
+    """tzrec/models/tdm.py:28-105: the SEQUENCE group through MultiWindowDINEncoder, concatenated with the other
+    groups in config order, then deep_mlp and output_mlp (num_class outputs; the example trains a two-class softmax
+    cross-entropy head with auc on probs1).  The SEQUENCE group always hands its rows over jagged.  The tree sampler,
+    tree construction and retrieval of the reference's TDM live in its data pipeline and are not part of the model."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self.init_input()
+        eg = self.embedding_group
+        non_seq_fea_dim = 0
+        self.seq_group_name = ""
+        self.non_seq_group_name = []
+        for fg in self._base_model_config.feature_groups:
+            if eg.group_type(fg.group_name) == "SEQUENCE":
+                self.seq_group_name = fg.group_name
+            else:
+                non_seq_fea_dim += eg.group_total_dim(fg.group_name)
+                self.non_seq_group_name.append(fg.group_name)
+        g = self.seq_group_name
+        eg.set_jagged_for_attention([g])
+        cfg = self._model_config.multiwindow_din
+        self.multiwindow_din = MultiWindowDINEncoder(eg.group_total_dim(f"{g}.sequence"),
+                                                     eg.group_total_dim(f"{g}.query"), g, list(cfg.windows_len),
+                                                     config_to_kwargs(cfg.attn_mlp))
+        self.deep_mlp = MLP(in_features=self.multiwindow_din.output_dim() + non_seq_fea_dim,
+                            **config_to_kwargs(self._model_config.final))
+        self.output_mlp = nn.Linear(self.deep_mlp.output_dim(), self._num_class)
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        grouped = self.build_input(batch)
+        x = torch.cat([self.multiwindow_din(grouped)] + [grouped[n] for n in self.non_seq_group_name], dim=1)
+        return self._output_to_prediction(self.output_mlp(self.deep_mlp(x)))
+
+
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
                  "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE,
-                 "pepnet": PEPNet, "dbmtl": DBMTL, "rocket_launching": RocketLaunching}
+                 "pepnet": PEPNet, "dbmtl": DBMTL, "rocket_launching": RocketLaunching, "tdm": TDM}
 
 
 class JRCLoss(nn.Module):
