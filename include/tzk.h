@@ -814,6 +814,42 @@ int64_t tzk_tdm_smem_bytes(const tzk_tdm_args* args_host, int32_t backward);
 int tzk_tdm_fwd(const tzk_tdm_args* args_host, int32_t grid, tzk_stream_t stream);
 int tzk_tdm_bwd(const tzk_tdm_args* args_host, int32_t grid, float* partials, float* dparams, tzk_stream_t stream);
 
+/* ---- DCN-v2's low-rank cross network (tzrec/modules/interaction.py CrossV2.forward, called from
+ * tzrec/models/dcn_v2.py DCNV2.predict: `net = self.cross(net)`), forward and backward.  Per layer l < L:
+ *   v_l = U_l x_l (U_l = u_kernels[l].weight [r, D]), w_l = V_l v_l + c_l (V_l = v_kernels[l].weight [D, r],
+ *   c_l = v_kernels[l].bias [D]), x_{l+1} = x0 * w_l + x_l;  y = x_L.
+ * The tile products run on the tensor cores with the 3xTF32 split (fp32-level results).  Every call first splits the
+ * weights it needs into hi / lo TF32 MMA fragments, zero-padded to r8 = r rounded up to 8 and D8 = D rounded up to 8,
+ * in `work` (8 L r8 D8 floats, 16-B aligned).
+ *   dcn_v2_fwd:         x0 [B, D] -> y [B, D] and the saved v [B, L r].
+ *   dcn_v2_bwd_data:    x0, v, dy [B, D] -> dx0 [B, D] and dv [B, L r] (dv_l = d v_l).
+ *   dcn_v2_bwd_weight:  x0, v, dv, dy -> dparams = dU [L, r, D] | dV [L, D, r] | dc [L, D], as per-chunk partials
+ *                       (`chunks` rows; chunk k owns the k-th of `chunks` equal runs of 64-row batch tiles) reduced in
+ *                       chunk order.  No float atomics.
+ * dcn_v2_smem_bytes: the dynamic shared memory of one CTA of pass 0 (fwd), 1 (bwd_data) or 2 (bwd_weight) for the
+ * description's shapes, or 0 outside the cover (1 <= L <= 8, 1 <= r <= 64, 1 <= D <= 512).  The description travels
+ * by value as a kernel parameter: graph-capturable. */
+#define TZK_DCN_V2_MAX_LAYERS 8
+typedef struct tzk_dcn_v2_args {
+  int64_t B;
+  int32_t D, L, r, pad_;
+  const float* x0;
+  const float* wu;      /* [L, r, D] */
+  const float* wv;      /* [L, D, r] */
+  const float* bias;    /* [L, D] */
+  float* work;          /* 8 L r8 D8 floats */
+  float* y;             /* dcn_v2_fwd */
+  float* v;             /* written by dcn_v2_fwd, read by both backward passes */
+  const float* dy;      /* backward */
+  float* dx0;           /* dcn_v2_bwd_data */
+  float* dv;            /* written by dcn_v2_bwd_data, read by dcn_v2_bwd_weight */
+} tzk_dcn_v2_args;
+int64_t tzk_dcn_v2_smem_bytes(const tzk_dcn_v2_args* args_host, int32_t pass);
+int tzk_dcn_v2_fwd(const tzk_dcn_v2_args* args_host, int32_t grid, tzk_stream_t stream);
+int tzk_dcn_v2_bwd_data(const tzk_dcn_v2_args* args_host, int32_t grid, tzk_stream_t stream);
+int tzk_dcn_v2_bwd_weight(const tzk_dcn_v2_args* args_host, int32_t chunks, float* partials, float* dparams,
+                          tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -92,6 +92,17 @@ class TzkTdmArgs(ctypes.Structure):
                 ("out", c_void_p), ("z", c_void_p), ("d_out", c_void_p), ("d_seq", c_void_p), ("d_query", c_void_p)]
 
 
+DCN_V2_MAX_LAYERS = 8
+
+
+class TzkDcnV2Args(ctypes.Structure):
+    """struct tzk_dcn_v2_args (include/tzk.h): DCN-v2's low-rank cross network."""
+
+    _fields_ = [("B", c_int64), ("D", c_int32), ("L", c_int32), ("r", c_int32), ("pad_", c_int32), ("x0", c_void_p),
+                ("wu", c_void_p), ("wv", c_void_p), ("bias", c_void_p), ("work", c_void_p), ("y", c_void_p),
+                ("v", c_void_p), ("dy", c_void_p), ("dx0", c_void_p), ("dv", c_void_p)]
+
+
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
 SIGNATURES = {
     "tzk_abi_version": (c_int32, []),
@@ -268,6 +279,11 @@ SIGNATURES = {
     "tzk_tdm_smem_bytes": (c_int64, [P, c_int32]),
     "tzk_tdm_fwd": (c_int32, [P, c_int32, P]),
     "tzk_tdm_bwd": (c_int32, [P, c_int32, P, P, P]),
+    # DCN-v2: the low-rank cross network (TzkDcnV2Args), forward, input gradient and weight gradient
+    "tzk_dcn_v2_smem_bytes": (c_int64, [P, c_int32]),
+    "tzk_dcn_v2_fwd": (c_int32, [P, c_int32, P]),
+    "tzk_dcn_v2_bwd_data": (c_int32, [P, c_int32, P]),
+    "tzk_dcn_v2_bwd_weight": (c_int32, [P, c_int32, P, P, P]),
 }
 
 _lib = None

@@ -132,7 +132,7 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
         **{k: _f({"dlrm": "DLRM", "deepfm": "DeepFM", "mmoe": "MMoE", "multi_tower_din": "MultiTowerDIN",
                   "multi_tower": "MultiTower", "wukong": "WuKong", "mask_net": "MaskNet", "ple": "PLE",
                   "pepnet": "PEPNet", "dbmtl": "DBMTL", "rocket_launching": "RocketLaunching",
-                  "tdm": "TDM"}.get(k, "Generic"))
+                  "tdm": "TDM", "dcn_v2": "DCNV2"}.get(k, "Generic"))
            for k in _MODEL_KINDS}),
     "FeatureGroupConfig": {"group_name": _f(S), "feature_names": _f(S, rep=True), "group_type": _f(E, "DEEP"),
                            "sequence_groups": _f("SeqGroupConfig", rep=True),
@@ -174,6 +174,8 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
                         "feature_based_distillation": _f(B, False), "feature_distillation_function": _f(E, "COSINE")},
     "TDM": {"multiwindow_din": _f("MultiWindowDINTower"), "final": _f("MLP")},
     "MultiWindowDINTower": {"windows_len": _f(I, rep=True), "attn_mlp": _f("MLP")},
+    "DCNV2": {"backbone": _f("MLP"), "cross": _f("CrossV2"), "deep": _f("MLP"), "final": _f("MLP")},
+    "CrossV2": {"cross_num": _f(I, 3), "low_rank": _f(I, 32)},
     "LossConfig": {"binary_cross_entropy": _f("Generic"), "softmax_cross_entropy": _f("SoftmaxCrossEntropy"),
                    "l2_loss": _f("Generic"), "jrc_loss": _f("JRCLoss"), "binary_focal_loss": _f("Generic")},
     "JRCLoss": {"session_name": _f(S), "alpha": _f(F, 0.5)},

@@ -383,6 +383,22 @@ def tdm_taobao() -> str:
             "    metrics {\n        auc {}\n    }\n    losses {\n        softmax_cross_entropy {}\n    }\n}\n")
 
 
+def dcn_v2_taobao() -> str:
+    """examples/multi_tower_taobao.config with ONE edit: its model_config replaced by the dcn_v2 example of the
+    reference's docs/source/models/dcn_v2.md (the reference ships no DCN-v2 example file).  The 16 Taobao features
+    (16 wide each, D = 256) in one DEEP group `features`; backbone 512-256-128, so the cross network runs at D = 128
+    with cross_num 2 and low_rank 32; deep 512-256 on the raw group; final 128-32; auc and binary cross-entropy."""
+    return (_header("taobao_multitask_sample_v1_train", "taobao_multitask_sample_v1/ds=20170513",
+                    "multi_tower_taobao", "FG_DAG", ["clk"], None, quota=False)
+            + _taobao_features()
+            + "model_config {\n" + _group("features", TAOBAO_MMOE_ORDER, "DEEP")
+            + "    dcn_v2 {\n" + _mlp("backbone", [512, 256, 128], "        ")
+            + "        cross {\n            cross_num: 2\n            low_rank: 32\n        }\n"
+            + _mlp("deep", [512, 256], "        ") + _mlp("final", [128, 32], "        ")
+            + "    }\n    num_class: 1\n"
+            "    metrics {\n        auc {}\n    }\n    losses {\n        binary_cross_entropy {}\n    }\n}\n")
+
+
 GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_taobao": mmoe_taobao,
               "multi_tower_din_taobao": multi_tower_din_taobao, "masknet_criteo": masknet_criteo,
               "ple_taobao": ple_taobao, "pepnet_taobao": pepnet_taobao, "dbmtl_taobao": dbmtl_taobao,
@@ -390,7 +406,7 @@ GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_
               "rocket_launching_criteo": rocket_launching_criteo, "tdm_taobao": tdm_taobao}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
-EDITED_GENERATORS = {"wukong_criteo": wukong_criteo}
+EDITED_GENERATORS = {"wukong_criteo": wukong_criteo, "dcn_v2_taobao": dcn_v2_taobao}
 # every built-in config by name (engine.Pipeline resolves names here)
 BUILTINS = {**GENERATORS, **EDITED_GENERATORS}
 

@@ -1211,3 +1211,76 @@ def torch_multiwindow_din(query: torch.Tensor, seq: torch.Tensor, offsets: torch
     cnt = torch.clamp(torch.minimum(lens.unsqueeze(1) - cum.unsqueeze(0), w.unsqueeze(0)), min=1)
     res = pooled.view(B, L, C) / cnt.unsqueeze(2)
     return torch.cat([res, q.unsqueeze(1).to(res.dtype)], dim=1).reshape(B, -1)
+
+
+# --------------------------------------------------------------------------------------------------------
+# DCN-v2 low-rank cross network (tzrec/modules/interaction.py CrossV2; csrc/tzk_dcn_v2.cuh)
+# --------------------------------------------------------------------------------------------------------
+DCN_V2_MAX_D = 512            # csrc/tzk_dcn_v2.cuh: input width
+DCN_V2_MAX_RANK = 64
+DCN_V2_MAX_LAYERS = 8
+# The model takes the fused path up to D r = 8192 (256 x 32, 128 x 64, 33 x 64).  The kernels accept up to 512 x 64,
+# but on an H100 at B = 65536 the torch loop's library GEMMs beat them at D 256, L 3, r 64 (DESIGN.md §8), so wider
+# products stay on the torch path.
+DCN_V2_MAX_DR = 8192
+
+
+def cross_v2_usable(x: torch.Tensor, u_kernels, v_kernels) -> bool:
+    """True when tzk_dcn_v2_fwd / _bwd_data / _bwd_weight cover the cross network: fp32 input and weights, autocast and
+    TF32 off, 1 <= D <= 512, 1 <= L <= 8, 1 <= r <= 64 with D r <= DCN_V2_MAX_DR, every v kernel with its bias, shared
+    memory within the H100's 227 KB; on CUDA (on the CPU only a test backend that implements the kernels)."""
+    if autocast_dtype(x) is not None or x.dtype != torch.float32 or x.dim() != 2:
+        return False
+    L = len(u_kernels)
+    if not 1 <= L <= DCN_V2_MAX_LAYERS or len(v_kernels) != L:
+        return False
+    D, r = x.shape[1], u_kernels[0].out_features
+    if not (1 <= D <= DCN_V2_MAX_D and 1 <= r <= DCN_V2_MAX_RANK and D * r <= DCN_V2_MAX_DR):
+        return False
+    for u, v in zip(u_kernels, v_kernels):
+        if u.weight.dtype != torch.float32 or v.weight.dtype != torch.float32 or v.bias is None:
+            return False
+        if tuple(u.weight.shape) != (r, D) or tuple(v.weight.shape) != (D, r):
+            return False
+    if x.is_cuda:
+        if _backend is not None or torch.backends.cuda.matmul.allow_tf32:
+            return False
+        from ._lib import TzkDcnV2Args, lib
+
+        a = TzkDcnV2Args()
+        a.D, a.L, a.r = D, L, r
+        return all(lib().tzk_dcn_v2_smem_bytes(ctypes.byref(a), p) > 0 for p in range(3))
+    return _backend is not None and hasattr(_backend, "dcn_v2_fwd")
+
+
+class _CrossV2(torch.autograd.Function):
+    """The whole cross network in one tzk_dcn_v2_fwd call; dx0 and every weight gradient from tzk_dcn_v2_bwd_data and
+    tzk_dcn_v2_bwd_weight.  Saves x0, the weights and v [B, L r] only."""
+
+    @staticmethod
+    def forward(ctx, x0, wu, wv, bias):
+        y, v = backend().dcn_v2_fwd(x0, wu, wv, bias)
+        ctx.save_for_backward(x0, wu, wv, bias, v)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x0, wu, wv, bias, v = ctx.saved_tensors
+        return backend().dcn_v2_bwd(x0, wu, wv, bias, v, dy.contiguous())
+
+
+def cross_v2(x: torch.Tensor, u_kernels, v_kernels) -> torch.Tensor:
+    """x_L of CrossV2 from one fused call each way.  The caller checks cross_v2_usable first."""
+    wu = torch.stack([u.weight for u in u_kernels])
+    wv = torch.stack([v.weight for v in v_kernels])
+    bias = torch.stack([v.bias for v in v_kernels])
+    return _CrossV2.apply(x.contiguous(), wu, wv, bias)
+
+
+def torch_cross_v2(x: torch.Tensor, u_kernels, v_kernels) -> torch.Tensor:
+    """CrossV2.forward of the reference in torch ops (the path on CPU tensors, under autocast, with TF32 on and outside
+    the kernels' cover)."""
+    x_l = x
+    for u, v in zip(u_kernels, v_kernels):
+        x_l = x * v(u(x_l)) + x_l
+    return x_l

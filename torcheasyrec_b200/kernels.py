@@ -1530,6 +1530,70 @@ class CudaKernels:
             o += per
         return d_query, d_seq, grads, views[o], views[o + 1], views[o + 2]
 
+    # ------------------------------------------------------------------ DCN-v2 cross network (csrc/tzk_dcn_v2.cuh)
+    # fwd and bwd_data run CTAs of up to 4 warps over 64-row groups: resident CTAs per SM from the shapes' shared
+    # memory (tzk_dcn_v2_smem_bytes) and the ptxas register counts (at most 168 registers at 128 threads -> 3).
+    # bwd_weight runs (32-column block) x (batch chunk) CTAs of 4 warps (at most 222 registers -> 2 per SM); the chunk
+    # count fixes the order of the parameter sums and depends only on the batch size, the shapes and the device.
+    def _dcn_v2_args(self, x0, wu, wv, bias):
+        from ._lib import TzkDcnV2Args
+
+        _need(x0, torch.float32, "x0")
+        for t, nm in ((wu, "wu"), (wv, "wv"), (bias, "bias")):
+            _need(t, torch.float32, nm)
+        a = TzkDcnV2Args()
+        a.B, a.D = x0.shape
+        a.L, a.r = wu.shape[0], wu.shape[1]
+        if tuple(wu.shape) != (a.L, a.r, a.D) or tuple(wv.shape) != (a.L, a.D, a.r) or tuple(bias.shape) != (a.L, a.D):
+            raise TzkError("dcn_v2: need x0 [B, D], wu [L, r, D], wv [L, D, r] and bias [L, D]")
+        a.x0, a.wu, a.wv, a.bias = x0.data_ptr(), wu.data_ptr(), wv.data_ptr(), bias.data_ptr()
+        r8, d8 = -(-a.r // 8) * 8, -(-a.D // 8) * 8
+        work = self._workspace("dcn_v2_work", 8 * a.L * r8 * d8 * 4, x0.device)
+        a.work = work.data_ptr()
+        return a
+
+    def _dcn_v2_smem(self, a, pass_: int) -> int:
+        smem = int(self._lib.tzk_dcn_v2_smem_bytes(ctypes.byref(a), pass_))
+        if smem == 0:
+            raise TzkError("dcn_v2: shapes outside the kernels' cover (Fn.cross_v2_usable)")
+        return smem
+
+    def _dcn_v2_tile_grid(self, a, pass_: int) -> int:
+        per_sm = max(1, min(3, (227 * 1024) // (self._dcn_v2_smem(a, pass_) + 1024)))
+        return self._grid(-(-int(a.B) // 64), per_sm)
+
+    def dcn_v2_fwd(self, x0, wu, wv, bias):
+        """x0 [B, D], wu [L, r, D], wv [L, D, r], bias [L, D] -> (y [B, D], v [B, L r])."""
+        a = self._dcn_v2_args(x0, wu, wv, bias)
+        y = torch.empty_like(x0)
+        v = torch.empty((a.B, a.L * a.r), dtype=torch.float32, device=x0.device)
+        a.y, a.v = y.data_ptr(), v.data_ptr()
+        check(self._lib.tzk_dcn_v2_fwd(ctypes.byref(a), self._dcn_v2_tile_grid(a, 0), _stream()), "tzk_dcn_v2_fwd")
+        self.launches += 2 * int(a.B > 0)
+        return y, v
+
+    def dcn_v2_bwd(self, x0, wu, wv, bias, v, dy):
+        """-> (dx0 [B, D], d wu [L, r, D], d wv [L, D, r], d bias [L, D]) from the saved v and dy = d y."""
+        _need(v, torch.float32, "v")
+        _need(dy, torch.float32, "dy")
+        a = self._dcn_v2_args(x0, wu, wv, bias)
+        if tuple(v.shape) != (a.B, a.L * a.r) or tuple(dy.shape) != (a.B, a.D):
+            raise TzkError("dcn_v2_bwd: need v [B, L r] and dy [B, D]")
+        dx0 = torch.empty_like(x0)
+        dv = torch.empty_like(v)
+        a.v, a.dy, a.dx0, a.dv = v.data_ptr(), dy.data_ptr(), dx0.data_ptr(), dv.data_ptr()
+        check(self._lib.tzk_dcn_v2_bwd_data(ctypes.byref(a), self._dcn_v2_tile_grid(a, 1), _stream()),
+              "tzk_dcn_v2_bwd_data")
+        blocks = -(-a.D // 32)
+        per_sm = max(1, min(2, (227 * 1024) // (self._dcn_v2_smem(a, 2) + 1024)))
+        chunks = self._grid(-(-int(a.B) // 64), per_sm, blocks)
+        shapes = [tuple(wu.shape), tuple(wv.shape), tuple(bias.shape)]
+        partials, dparams, views = self._batch_sums("dcn_v2_bwd", chunks, shapes, x0.device)
+        check(self._lib.tzk_dcn_v2_bwd_weight(ctypes.byref(a), chunks, _ptr(partials), _ptr(dparams), _stream()),
+              "tzk_dcn_v2_bwd_weight")
+        self.launches += 1 + 5 * int(a.B > 0)
+        return dx0, views[0], views[1], views[2]
+
 @dataclass
 class ColPlan:
     """CSR description of a column gather-sum (K6): column c of the destination sums

@@ -1633,9 +1633,65 @@ class TDM(RankModel):
         return self._output_to_prediction(self.output_mlp(self.deep_mlp(x)))
 
 
+class CrossV2(nn.Module):
+    """tzrec/modules/interaction.py:135-180: the low-rank cross network, x_{l+1} = x0 * v_l(u_l(x_l)) + x_l with
+    u_kernels[l] = Linear(D, r, bias=False) and v_kernels[l] = Linear(r, D).  One fused call each way on the GPU
+    (Fn.cross_v2) when Fn.cross_v2_usable holds; else the reference's loop (Fn.torch_cross_v2)."""
+
+    def __init__(self, input_dim: int, cross_num: int = 3, low_rank: int = 32) -> None:
+        super().__init__()
+        self.cross_num = cross_num
+        self._low_rank = low_rank
+        self._input_dim = input_dim
+        self.u_kernels = nn.ModuleList([nn.Linear(input_dim, low_rank, bias=False) for _ in range(cross_num)])
+        self.v_kernels = nn.ModuleList([nn.Linear(low_rank, input_dim, bias=True) for _ in range(cross_num)])
+
+    def output_dim(self) -> int:
+        return self._input_dim
+
+    def forward(self, input: torch.Tensor) -> torch.Tensor:
+        if Fn.cross_v2_usable(input, self.u_kernels, self.v_kernels):
+            return Fn.cross_v2(input, self.u_kernels, self.v_kernels)
+        return Fn.torch_cross_v2(input, self.u_kernels, self.v_kernels)
+
+
+class DCNV2(RankModel):
+    """tzrec/models/dcn_v2.py:26-88: the first feature group through an optional backbone MLP and the cross network,
+    concatenated with an optional deep MLP on the raw group, then final and a bias-less output Linear."""
+
+    def __init__(self, model_config, features, labels, sample_weights=None, **kwargs) -> None:
+        super().__init__(model_config, features, labels, sample_weights, **kwargs)
+        self.init_input()
+        self.group_name = self.embedding_group.group_names()[0]
+        feature_dim = self.embedding_group.group_total_dim(self.group_name)
+        cfg = self._model_config
+        self.backbone = None
+        if cfg.HasField("backbone"):
+            self.backbone = MLP(in_features=feature_dim, **config_to_kwargs(cfg.backbone))
+            feature_dim = self.backbone.output_dim()
+        self.cross = CrossV2(input_dim=feature_dim, **config_to_kwargs(cfg.cross))
+        final_input_dim = self.cross.output_dim()
+        self.deep = None
+        if cfg.HasField("deep"):
+            self.deep = MLP(in_features=self.embedding_group.group_total_dim(self.group_name),
+                            **config_to_kwargs(cfg.deep))
+            final_input_dim += self.deep.output_dim()
+        self.final = MLP(in_features=final_input_dim, **config_to_kwargs(cfg.final))
+        self.output_mlp = nn.Linear(self.final.output_dim(), self._num_class, bias=False)
+
+    def predict(self, batch: Batch) -> Dict[str, torch.Tensor]:
+        features = self.build_input(batch)[self.group_name]
+        net = self.backbone(features) if self.backbone else features
+        net = self.cross(net)
+        if self.deep:
+            net = torch.cat([net, self.deep(features)], dim=-1)
+        return self._output_to_prediction(self.output_mlp(self.final(net)))
+
+
 MODEL_CLASSES = {"dlrm": DLRM, "deepfm": DeepFM, "multi_tower_din": MultiTowerDIN, "multi_tower": MultiTower,
                  "mmoe": MMoE, "wukong": WuKong, "mask_net": MaskNet, "ple": PLE,
-                 "pepnet": PEPNet, "dbmtl": DBMTL, "rocket_launching": RocketLaunching, "tdm": TDM}
+                 "pepnet": PEPNet, "dbmtl": DBMTL, "rocket_launching": RocketLaunching, "tdm": TDM,
+                 "dcn_v2": DCNV2}
 
 
 class JRCLoss(nn.Module):
