@@ -850,6 +850,52 @@ int tzk_dcn_v2_bwd_data(const tzk_dcn_v2_args* args_host, int32_t grid, tzk_stre
 int tzk_dcn_v2_bwd_weight(const tzk_dcn_v2_args* args_host, int32_t chunks, float* partials, float* dparams,
                           tzk_stream_t stream);
 
+/* ---- SelfAttentionEncoder's attention core (tzrec/modules/sequence.py SelfAttentionEncoder.forward: the
+ * nn.MultiheadAttention of the in-projected rows, summed over the sequence), forward and backward over jagged rows.
+ * Sample b owns rows offsets[b] .. offsets[b + 1] (offsets [B + 1] int64, offsets[0] = 0, offsets[B] = N) of the
+ * in-projected q, k, v [N, E] (E = H hd, row strides ldq / ldk / ldv floats); the first L_b = min(len_b, max_len) rows
+ * are kept (max_len 0: all).  Per head h over the kept rows: s_ij = (q_i sqrt(1/hd)) . k_j, p = softmax over j.
+ *   self_attn_pool_fwd:  pooled [B, E], pooled[b, h] = sum_i sum_j p_ij v_j; lse [N, H] = one log-sum-exp per kept row
+ *                        and head (0 on cropped rows).
+ *   self_attn_pool_bwd:  d_pooled [B, E] -> dq, dk, dv [N, E] (contiguous; 0 on cropped rows), with the workspace
+ *                        dsum [N, H] (D_i = sum_j p_ij u_j, u_j = g . v_j).
+ * One CTA per (sample, head) work item at a time, grid-stride: every item writes only its own outputs, so the bits do not
+ * depend on the grid.  No float atomics, no host read of any length: graph-capturable.
+ * seq_attn_smem_bytes: the dynamic shared memory of one CTA, or 0 outside the cover (1 <= hd <= 128).
+ *
+ * PoolingEncoder over jagged rows: out [B, D] = sum (mean: / max(L_b, 1)) of the first L_b rows of seq [N, D];
+ * jagged_pool_bwd writes d_seq [N, D] = d_out (mean: / max(L_b, 1)) on kept rows and 0 on cropped rows. */
+typedef struct tzk_seq_attn_args {
+  int64_t B, N;
+  int32_t H, hd, max_len, pad_;
+  int64_t ldq, ldk, ldv;
+  const int64_t* offsets;
+  const float* q;
+  const float* k;
+  const float* v;
+  float* pooled;         /* self_attn_pool_fwd */
+  float* lse;            /* written by self_attn_pool_fwd, read by self_attn_pool_bwd */
+  const float* d_pooled; /* self_attn_pool_bwd only */
+  float* dq;             /* self_attn_pool_bwd only */
+  float* dk;             /* self_attn_pool_bwd only */
+  float* dv;             /* self_attn_pool_bwd only */
+  float* dsum;           /* self_attn_pool_bwd workspace [N, H] */
+} tzk_seq_attn_args;
+int64_t tzk_seq_attn_smem_bytes(const tzk_seq_attn_args* args_host);
+int tzk_self_attn_pool_fwd(const tzk_seq_attn_args* args_host, int32_t grid, tzk_stream_t stream);
+int tzk_self_attn_pool_bwd(const tzk_seq_attn_args* args_host, int32_t grid, tzk_stream_t stream);
+typedef struct tzk_jagged_pool_args {
+  int64_t B, N;
+  int32_t D, max_len, mean, pad_;
+  const int64_t* offsets;
+  const float* seq;      /* jagged_pool_fwd */
+  float* out;            /* jagged_pool_fwd */
+  const float* d_out;    /* jagged_pool_bwd */
+  float* d_seq;          /* jagged_pool_bwd */
+} tzk_jagged_pool_args;
+int tzk_jagged_pool_fwd(const tzk_jagged_pool_args* args_host, int32_t grid, tzk_stream_t stream);
+int tzk_jagged_pool_bwd(const tzk_jagged_pool_args* args_host, int32_t grid, tzk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -103,6 +103,23 @@ class TzkDcnV2Args(ctypes.Structure):
                 ("v", c_void_p), ("dy", c_void_p), ("dx0", c_void_p), ("dv", c_void_p)]
 
 
+class TzkSeqAttnArgs(ctypes.Structure):
+    """struct tzk_seq_attn_args (include/tzk.h): SelfAttentionEncoder's attention core over jagged rows."""
+
+    _fields_ = [("B", c_int64), ("N", c_int64), ("H", c_int32), ("hd", c_int32), ("max_len", c_int32),
+                ("pad_", c_int32), ("ldq", c_int64), ("ldk", c_int64), ("ldv", c_int64), ("offsets", c_void_p),
+                ("q", c_void_p), ("k", c_void_p), ("v", c_void_p), ("pooled", c_void_p), ("lse", c_void_p),
+                ("d_pooled", c_void_p), ("dq", c_void_p), ("dk", c_void_p), ("dv", c_void_p), ("dsum", c_void_p)]
+
+
+class TzkJaggedPoolArgs(ctypes.Structure):
+    """struct tzk_jagged_pool_args (include/tzk.h): PoolingEncoder over jagged rows."""
+
+    _fields_ = [("B", c_int64), ("N", c_int64), ("D", c_int32), ("max_len", c_int32), ("mean", c_int32),
+                ("pad_", c_int32), ("offsets", c_void_p), ("seq", c_void_p), ("out", c_void_p), ("d_out", c_void_p),
+                ("d_seq", c_void_p)]
+
+
 # name -> (restype, argtypes); mirrors include/tzk.h one to one (tests/test_abi.py checks both directions)
 SIGNATURES = {
     "tzk_abi_version": (c_int32, []),
@@ -284,6 +301,13 @@ SIGNATURES = {
     "tzk_dcn_v2_fwd": (c_int32, [P, c_int32, P]),
     "tzk_dcn_v2_bwd_data": (c_int32, [P, c_int32, P]),
     "tzk_dcn_v2_bwd_weight": (c_int32, [P, c_int32, P, P, P]),
+    # sequence encoders of DEEP groups: the self-attention core (TzkSeqAttnArgs) and the pooling encoder
+    # (TzkJaggedPoolArgs) over jagged rows, each direction
+    "tzk_seq_attn_smem_bytes": (c_int64, [P]),
+    "tzk_self_attn_pool_fwd": (c_int32, [P, c_int32, P]),
+    "tzk_self_attn_pool_bwd": (c_int32, [P, c_int32, P]),
+    "tzk_jagged_pool_fwd": (c_int32, [P, c_int32, P]),
+    "tzk_jagged_pool_bwd": (c_int32, [P, c_int32, P]),
 }
 
 _lib = None

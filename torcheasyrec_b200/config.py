@@ -181,9 +181,13 @@ SCHEMA: Dict[str, Dict[str, Tuple[str, bool, Any]]] = {
     "JRCLoss": {"session_name": _f(S), "alpha": _f(F, 0.5)},
     "SoftmaxCrossEntropy": {"label_smoothing": _f(F, 0.0)},
     "SeqEncoderConfig": {"din_encoder": _f("DINEncoder"), "simple_attention": _f("Generic"),
-                         "pooling_encoder": _f("Generic"), "multi_window_din_encoder": _f("Generic"),
-                         "self_attention_encoder": _f("Generic")},
+                         "pooling_encoder": _f("PoolingEncoder"), "multi_window_din_encoder": _f("MultiWindowDINEncoder"),
+                         "self_attention_encoder": _f("SelfAttentionEncoder")},
     "DINEncoder": {"name": _f(S), "input": _f(S), "attn_mlp": _f("MLP"), "max_seq_length": _f(I, 0)},
+    "PoolingEncoder": {"name": _f(S), "input": _f(S), "pooling_type": _f(S, "mean"), "max_seq_length": _f(I, 0)},
+    "SelfAttentionEncoder": {"name": _f(S), "input": _f(S), "multihead_attn_dim": _f(I, 512), "num_heads": _f(I, 8),
+                             "dropout": _f(F, 0.0), "max_seq_length": _f(I, 0)},
+    "MultiWindowDINEncoder": {"name": _f(S), "input": _f(S), "attn_mlp": _f("MLP"), "windows_len": _f(I, rep=True)},
     "MetricConfig": {"auc": _f("AUC"), "multiclass_auc": _f("Generic"), "recall_at_k": _f("Generic"),
                      "mean_absolute_error": _f("Generic"), "mean_squared_error": _f("Generic"),
                      "accuracy": _f("Generic"), "grouped_auc": _f("Generic")},

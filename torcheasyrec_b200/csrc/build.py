@@ -10,9 +10,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["tzk_core.cu", "tzk_gather.cu", "tzk_bwd.cu", "tzk_dist.cu", "tzk_dense.cu", "tzk_tower.cu", "tzk_din.cu", "tzk_peer.cu", "tzk_interact_wide.cu",
            "tzk_interact_bf16.cu", "tzk_metrics.cu", "tzk_wukong.cu",
-           "tzk_masknet.cu", "tzk_ple.cu", "tzk_pepnet.cu", "tzk_jrc.cu", "tzk_rocket.cu", "tzk_tdm.cu", "tzk_dcn_v2.cu"]
+           "tzk_masknet.cu", "tzk_ple.cu", "tzk_pepnet.cu", "tzk_jrc.cu", "tzk_rocket.cu", "tzk_tdm.cu", "tzk_dcn_v2.cu",
+           "tzk_seq_attn.cu"]
 HEADERS = ["tzk_common.cuh", "tzk_tower_bwd2.cuh", "tzk_interact_tc.cuh", "tzk_tower_tail.cuh", "tzk_interact_bf16.cuh",
            "tzk_metrics.cuh", "tzk_wukong.cuh", "tzk_masknet.cuh", "tzk_ple.cuh", "tzk_pepnet.cuh", "tzk_jrc.cuh", "tzk_rocket.cuh", "tzk_tdm.cuh", "tzk_dcn_v2.cuh",
+           "tzk_seq_attn.cuh",
            "tzk_launch.cuh",
            "tzk_batch_sum.cuh",
 "tzk_sm90_ptx.h", "tzk_tma.h", "tzk_wgrad3x.cuh", "tzk_wgmma.cuh", os.path.join("..", "..", "include", "tzk.h")]

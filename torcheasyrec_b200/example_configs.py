@@ -310,6 +310,20 @@ def dbmtl_taobao_seq() -> str:
             + _dbmtl_towers(10000, "binary_cross_entropy {}") + "    }\n}\n")
 
 
+def dbmtl_taobao_seq_encoders() -> str:
+    """dbmtl_taobao_seq with two more encoders on click_50_seq beside its DIN encoder: `self_attention_encoder {}` (512
+    dims, 8 heads) and `pooling_encoder { pooling_type: "mean" }`.  The edit: the reference ships no example with these
+    encoders in a DEEP group."""
+    extra = ("        sequence_encoders {\n            self_attention_encoder {\n            }\n        }\n"
+             "        sequence_encoders {\n            pooling_encoder {\n"
+             '                pooling_type: "mean"\n            }\n        }\n')
+    text = dbmtl_taobao_seq()
+    end = text.index("    dbmtl {\n")
+    head = text[:end]
+    close = head.rindex("    }\n")
+    return (head[:close] + extra + head[close:] + text[end:]).replace('dbmtl_seq"', 'dbmtl_seq_encoders"')
+
+
 def rocket_launching_criteo() -> str:
     """examples/rocket_launching_criteo.config: dlrm_criteo's features in one DEEP group `deep` (13 raw + 26 id(D=16),
     429 wide); rocket_launching{booster 256-128-64-32, light 96-64-32, feature_based_distillation}; a two-class head
@@ -406,7 +420,8 @@ GENERATORS = {"dlrm_criteo": dlrm_criteo, "deepfm_criteo": deepfm_criteo, "mmoe_
               "rocket_launching_criteo": rocket_launching_criteo, "tdm_taobao": tdm_taobao}
 # built-in configs that differ from their reference example by a documented edit (each generator's docstring names it),
 # so they are not in GENERATORS, whose every entry parses to the same tree as the reference's file
-EDITED_GENERATORS = {"wukong_criteo": wukong_criteo, "dcn_v2_taobao": dcn_v2_taobao}
+EDITED_GENERATORS = {"wukong_criteo": wukong_criteo, "dcn_v2_taobao": dcn_v2_taobao,
+                     "dbmtl_taobao_seq_encoders": dbmtl_taobao_seq_encoders}
 # every built-in config by name (engine.Pipeline resolves names here)
 BUILTINS = {**GENERATORS, **EDITED_GENERATORS}
 

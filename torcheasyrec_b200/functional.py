@@ -8,6 +8,7 @@ tensors.
 
 import contextlib
 import ctypes
+import math
 from typing import List, Optional, Sequence
 
 import torch
@@ -1284,3 +1285,123 @@ def torch_cross_v2(x: torch.Tensor, u_kernels, v_kernels) -> torch.Tensor:
     for u, v in zip(u_kernels, v_kernels):
         x_l = x * v(u(x_l)) + x_l
     return x_l
+
+
+# --------------------------------------------------------------------------------------------------------
+# sequence encoders of DEEP groups (tzrec/modules/sequence.py SelfAttentionEncoder / PoolingEncoder;
+# csrc/tzk_seq_attn.cuh)
+# --------------------------------------------------------------------------------------------------------
+SELF_ATTN_MAX_HD = 128        # csrc/tzk_seq_attn.cuh: head width
+
+
+def self_attn_pool_usable(q: torch.Tensor, H: int, dropout: float, training: bool) -> bool:
+    """True when tzk_self_attn_pool_fwd / _bwd cover the attention: fp32 rows, autocast off, 1 <= hd <= 128, no dropout
+    in training (torch's dropout RNG cannot be matched); on CUDA (on the CPU only a test backend that implements the
+    kernels)."""
+    if autocast_dtype(q) is not None or q.dtype != torch.float32 or q.dim() != 2 or H < 1 or q.shape[1] % H != 0:
+        return False
+    if not 1 <= q.shape[1] // H <= SELF_ATTN_MAX_HD or (dropout > 0.0 and training):
+        return False
+    if q.is_cuda:
+        return _backend is None
+    return _backend is not None and hasattr(_backend, "self_attn_pool_fwd")
+
+
+class _SelfAttnPool(torch.autograd.Function):
+    """The attention core in one tzk_self_attn_pool_fwd call (saves the lse [N, H] only); dq, dk, dv in one
+    tzk_self_attn_pool_bwd call."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, offsets, H, max_len):
+        pooled, lse = backend().self_attn_pool_fwd(q, k, v, offsets, H, max_len)
+        ctx.save_for_backward(q, k, v, offsets, lse)
+        ctx.spec = (H, max_len)
+        return pooled
+
+    @staticmethod
+    def backward(ctx, d_pooled):
+        q, k, v, offsets, lse = ctx.saved_tensors
+        dq, dk, dv = backend().self_attn_pool_bwd(q, k, v, offsets, *ctx.spec, lse, d_pooled.contiguous())
+        return dq, dk, dv, None, None, None
+
+
+def self_attn_pool(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, offsets: torch.Tensor, H: int,
+                   max_len: int = 0) -> torch.Tensor:
+    """pooled [B, E]: per sample b and head, sum_i sum_j p_ij v_j over the first L_b = min(len_b, max_len) rows (0:
+    all) of the in-projected jagged rows q, k, v [N, E], p = softmax_j((q_i sqrt(1/hd)) . k_j).  One fused call each
+    way; the caller checks self_attn_pool_usable first."""
+    return _SelfAttnPool.apply(q.contiguous(), k.contiguous(), v.contiguous(), offsets, int(H), int(max_len))
+
+
+def torch_self_attn_pool(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, offsets: torch.Tensor, H: int,
+                         max_len: int = 0, dropout: float = 0.0, training: bool = False) -> torch.Tensor:
+    """self_attn_pool in torch ops (the path under autocast, on CPU tensors, with dropout in training and outside the
+    kernels' cover): the kept rows padded to the batch's longest kept length (one host read), every key beyond a
+    sample's length masked, and every padded query row's probabilities zeroed after the softmax, so no row is NaN and
+    every gradient is finite.  `dropout` applies to the attention probabilities, as in nn.MultiheadAttention."""
+    N, E = q.shape
+    B, hd = offsets.numel() - 1, E // H
+    lens = offsets[1:] - offsets[:-1]
+    kept = torch.clamp_max(lens, max_len) if max_len > 0 else lens
+    T = int(kept.max()) if B > 0 else 0
+    seg = _segments(offsets, N)
+    pos = torch.arange(N, device=q.device) - offsets[:-1][seg]
+    keep = pos < kept[seg]
+    idx = seg[keep] * max(T, 1) + pos[keep]
+
+    def pad(x):
+        out = torch.zeros((B * max(T, 1), E), dtype=x.dtype, device=x.device).index_copy(0, idx, x[keep])
+        return out.view(B, max(T, 1), H, hd).transpose(1, 2)                    # [B, H, T, hd]
+
+    qp, kp, vp = pad(q) * math.sqrt(1.0 / hd), pad(k), pad(v)
+    valid = torch.arange(max(T, 1), device=q.device).unsqueeze(0) < kept.unsqueeze(1)          # [B, T]
+    s = torch.matmul(qp, kp.transpose(-1, -2)).masked_fill(~valid[:, None, None, :], torch.finfo(qp.dtype).min)
+    p = torch.softmax(s, dim=-1) * valid[:, None, :, None].to(qp.dtype)
+    if dropout > 0.0 and training:
+        p = torch.nn.functional.dropout(p, dropout, True)
+    c = p.sum(dim=-2)                                                           # [B, H, T]
+    return torch.matmul(c.unsqueeze(-2), vp).reshape(B, E)
+
+
+def jagged_pool_usable(seq: torch.Tensor) -> bool:
+    """True when tzk_jagged_pool_fwd / _bwd take the pooling: fp32 rows, autocast off; on CUDA (on the CPU only a test
+    backend that implements the kernels)."""
+    if autocast_dtype(seq) is not None or seq.dtype != torch.float32 or seq.dim() != 2:
+        return False
+    if seq.is_cuda:
+        return _backend is None
+    return _backend is not None and hasattr(_backend, "jagged_pool_fwd")
+
+
+class _JaggedPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seq, offsets, max_len, mean):
+        ctx.save_for_backward(offsets)
+        ctx.spec = (seq.shape[0], max_len, mean)
+        return backend().jagged_pool_fwd(seq, offsets, max_len, mean)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        offsets, = ctx.saved_tensors
+        N, max_len, mean = ctx.spec
+        return backend().jagged_pool_bwd(d_out.contiguous(), offsets, N, max_len, mean), None, None, None
+
+
+def jagged_pool(seq: torch.Tensor, offsets: torch.Tensor, max_len: int = 0, mean: bool = True) -> torch.Tensor:
+    """[B, D]: the sum, or the mean over max(L_b, 1), of each sample's first L_b = min(len_b, max_len) rows (0: all)
+    of jagged rows seq [N, D], one fused call each way.  The caller checks jagged_pool_usable first."""
+    return _JaggedPool.apply(seq.contiguous(), offsets, int(max_len), bool(mean))
+
+
+def torch_jagged_pool(seq: torch.Tensor, offsets: torch.Tensor, max_len: int = 0, mean: bool = True) -> torch.Tensor:
+    """jagged_pool in torch ops over the same rows (index_add into the samples; no host read)."""
+    N, B = seq.shape[0], offsets.numel() - 1
+    seg = _segments(offsets, N)
+    lens = offsets[1:] - offsets[:-1]
+    rows = seq
+    if max_len > 0:
+        pos = torch.arange(N, device=seq.device) - offsets[:-1][seg]
+        rows = seq * (pos < max_len).unsqueeze(1).to(seq.dtype)
+        lens = torch.clamp_max(lens, max_len)
+    out = torch.zeros((B, seq.shape[1]), dtype=seq.dtype, device=seq.device).index_add(0, seg, rows)
+    return out / torch.clamp_min(lens, 1).unsqueeze(1).to(out.dtype) if mean else out

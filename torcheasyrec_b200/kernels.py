@@ -1594,6 +1594,95 @@ class CudaKernels:
         self.launches += 1 + 5 * int(a.B > 0)
         return dx0, views[0], views[1], views[2]
 
+    # ------------------------------------------------------------------ sequence encoders (csrc/tzk_seq_attn.cuh)
+    # The attention core runs one CTA of 256 threads per (sample, head) item at a time, grid-stride; resident CTAs per
+    # SM from the ptxas register counts (fwd 100 -> 2, bwd up to 168 -> 1) and the shared memory of hd.  Every item
+    # writes only its own outputs, so the grid changes no bits.
+    def _seq_attn_args(self, q, k, v, offsets, H: int, max_len: int):
+        from ._lib import TzkSeqAttnArgs
+
+        for t, nm in ((q, "q"), (k, "k"), (v, "v")):
+            _need(t, torch.float32, nm)
+        _need(offsets, torch.int64, "offsets")
+        a = TzkSeqAttnArgs()
+        a.N, E = q.shape
+        a.B, a.H, a.max_len = offsets.numel() - 1, int(H), int(max_len)
+        if a.B < 0 or H < 1 or E % H != 0 or q.dim() != 2 or tuple(k.shape) != (a.N, E) or tuple(v.shape) != (a.N, E):
+            raise TzkError("self_attn_pool: need q, k, v [N, H hd] and offsets [B + 1]")
+        a.hd = E // H
+        a.ldq = a.ldk = a.ldv = E
+        a.offsets, a.q, a.k, a.v = offsets.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr()
+        return a
+
+    def _seq_attn_grid(self, a, backward: bool) -> int:
+        smem = int(self._lib.tzk_seq_attn_smem_bytes(ctypes.byref(a)))
+        if smem == 0:
+            raise TzkError("self_attn_pool: shapes outside the kernels' cover (Fn.self_attn_pool_usable)")
+        per_sm = max(1, min(1 if backward else 2, (227 * 1024) // (smem + 1024)))
+        return self._grid(int(a.B) * int(a.H), per_sm)
+
+    def self_attn_pool_fwd(self, q, k, v, offsets, H: int, max_len: int):
+        """q, k, v [N, E], offsets [B + 1] int64 -> (pooled [B, E], lse [N, H])."""
+        a = self._seq_attn_args(q, k, v, offsets, H, max_len)
+        pooled = torch.empty((a.B, a.H * a.hd), dtype=torch.float32, device=q.device)
+        lse = torch.empty((a.N, a.H), dtype=torch.float32, device=q.device)
+        a.pooled, a.lse = pooled.data_ptr(), lse.data_ptr()
+        check(self._lib.tzk_self_attn_pool_fwd(ctypes.byref(a), self._seq_attn_grid(a, False), _stream()),
+              "tzk_self_attn_pool_fwd")
+        self.launches += int(a.B > 0)
+        return pooled, lse
+
+    def self_attn_pool_bwd(self, q, k, v, offsets, H: int, max_len: int, lse, d_pooled):
+        """-> (dq, dk, dv [N, E]) from the saved lse [N, H] and d_pooled [B, E]."""
+        _need(lse, torch.float32, "lse")
+        _need(d_pooled, torch.float32, "d_pooled")
+        a = self._seq_attn_args(q, k, v, offsets, H, max_len)
+        E = a.H * a.hd
+        if tuple(lse.shape) != (a.N, a.H) or tuple(d_pooled.shape) != (a.B, E):
+            raise TzkError("self_attn_pool_bwd: need lse [N, H] and d_pooled [B, E]")
+        dq, dk, dv = (torch.empty((a.N, E), dtype=torch.float32, device=q.device) for _ in range(3))
+        dsum = self._workspace("self_attn_pool_dsum", max(a.N * a.H, 1) * 4, q.device)
+        a.lse, a.d_pooled, a.dsum = lse.data_ptr(), d_pooled.data_ptr(), dsum.data_ptr()
+        a.dq, a.dk, a.dv = dq.data_ptr(), dk.data_ptr(), dv.data_ptr()
+        check(self._lib.tzk_self_attn_pool_bwd(ctypes.byref(a), self._seq_attn_grid(a, True), _stream()),
+              "tzk_self_attn_pool_bwd")
+        self.launches += int(a.B > 0)
+        return dq, dk, dv
+
+    def _jagged_pool_args(self, offsets, D: int, max_len: int, mean: bool):
+        from ._lib import TzkJaggedPoolArgs
+
+        _need(offsets, torch.int64, "offsets")
+        a = TzkJaggedPoolArgs()
+        a.B, a.D, a.max_len, a.mean = offsets.numel() - 1, int(D), int(max_len), int(bool(mean))
+        a.offsets = offsets.data_ptr()
+        return a
+
+    def jagged_pool_fwd(self, seq, offsets, max_len: int, mean: bool):
+        """seq [N, D] jagged rows -> out [B, D]: the sum (mean: over max(kept rows, 1)) of each sample's first
+        max_len rows (0: all)."""
+        _need(seq, torch.float32, "seq")
+        a = self._jagged_pool_args(offsets, seq.shape[1], max_len, mean)
+        a.N = seq.shape[0]
+        out = torch.empty((a.B, a.D), dtype=torch.float32, device=seq.device)
+        a.seq, a.out = seq.data_ptr(), out.data_ptr()
+        check(self._lib.tzk_jagged_pool_fwd(ctypes.byref(a), self._grid(-(-max(a.B, 1) // 8), 8), _stream()),
+              "tzk_jagged_pool_fwd")
+        self.launches += int(a.B > 0)
+        return out
+
+    def jagged_pool_bwd(self, d_out, offsets, N: int, max_len: int, mean: bool):
+        """d_out [B, D] -> d_seq [N, D] (0 on cropped rows)."""
+        _need(d_out, torch.float32, "d_out")
+        a = self._jagged_pool_args(offsets, d_out.shape[1], max_len, mean)
+        a.N = int(N)
+        d_seq = torch.empty((a.N, a.D), dtype=torch.float32, device=d_out.device)
+        a.d_out, a.d_seq = d_out.data_ptr(), d_seq.data_ptr()
+        check(self._lib.tzk_jagged_pool_bwd(ctypes.byref(a), self._grid(-(-max(a.B, 1) // 8), 8), _stream()),
+              "tzk_jagged_pool_bwd")
+        self.launches += int(a.B > 0)
+        return d_seq
+
 @dataclass
 class ColPlan:
     """CSR description of a column gather-sum (K6): column c of the destination sums

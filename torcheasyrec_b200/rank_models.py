@@ -272,17 +272,127 @@ class MultiWindowDINEncoder(nn.Module):
         return torch.cat([result, query.unsqueeze(1)], dim=1).reshape(result.shape[0], -1)
 
 
+class PoolingEncoder(nn.Module):
+    """tzrec/modules/sequence.py:174-218: the sum, or the mean over max(min(len, max_seq_length), 1), of the first
+    max_seq_length rows (0: all).  Jagged rows: tzk_jagged_pool_fwd / _bwd (csrc/tzk_seq_attn.cuh) when
+    Fn.jagged_pool_usable holds, else Fn.torch_jagged_pool; the padded [B, T, D] form is the reference's formulation."""
+
+    def __init__(self, sequence_dim: int, input: str, pooling_type: str = "mean", max_seq_length: int = 0,
+                 **_: Any) -> None:
+        super().__init__()
+        assert pooling_type in ["sum", "mean"], "only sum|mean pooling type supported now."
+        self._sequence_dim, self._pooling_type, self._max_seq_length = sequence_dim, pooling_type, max_seq_length
+        self._s, self._l = f"{input}.sequence", f"{input}.sequence_length"
+
+    def output_dim(self) -> int:
+        return self._sequence_dim
+
+    def forward(self, emb: Dict[str, torch.Tensor]) -> torch.Tensor:
+        sequence = emb[self._s]
+        offsets = emb.get(self._s + "_offsets")
+        mean = self._pooling_type == "mean"
+        if offsets is not None:
+            if Fn.jagged_pool_usable(sequence):
+                return Fn.jagged_pool(sequence, offsets, self._max_seq_length, mean)
+            return Fn.torch_jagged_pool(sequence, offsets, self._max_seq_length, mean)
+        if self._max_seq_length > 0:
+            sequence = sequence[:, : self._max_seq_length, :]
+        feature = torch.sum(sequence, dim=1)
+        if mean:
+            seq_len = emb[self._l]
+            if self._max_seq_length > 0:
+                seq_len = torch.clamp_max(seq_len, self._max_seq_length)
+            feature = feature / torch.clamp_min(seq_len, 1).unsqueeze(1)
+        return feature
+
+
+def _attention_mask(sequence: torch.Tensor, num_heads: int, sequence_length: torch.Tensor) -> torch.Tensor:
+    """tzrec/modules/sequence.py:34-46: [B H, T, T], True where query or key is beyond the sample's length."""
+    B, T, _ = sequence.size()
+    mask = torch.arange(T, device=sequence_length.device).unsqueeze(0).expand(B, T)
+    mask = (mask < sequence_length.unsqueeze(1)).int()
+    mask = ~(torch.multiply(mask.unsqueeze(2), mask.unsqueeze(1)).type(torch.bool))
+    return mask.repeat_interleave(repeats=num_heads, dim=0)
+
+
+class SelfAttentionEncoder(nn.Module):
+    """tzrec/modules/sequence.py:221-285: Q / K / V Linears, an nn.MultiheadAttention over the sequence, its output rows
+    summed and divided by max(len, 1).  State-dict keys are the reference's.
+
+    Jagged rows (`<input>.sequence_offsets` present): the Linears and the three in-projections run over the N rows, the
+    attention core is Fn.self_attn_pool (csrc/tzk_seq_attn.cuh) when Fn.self_attn_pool_usable holds, else
+    Fn.torch_self_attn_pool, and out_proj runs once per sample after pooling:
+        out = (pooled Wo^T + L_b bo) / max(len_b, 1),   L_b = min(len_b, max_seq_length)
+    (the reference's padded rows give 0, not the bias, after nan_to_num; it divides by the uncropped length).  Its
+    padded query rows see every key masked, so their softmax is NaN and every parameter gradient of the padded form is
+    NaN whenever lengths differ in the batch; over jagged rows no row is all-masked and the gradients are finite.
+    The padded [B, T, D] form (TZK_DIN_JAGGED=0) is the reference's formulation verbatim, NaN gradients included."""
+
+    def __init__(self, sequence_dim: int, input: str, multihead_attn_dim: int, num_heads: int = 8,
+                 dropout: float = 0.0, max_seq_length: int = 0, **_: Any) -> None:
+        super().__init__()
+        self._sequence_dim, self._max_seq_length = sequence_dim, max_seq_length
+        self._num_heads, self._multihead_attn_dim, self._dropout = num_heads, multihead_attn_dim, float(dropout)
+        self._head_dim = multihead_attn_dim // num_heads
+        assert self._head_dim * num_heads == multihead_attn_dim, "multihead_attn_dim must be divisible by num_heads"
+        self._query = nn.Linear(sequence_dim, multihead_attn_dim)
+        self._key = nn.Linear(sequence_dim, multihead_attn_dim)
+        self._value = nn.Linear(sequence_dim, multihead_attn_dim)
+        self._multihead_attn = nn.MultiheadAttention(multihead_attn_dim, num_heads=num_heads, dropout=dropout,
+                                                     batch_first=True)
+        self._s, self._l = f"{input}.sequence", f"{input}.sequence_length"
+
+    def output_dim(self) -> int:
+        return self._multihead_attn_dim
+
+    def forward(self, emb: Dict[str, torch.Tensor]) -> torch.Tensor:
+        sequence = emb[self._s]
+        offsets = emb.get(self._s + "_offsets")
+        if offsets is not None:
+            return self._jagged(sequence, offsets)
+        if self._max_seq_length > 0:
+            sequence = sequence[:, : self._max_seq_length, :]
+        Q, K, V = self._query(sequence), self._key(sequence), self._value(sequence)
+        seq_len = emb[self._l]
+        attn_mask = _attention_mask(sequence, self._num_heads, seq_len)
+        attn_output, _ = self._multihead_attn(Q, K, V, attn_mask=attn_mask)
+        attn_output = torch.nan_to_num(attn_output, nan=0.0)
+        return attn_output.sum(dim=1) / torch.clamp_min(seq_len, 1).unsqueeze(1)
+
+    def _jagged(self, sequence: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
+        mha, E, H = self._multihead_attn, self._multihead_attn_dim, self._num_heads
+        w, b = mha.in_proj_weight, mha.in_proj_bias
+        q = F.linear(self._query(sequence), w[:E], b[:E])
+        k = F.linear(self._key(sequence), w[E:2 * E], b[E:2 * E])
+        v = F.linear(self._value(sequence), w[2 * E:], b[2 * E:])
+        if Fn.self_attn_pool_usable(q, H, self._dropout, self.training):
+            pooled = Fn.self_attn_pool(q, k, v, offsets, H, self._max_seq_length)
+        else:
+            pooled = Fn.torch_self_attn_pool(q, k, v, offsets, H, self._max_seq_length, self._dropout, self.training)
+        lens = offsets[1:] - offsets[:-1]
+        kept = torch.clamp_max(lens, self._max_seq_length) if self._max_seq_length > 0 else lens
+        out = F.linear(pooled, mha.out_proj.weight) + kept.unsqueeze(1).to(pooled.dtype) * mha.out_proj.bias
+        return out / torch.clamp_min(lens, 1).unsqueeze(1).to(out.dtype)
+
+
+# the encoder kinds a DEEP group's sequence_encoders may hold (simple_attention stays outside the hot-path scope)
+_SEQ_ENCODERS = {"din_encoder": DINEncoder, "pooling_encoder": PoolingEncoder,
+                 "self_attention_encoder": SelfAttentionEncoder, "multi_window_din_encoder": MultiWindowDINEncoder}
+
+
 def _create_seq_encoder(seq_encoder_config: Message, group_total_dim: Dict[str, int]) -> nn.Module:
-    """tzrec/modules/sequence.py:370-394 for the encoder kinds built here (din_encoder): the encoder of a DEEP group's
-    sequence group, with query_dim / sequence_dim from `<input>.query` / `<input>.sequence`."""
+    """tzrec/modules/sequence.py:370-394 for the encoder kinds built here (din_encoder, pooling_encoder,
+    self_attention_encoder, multi_window_din_encoder): the encoder of a DEEP group's sequence group, with query_dim /
+    sequence_dim from `<input>.query` / `<input>.sequence`."""
     kind = seq_encoder_config.WhichOneof("seq_module")
-    if kind != "din_encoder":
-        raise NotImplementedError(f"sequence encoder {kind} is outside the hot-path scope (din_encoder only)")
-    cfg = seq_encoder_config.din_encoder
+    if kind not in _SEQ_ENCODERS:
+        raise NotImplementedError(f"sequence encoder {kind} is outside the hot-path scope (din_encoder, "
+                                  "pooling_encoder, self_attention_encoder and multi_window_din_encoder only)")
+    cfg = getattr(seq_encoder_config, kind)
     kw = config_to_kwargs(cfg)
     kw.pop("name", None)
-    return DINEncoder(sequence_dim=group_total_dim[f"{cfg.input}.sequence"],
-                      query_dim=group_total_dim[f"{cfg.input}.query"], **kw)
+    return _SEQ_ENCODERS[kind](sequence_dim=group_total_dim[f"{cfg.input}.sequence"],
+                               query_dim=group_total_dim[f"{cfg.input}.query"], **kw)
 
 
 # --------------------------------------------------------------------------------------------------------
@@ -325,12 +435,12 @@ class RankModel(nn.Module):
                       wide_init_fn=self._model_config.wide_init_fn if self._model_config.HasField("wide_init_fn") else None)
         self.embedding_group = EmbeddingGroup(self._features, list(self._base_model_config.feature_groups),
                                               device=self._device, seq_encoder_factory=_create_seq_encoder, **kw)
-        # DIN encoders of DEEP groups read their sequence rows jagged, as MultiTowerDIN's attention towers do
+        # the sequence encoders of DEEP groups read their sequence rows jagged, as MultiTowerDIN's attention towers do
         # (TZK_DIN_JAGGED=0 keeps the padded [B, T, D] form)
-        din_inputs = [enc.din_encoder.input for fg in self._base_model_config.feature_groups
-                      for enc in fg.sequence_encoders if enc.WhichOneof("seq_module") == "din_encoder"]
-        if din_inputs and os.environ.get("TZK_DIN_JAGGED", "1") != "0":
-            self.embedding_group.set_jagged_for_attention(din_inputs)
+        seq_inputs = [getattr(enc, enc.WhichOneof("seq_module")).input for fg in self._base_model_config.feature_groups
+                      for enc in fg.sequence_encoders]
+        if seq_inputs and os.environ.get("TZK_DIN_JAGGED", "1") != "0":
+            self.embedding_group.set_jagged_for_attention(list(dict.fromkeys(seq_inputs)))
 
     def build_input(self, batch: Batch) -> Dict[str, torch.Tensor]:
         """rank_model.py:114-131."""
